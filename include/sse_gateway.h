@@ -22,6 +22,10 @@ extern "C" {
 typedef struct ssegw ssegw;
 
 ssegw *ssegw_new(int device, uint32_t max_conns, uint32_t bytes_per_batch, int *status);
+/* ssegw_new with a line pool (sse_init_ex): lines longer than the 64 KiB carry slot of the worst-case config continue in the
+ * pool instead of failing their stream. Elements can then be longer than a receive buffer: ssegw_recv and friends return
+ * SSE_ERR_ARG with *n set to the element's length and keep it queued, so the caller can grow the buffer and call again. */
+ssegw *ssegw_new_ex(int device, uint32_t max_conns, uint32_t bytes_per_batch, const sse_line_pool *pool, int *status);
 void   ssegw_free(ssegw *g);
 int    ssegw_stream_chat_completions(ssegw *g, uint8_t mode);
 size_t ssegw_upstream_write(ssegw *g, int stream, const uint8_t *data, size_t n);

@@ -65,7 +65,7 @@ typedef struct {
     uint32_t max_usages;       /* usage objects per batch */
     uint32_t text_arena_bytes; /* decoded (unescaped) strings per batch */
     uint32_t max_runs;         /* extra result runs per batch (segments with > 64 lines) */
-    uint32_t carry_slot_bytes; /* per-connection held-back tail capacity == longest supported line */
+    uint32_t carry_slot_bytes; /* per-connection held-back tail capacity == longest line without a line pool (sse_init_ex) */
     uint32_t n_slots;          /* batches in flight (pipeline depth), 1..8 */
     uint32_t flags;            /* SSE_FLAG_* */
 } sse_config;
@@ -147,7 +147,8 @@ typedef struct { int64_t prompt_tokens, completion_tokens, total_tokens; } sse_u
 /* sse_seg_result.flags */
 #define SSE_SEG_TERMINATED   0x01u  /* a chunk with SSE_F_TERMINATES was emitted in this batch */
 #define SSE_SEG_FINISHED     0x02u  /* connection had terminated earlier: bytes ignored (never read by the reference) */
-#define SSE_SEG_LINE_TOO_LONG 0x04u /* a line exceeded carry_slot_bytes: stream failed, connection dead until reset */
+#define SSE_SEG_LINE_TOO_LONG 0x04u /* a line exceeded carry_slot_bytes and could not continue in the line pool (longer than
+                                       max_line_bytes, or no free page): stream failed, connection dead until reset */
 #define SSE_SEG_DEAD         0x08u  /* connection is in the failed state */
 
 /* A run: contiguous frames/recs produced by up to 64 consecutive lines of one segment. */
@@ -160,7 +161,7 @@ typedef struct {
 /* Per-segment result, same index as the submitted sse_seg. 32 bytes. */
 typedef struct {
     sse_run  run;          /* first run inline */
-    uint32_t carry_len;    /* bytes held back (unterminated tail), carried to the next batch */
+    uint32_t carry_len;    /* bytes held back (unterminated tail), carried to the next batch: carry slot plus line pool */
     uint32_t flags;        /* SSE_SEG_* */
     uint32_t reserved;
 } sse_seg_result;
@@ -212,6 +213,28 @@ void sse_default_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_per_
  * memory grows to ~30x the batch size, meant for small batcher arenas (sse_gateway.h uses it). With sse_default_config the
  * capacities fit realistic SSE traffic and a pathological batch fails as a whole with SSE_ERR_OVERFLOW. */
 void sse_worst_case_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_per_batch);
+
+/* Line pool: pages in HBM shared by all connections of a context. A line that outgrows its connection's carry slot
+ * continues in pool pages instead of failing the stream; its pages return to the pool when the line completes, when the
+ * connection dies or finishes, and on sse_reset_conn / sse_reset_all. A connection fails (SSE_SEG_LINE_TOO_LONG |
+ * SSE_SEG_DEAD) only when its line would exceed max_line_bytes or no page is free. A completed pooled line is always
+ * materialised in the out arena (never a zero-copy span). Not available with SSE_FLAG_KERNEL_FUSED. */
+#define SSE_MAX_LINE_BYTES 16777215u   /* decode work items carry a 24-bit payload length */
+typedef struct {
+    uint32_t struct_size;      /* sizeof(sse_line_pool) */
+    uint32_t page_bytes;       /* pool page size, multiple of 16; 0 = library default (64 KiB) */
+    uint32_t pool_pages;       /* pages shared by all connections for lines longer than carry_slot_bytes; 0 = no pool */
+    uint32_t max_line_bytes;   /* longest line ONE connection may assemble (carry_slot_bytes .. SSE_MAX_LINE_BYTES): no upstream can take the whole pool */
+} sse_line_pool;
+/* sse_init with a line pool (pool NULL == sse_init). The per-batch result capacities grow as sse_line_pool_config says. */
+int  sse_init_ex(int device, const sse_config *cfg, const sse_line_pool *pool, sse_ctx **out);
+/* The capacities sse_init_ex will actually allocate: up to pool_pages * page_bytes bytes of pooled lines can complete in one
+ * batch, so out, frames, recs, tcs, usages, text and runs each grow by that many bytes at the ratio to in_arena_bytes the
+ * config already has (a worst-case config stays overflow-free, a default one stays sized for realistic traffic). A NULL or
+ * zero-page pool leaves cfg unchanged. */
+void sse_line_pool_config(sse_config *cfg, const sse_line_pool *pool);
+/* Pages held by connections now and the most ever held at once; ordered after already submitted batches and resets. */
+int  sse_line_pool_stats(sse_ctx *ctx, uint32_t *pages_in_use, uint32_t *pages_high_water);
 
 /* pipeline: acquire -> fill -> submit -> collect -> release (one slot = one batch in flight) */
 int sse_acquire(sse_ctx *ctx, int *slot, sse_batch *batch);

@@ -10,6 +10,7 @@ SSE_OK, SSE_ERR_NO_DEVICE, SSE_ERR_CUDA, SSE_ERR_ARG, SSE_ERR_BUSY, SSE_ERR_OVER
 MODE_P, MODE_R, MODE_PARSE = 0, 1, 2
 FLAG_KERNEL_FUSED, FLAG_COPY_OUT, FLAG_TEMPLATES = 4, 8, 16
 NONE = 0xFFFFFFFF
+MAX_LINE_BYTES = 16777215   # SSE_MAX_LINE_BYTES: decode work items carry a 24-bit payload length
 
 F_JSON_OK, F_HAS_USAGE, F_TC_NONNIL, F_TC_VALID, F_CONTENT_TEXT = 0x1, 0x2, 0x4, 0x8, 0x10
 F_DONE_LINE, F_DONE_EXACT, F_TERMINATES, F_DEPTH_LIMIT, F_TOO_LONG = 0x20, 0x40, 0x80, 0x100, 0x200
@@ -23,6 +24,10 @@ class Config(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in (
         "struct_size", "max_conns", "max_segs", "in_arena_bytes", "out_arena_bytes", "max_frames", "max_recs",
         "max_tcs", "max_usages", "text_arena_bytes", "max_runs", "carry_slot_bytes", "n_slots", "flags")]
+
+
+class LinePool(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("struct_size", "page_bytes", "pool_pages", "max_line_bytes")]
 
 
 class Seg(C.Structure):
@@ -86,7 +91,7 @@ class ToolCall(C.Structure):
 assert C.sizeof(Seg) == 16 and C.sizeof(Rec) == 32 and C.sizeof(Tc) == 48 and C.sizeof(SegResult) == 32
 
 EXPORTS = [
-    "sse_init", "sse_destroy", "sse_strerror", "sse_last_cuda_error", "sse_abi_version", "sse_default_config", "sse_worst_case_config",
+    "sse_init", "sse_init_ex", "sse_line_pool_config", "sse_line_pool_stats", "sse_destroy", "sse_strerror", "sse_last_cuda_error", "sse_abi_version", "sse_default_config", "sse_worst_case_config",
     "sse_acquire", "sse_submit", "sse_collect", "sse_release", "sse_reset_conn", "sse_reset_all",
     "sse_upload", "sse_launch", "sse_download", "sse_launch_count", "sse_at",
     "sse_agent_new", "sse_agent_free", "sse_agent_reset", "sse_agent_feed", "sse_agent_content",
@@ -114,6 +119,10 @@ def load(build_if_missing: bool = True):
     L = C.CDLL(path)
     vp, u32, i32 = C.c_void_p, C.c_uint32, C.c_int
     L.sse_init.argtypes = [i32, C.POINTER(Config), C.POINTER(vp)]
+    L.sse_init_ex.argtypes = [i32, C.POINTER(Config), C.POINTER(LinePool), C.POINTER(vp)]
+    L.sse_line_pool_config.argtypes = [C.POINTER(Config), C.POINTER(LinePool)]
+    L.sse_line_pool_config.restype = None
+    L.sse_line_pool_stats.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
     L.sse_destroy.argtypes = [vp]
     L.sse_destroy.restype = None
     L.sse_strerror.argtypes = [i32]

@@ -547,8 +547,11 @@ __device__ __noinline__ void append_run(const KParams &P, RunChain &rc, uint32_t
 // A line that never fit the window, assembled in the connection's carry slot (HBM): classified and emitted straight from
 // global memory. seg >= 0 (split pipeline): its payload becomes a work item like any other line's -- the decode kernel
 // reads payloads from the arenas, so a line of any length up to carry_slot_bytes is decoded. seg < 0 (first-generation
-// kernel): the payload is not decoded (SSE_F_TOO_LONG).
-__device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, const uint8_t *line, int L, uint32_t mode, int seg = -1) {
+// kernel): the payload is not decoded (SSE_F_TOO_LONG). at != SSE_NONE: the line already stands in the out arena at offset
+// `at` (a pooled line gathered there, one spare byte after it) and is emitted in place: frame, payload and the swallowed
+// line's materialised payload are spans of it, nothing is copied.
+__device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, const uint8_t *line, int L, uint32_t mode, int seg = -1,
+                                               uint32_t at = SSE_NONE) {
     const uint32_t lane = lane_id();
     int a = 0, b = L;           // frame source [a, b) ; R: trimmed
     bool emit = true, done = false, parse = false, pref = false;
@@ -572,24 +575,29 @@ __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, c
     const bool exact = item && done && pref && pe - ps == 6;          // `data: [DONE]` cannot be this long; kept for symmetry
     const uint32_t extra = (item && !emit) ? (uint32_t)(pe - ps) : 0u;   // a swallowed line's payload is materialised for the decoder
     uint32_t nf = emit ? 1u : 0u, nr = parse ? 1u : 0u;
+    const bool in_place = at != SSE_NONE;
     uint32_t ob = 0, fb = 0, rb = 0, qb = 0;
     if (lane == 0) {
-        if (nf || extra) ob = atomicAdd(&P.ctr->out_bytes, ((uint32_t)flen + extra + 15u) & ~15u);
+        if ((nf || extra) && !in_place) ob = atomicAdd(&P.ctr->out_bytes, ((uint32_t)flen + extra + 15u) & ~15u);
         if (nf) fb = atomicAdd(&P.ctr->n_frames, 1u);
         if (nr) rb = atomicAdd(&P.ctr->n_recs, 1u);
         if (item && !exact) qb = atomicAdd(&P.ctr->n_items, 1u);
     }
     ob = __shfl_sync(FULL, ob, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0); qb = __shfl_sync(FULL, qb, 0);
-    bool ovf = ((nf || extra) && (ob + (uint32_t)flen + extra + 16u > P.cap_out)) || (nf && fb >= P.cap_frames) || (nr && rb >= P.cap_recs) ||
-               (item && !exact && qb >= P.cap_items);
+    bool ovf = (!in_place && (nf || extra) && (ob + (uint32_t)flen + extra + 16u > P.cap_out)) || (nf && fb >= P.cap_frames) ||
+               (nr && rb >= P.cap_recs) || (item && !exact && qb >= P.cap_items);
     if (ovf) { if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT); return false; }
+    // frame and payload offsets in the out arena
+    const uint32_t fo = in_place ? at + (uint32_t)((mode & SSE_MODE_R) ? a : 0) : ob;
+    const uint32_t po = in_place ? at + (uint32_t)ps : (emit ? ob + (uint32_t)(ps - ((mode & SSE_MODE_R) ? a : 0)) : ob);
     if (emit) {
         if (mode & SSE_MODE_R) {
-            copy_g2g_bytes(P.out + ob, line + a, b - a);
-            if (lane < 2) P.out[ob + (uint32_t)(b - a) + lane] = '\n';
-        } else copy_g2g_bytes(P.out + ob, line, L);
-        if (lane == 0) { sse_frame f; f.off = ob; f.len = (uint32_t)flen; P.frames[fb] = f; }
-    } else if (extra) copy_g2g_bytes(P.out + ob, line + ps, pe - ps);
+            if (!in_place) copy_g2g_bytes(P.out + fo, line + a, b - a);
+            __syncwarp();   // in place: every lane has read the line's trimmed end before it is overwritten
+            if (lane < 2) P.out[fo + (uint32_t)(b - a) + lane] = '\n';
+        } else if (!in_place) copy_g2g_bytes(P.out + fo, line, L);
+        if (lane == 0) { sse_frame f; f.off = fo; f.len = (uint32_t)flen; P.frames[fb] = f; }
+    } else if (extra && !in_place) copy_g2g_bytes(P.out + ob, line + ps, pe - ps);
     if (parse && lane == 0) {
         sse_rec r;
         r.frame = emit ? fb : SSE_NONE;
@@ -599,13 +607,146 @@ __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, c
         P.recs[rb] = r;
         if (item && !exact) {
             uint4 it;
-            it.x = emit ? ob + (uint32_t)(ps - ((mode & SSE_MODE_R) ? a : 0)) : ob;
+            it.x = po;
             it.y = (uint32_t)(pe - ps) | (done ? 0x40000000u : ((mode & SSE_MODE_R) ? 0x80000000u : 0u));
             it.z = rb; it.w = (uint32_t)seg;
             P.items[qb] = it;
         }
     }
     append_run(P, rc, fb, nf, rb, nr);
+    return true;
+}
+
+// ---------------------------------------------------------------- line pool (lines longer than the carry slot)
+// One lane at a time moves pages, under a spin lock: a page moves once per page_bytes of a long line, so the lock is cold. Pool
+// metadata is read and written volatile (L2), because the lanes that move pages run on every SM.
+__device__ __forceinline__ void pool_lock(PoolHdr *h) {
+    uint32_t ns = 32;      // exponential back-off: hundreds of long lines may want a page at once
+    while (atomicCAS(&h->lock, 0u, 1u) != 0u) { __nanosleep(ns); if (ns < 2048u) ns <<= 1; }
+    __threadfence();
+}
+__device__ __forceinline__ void pool_unlock(PoolHdr *h) {
+    __threadfence();
+    atomicExch(&h->lock, 0u);
+}
+__device__ __forceinline__ uint32_t pool_next_page(const KParams &P, uint32_t pg) { return ((volatile uint32_t *)P.pool_next)[pg]; }
+
+// Every page of conn's chain back on the free stack (caller holds the lock).
+__device__ __noinline__ void pool_release_locked(const KParams &P, uint32_t conn) {
+    volatile PoolHdr *h = P.pool_hdr;
+    volatile PoolChain *c = P.pool_chain + conn;
+    volatile uint32_t *stk = P.pool_stack;
+    uint32_t n = h->n_free, pg = c->first;
+    const uint32_t k = c->n_pages;
+    for (uint32_t i = 0; i < k; i++) { stk[n++] = pg; pg = pool_next_page(P, pg); }
+    h->n_free = n;
+    c->first = c->last = SSE_NONE; c->n_pages = 0;
+}
+
+// conn's chain grows from `have` to `want` > have pages, all or none (caller holds the lock). Returns the page the next bytes
+// go to (the old last page when it has room: from_last), SSE_NONE when too few pages are free.
+__device__ __noinline__ uint32_t pool_grow_locked(const KParams &P, uint32_t conn, uint32_t have, uint32_t want, bool from_last) {
+    volatile PoolHdr *h = P.pool_hdr;
+    volatile PoolChain *c = P.pool_chain + conn;
+    volatile uint32_t *stk = P.pool_stack, *nxt = P.pool_next;
+    uint32_t n = h->n_free;
+    if (want - have > n) return SSE_NONE;
+    uint32_t first = have ? c->first : SSE_NONE, last = have ? c->last : SSE_NONE;
+    uint32_t start = from_last ? last : SSE_NONE;
+    for (uint32_t k = have; k < want; k++) {
+        const uint32_t p = stk[--n];
+        if (last == SSE_NONE) first = p; else nxt[last] = p;
+        if (start == SSE_NONE) start = p;
+        last = p;
+    }
+    h->n_free = n;
+    if (P.pool_pages - n > h->high_water) h->high_water = P.pool_pages - n;
+    c->first = first; c->last = last; c->n_pages = want;
+    return start;
+}
+
+// Cold path of a line that outgrows the carry slot. The held-back line (clen bytes: in the slot while clen <= carry_slot,
+// else all of them in pool pages) grows by `take` bytes of the warp's window at src. Takes the pages the longer line needs,
+// moves the slot bytes to the first page when the line leaves the slot, appends. Fails, and returns the connection's pages,
+// when the line would exceed max_line or too few pages are free (a pool of zero pages never has a free page).
+__device__ __noinline__ bool pool_append(const KParams &P, uint32_t conn, const uint8_t *slot, int clen, const uint8_t *src, int take) {
+    if (take == 0) return true;     // nothing to hold (an empty segment): the line and its chain stay as they are
+    const uint32_t lane = lane_id(), PB = P.page_bytes;
+    const bool leave_slot = clen <= (int)P.carry_slot;
+    const uint32_t old_len = leave_slot ? 0u : (uint32_t)clen, new_len = (uint32_t)clen + (uint32_t)take;
+    uint32_t pg = SSE_NONE;
+    if (lane == 0) {
+        const bool fits = new_len <= P.max_line;        // (max_line == carry_slot without a pool)
+        const uint32_t have = (old_len + PB - 1) / PB, want = (new_len + PB - 1) / PB;
+        if (fits && have == want) {
+            // the bytes fit the last page (take > 0 and no new page: the line is pooled and its last page has room). Only
+            // this warp changes the connection's chain during the launch, so it is read without the lock
+            pg = ((volatile PoolChain *)P.pool_chain)[conn].last;
+        } else if (fits || !leave_slot) {
+            pool_lock(P.pool_hdr);
+            if (fits) pg = pool_grow_locked(P, conn, have, want, (old_len % PB) != 0);
+            if (pg == SSE_NONE) pool_release_locked(P, conn);
+            pool_unlock(P.pool_hdr);
+        }
+    }
+    pg = __shfl_sync(FULL, pg, 0);
+    __syncwarp();
+    if (pg == SSE_NONE) return false;
+    uint32_t off = old_len % PB;
+    if (leave_slot) {        // slot -> pages: both 16-byte aligned, whole vectors (the slot is a multiple of 16 bytes long)
+        for (uint32_t d = 0; d < (uint32_t)clen;) {
+            if (off == PB) { pg = pool_next_page(P, pg); off = 0; }
+            const uint32_t n = min(PB - off, (uint32_t)clen - d);
+            const uint4 *s = reinterpret_cast<const uint4 *>(slot + d);
+            uint4 *o = reinterpret_cast<uint4 *>(P.pool + (size_t)pg * PB);
+            for (uint32_t i = lane; i < (n + 15u) >> 4; i += 32) o[i] = s[i];
+            d += n; off += n;
+        }
+        __syncwarp();        // the vector tail past clen is overwritten below
+    }
+    for (uint32_t d = 0; d < (uint32_t)take;) {
+        if (off == PB) { pg = pool_next_page(P, pg); off = 0; }
+        const uint32_t n = min(PB - off, (uint32_t)take - d);
+        copy_s2g_vec(P.pool + (size_t)pg * PB + off, src + d, (int)n);
+        d += n; off += n;
+    }
+    __syncwarp();
+    return true;
+}
+
+// A pooled line is complete (its last byte, the '\n', was appended): gathered from its pages into the out arena with 16-byte
+// copies, its pages returned to the pool, then classified and emitted in place by process_long_line.
+__device__ __noinline__ bool pool_long_line(const KParams &P, RunChain &rc, uint32_t conn, int L, uint32_t mode, int seg) {
+    const uint32_t lane = lane_id(), PB = P.page_bytes;
+    const uint32_t bytes = ((uint32_t)L + 1u + 15u) & ~15u;    // + 1: mode R's frame ends in a second '\n'
+    uint32_t ob = 0, pg = 0;
+    if (lane == 0) { ob = atomicAdd(&P.ctr->out_bytes, bytes); pg = ((volatile PoolChain *)P.pool_chain)[conn].first; }
+    ob = __shfl_sync(FULL, ob, 0); pg = __shfl_sync(FULL, pg, 0);
+    // on overflow the batch is discarded and the chain stays with the connection: its state still describes the line
+    if (ob + bytes + 16u > P.cap_out) { if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT); return false; }
+    for (uint32_t d = 0; d < (uint32_t)L; d += PB) {
+        if (d) pg = pool_next_page(P, pg);
+        const uint32_t nv = (min(PB, (uint32_t)L - d) + 15u) >> 4;
+        const uint4 *s = reinterpret_cast<const uint4 *>(P.pool + (size_t)pg * PB);
+        uint4 *o = reinterpret_cast<uint4 *>(P.out + ob + d);
+        for (uint32_t i = lane; i < nv; i += 32) o[i] = __ldcg(s + i);
+    }
+    __syncwarp();
+    if (lane == 0) { pool_lock(P.pool_hdr); pool_release_locked(P, conn); pool_unlock(P.pool_hdr); }
+    __syncwarp();
+    return process_long_line(P, rc, P.out + ob, L, mode, seg, ob);
+}
+
+// A line assembled outside the window is complete (clen bytes, '\n' included): in the carry slot, or in the pool.
+__device__ __noinline__ bool complete_long_line(const KParams &P, RunChain &rc, uint32_t conn, const uint8_t *slot, int clen, uint32_t mode, int seg) {
+    return clen > (int)P.carry_slot ? pool_long_line(P, rc, conn, clen, mode, seg) : process_long_line(P, rc, slot, clen, mode, seg);
+}
+
+// Holds `take` bytes of the window back as the continuation of the connection's unterminated line: in the carry slot while
+// the line fits it, else in line-pool pages. false: the line cannot be held (longer than max_line, or no free page).
+__device__ __forceinline__ bool hold_back(const KParams &P, uint32_t conn, uint8_t *slot, int clen, const uint8_t *src, int take) {
+    if (clen + take > (int)P.carry_slot) return pool_append(P, conn, slot, clen, src, take);
+    copy_s2g_bytes(slot + clen, src, take);
     return true;
 }
 

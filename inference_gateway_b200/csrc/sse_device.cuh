@@ -8,17 +8,33 @@
 //                                      ReadBytes would keep these bytes inside bufio.Reader)
 //   out, frames, recs, tcs, usages, text, runs, seg_results   per-batch results (see include/sse_gpu.h)
 //   ctr     Counters                   bump allocators + work ticket, zeroed per launch
+// line pool (sse_init_ex, optional; one per context):
+//   pool        u8[pool_pages*page_bytes]  pages holding lines longer than the carry slot, page k = bytes [k*page_bytes, ...)
+//                                          of the line in chain order
+//   pool_hdr    PoolHdr                    lock + free-stack height + high-water mark
+//   pool_stack  u32[pool_pages]            free pages: pool_stack[0 .. n_free)
+//   pool_next   u32[pool_pages]            next page of the same chain
+//   pool_chain  PoolChain[max_conns]       per connection: first / last page, pages held (0: none)
 #pragma once
 #include <cstddef>
 #include <stdint.h>
 #include "../../include/sse_gpu.h"
 
 struct ConnState {
-    uint32_t carry_len;
+    uint32_t carry_len;    // bytes of the held-back line: in the carry slot while <= carry_slot, else all of them in pool pages
     uint32_t flags;
 };
+struct PoolHdr {
+    uint32_t lock;         // taken by one lane around every allocation / release (pages move rarely: one per page_bytes of a long line)
+    uint32_t n_free;
+    uint32_t high_water;   // most pages ever held at once
+    uint32_t pad;
+};
+struct PoolChain {
+    uint32_t first, last, n_pages, pad;
+};
 #define CONN_FINISHED 1u   // mode R: terminating chunk seen (agent.go:235-242); later bytes are never read
-#define CONN_DEAD     2u   // line exceeded carry_slot_bytes
+#define CONN_DEAD     2u   // line exceeded carry_slot_bytes and could not continue in the line pool
 #define CONN_LONG     4u   // a line longer than the smem window is being assembled in the carry slot
 
 #ifndef SSE_LEN_SHIFT
@@ -80,6 +96,11 @@ struct KParams {
     // fused pipeline (plan -> fused tile kernel)
     uint2 *tiles;            uint32_t cap_tiles;   // {first segment, segment count} per tile
     uint32_t *tcache;                              // skeleton templates kept between launches: [0] words used, [1..256] buckets, store
+    // line pool (pool_pages == 0: none; max_line == carry_slot then, and every line longer than the slot fails its connection)
+    uint8_t *pool;           PoolHdr *pool_hdr;
+    uint32_t *pool_stack;    uint32_t *pool_next;
+    PoolChain *pool_chain;
+    uint32_t page_bytes, pool_pages, max_line;
 };
 
 #ifdef __CUDACC__
@@ -92,6 +113,7 @@ __device__ __forceinline__ void sse_overflow(Counters *c, uint32_t which) {
 // launch wrappers (sse_kernel.cu)
 int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count);           // split pipeline, stage 1
 int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device);  // split pipeline, stages 2+3
+int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream);              // line pool: reset one connection (SSE_NONE: all)
 int sse_v2_prepare(int device);                                                        // builds + uploads the automaton tables
 int sse_fused_prepare(int device);                                                     // fused pipeline: tables + kernel attributes
 int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device);        // plan kernel + fused tile kernel

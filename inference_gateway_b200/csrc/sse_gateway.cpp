@@ -53,11 +53,15 @@ struct ssegw {
 extern "C" {
 
 ssegw *ssegw_new(int device, uint32_t max_conns, uint32_t bytes_per_batch, int *status) {
+    return ssegw_new_ex(device, max_conns, bytes_per_batch, nullptr, status);
+}
+
+ssegw *ssegw_new_ex(int device, uint32_t max_conns, uint32_t bytes_per_batch, const sse_line_pool *pool, int *status) {
     ssegw *g = new ssegw();
     // worst-case result capacities: whatever the upstreams send (a flood of one-byte lines, of empty tool-call elements ...), a
-    // batch cannot overflow, so one connection can never fail the batch of the others
+    // batch cannot overflow, so one connection can never fail the batch of the others; a line pool grows them by its size
     sse_worst_case_config(&g->cfg, max_conns, bytes_per_batch);
-    int rc = sse_init(device, &g->cfg, &g->ctx);
+    int rc = sse_init_ex(device, &g->cfg, pool, &g->ctx);
     if (status) *status = rc;
     if (rc != SSE_OK) { delete g; return nullptr; }   // no CUDA device: error, never a CPU path
     g->streams.resize(max_conns);
@@ -191,7 +195,7 @@ int ssegw_proxy_step(ssegw *g, int id, uint8_t *buf, size_t cap, size_t *n) {
 int ssegw_agent_recv(ssegw *g, int id, uint8_t *buf, size_t cap, size_t *n) {
     Stream &s = g->streams[(size_t)id];
     int rc = ssegw_recv(g, id, buf, cap, n);
-    if (rc == 1) return 1;
+    if (rc == 1 || rc == SSE_ERR_ARG) return rc;      // SSE_ERR_ARG: the next element is longer than cap (*n), still queued
     const bool over = s.terminated || rc == -1;
     if (over && !s.done_sent) {
         static const char done[] = "data: [DONE]\n\n";

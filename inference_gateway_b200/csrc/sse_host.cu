@@ -61,6 +61,10 @@ struct sse_ctx {
     ConnState *d_conns = nullptr;
     uint8_t *d_carry = nullptr;
     uint32_t *d_tcache = nullptr;        // fused kernel: skeleton templates kept between launches
+    sse_line_pool pool{};                // pool_pages == 0: no line pool
+    uint8_t *d_pool = nullptr; PoolHdr *d_pool_hdr = nullptr; uint32_t *d_pool_stack = nullptr, *d_pool_next = nullptr;
+    PoolChain *d_pool_chain = nullptr;
+    PoolHdr *h_pool_hdr = nullptr;       // pinned: sse_line_pool_stats
     cudaStream_t ctl_stream = nullptr;
     cudaEvent_t last_kernel = nullptr;   // completion of the most recently launched kernel
     bool have_last = false;
@@ -100,6 +104,19 @@ KParams make_params(sse_ctx *c, Slot &s, uint32_t n_segs) {
     p.items_sorted = s.d_items2; p.flags = c->cfg.flags;
     p.tiles = s.d_tiles; p.cap_tiles = c->cfg.max_segs + 64;
     p.tcache = (c->cfg.flags & SSE_FLAG_TEMPLATES) ? c->d_tcache : nullptr;
+    p.pool = c->d_pool; p.pool_hdr = c->d_pool_hdr; p.pool_stack = c->d_pool_stack; p.pool_next = c->d_pool_next;
+    p.pool_chain = c->d_pool_chain;
+    p.page_bytes = c->pool.page_bytes; p.pool_pages = c->pool.pool_pages;
+    p.max_line = c->pool.pool_pages ? c->pool.max_line_bytes : c->cfg.carry_slot_bytes;
+    return p;
+}
+
+// KParams for the line-pool maintenance kernel (no batch slot involved)
+KParams pool_params(sse_ctx *c) {
+    KParams p{};
+    p.max_conns = c->cfg.max_conns; p.conns = c->d_conns;
+    p.pool = c->d_pool; p.pool_hdr = c->d_pool_hdr; p.pool_stack = c->d_pool_stack; p.pool_next = c->d_pool_next;
+    p.pool_chain = c->d_pool_chain; p.page_bytes = c->pool.page_bytes; p.pool_pages = c->pool.pool_pages;
     return p;
 }
 
@@ -226,8 +243,35 @@ void sse_worst_case_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_p
     cfg->max_runs = clamp(in / 256 + 2ull * max_conns + 1024);
 }
 
-int sse_init(int device, const sse_config *cfg, sse_ctx **out) {
-    if (!cfg || !out || cfg->struct_size != sizeof(sse_config)) return SSE_ERR_ARG;
+void sse_line_pool_config(sse_config *cfg, const sse_line_pool *pool) {
+    if (!cfg || !pool || pool->struct_size != sizeof(sse_line_pool) || pool->pool_pages == 0 || cfg->in_arena_bytes == 0) return;
+    // every capacity grows by the pool's bytes at the ratio (capacity / input byte) the config already has
+    const unsigned __int128 extra = (unsigned __int128)pool->pool_pages * (pool->page_bytes ? pool->page_bytes : 65536u);
+    const uint64_t in = cfg->in_arena_bytes, cap = 0xF0000000ull;
+    auto grow = [&](uint32_t &x) {
+        const unsigned __int128 v = (unsigned __int128)x + ((unsigned __int128)x * extra + in - 1) / in;
+        x = (uint32_t)(v > cap ? cap : (uint64_t)v);
+    };
+    grow(cfg->out_arena_bytes); grow(cfg->max_frames); grow(cfg->max_recs); grow(cfg->max_tcs);
+    grow(cfg->max_usages); grow(cfg->text_arena_bytes); grow(cfg->max_runs);
+}
+
+int sse_init(int device, const sse_config *cfg, sse_ctx **out) { return sse_init_ex(device, cfg, nullptr, out); }
+
+int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_in, sse_ctx **out) {
+    if (!cfg_in || !out || cfg_in->struct_size != sizeof(sse_config)) return SSE_ERR_ARG;
+    sse_line_pool pool{};
+    pool.struct_size = sizeof pool;
+    sse_config grown = *cfg_in;
+    if (pool_in) {
+        if (pool_in->struct_size != sizeof(sse_line_pool) || (pool_in->page_bytes & 15u) || pool_in->pool_pages == SSE_NONE ||
+            pool_in->max_line_bytes > SSE_MAX_LINE_BYTES || pool_in->max_line_bytes < cfg_in->carry_slot_bytes ||
+            (cfg_in->flags & SSE_FLAG_KERNEL_FUSED)) return SSE_ERR_ARG;   // the tile kernel has no line pool
+        pool = *pool_in;
+        if (!pool.page_bytes) pool.page_bytes = 65536;
+        sse_line_pool_config(&grown, &pool);
+    }
+    const sse_config *cfg = &grown;
     if (cfg->n_slots < 1 || cfg->n_slots > 8 || cfg->max_conns == 0 || cfg->max_segs == 0 ||
         (cfg->in_arena_bytes & 15u) || cfg->carry_slot_bytes < 8192 + 16 || (cfg->carry_slot_bytes & 15u)) return SSE_ERR_ARG;
     if ((uint64_t)in_base_of(*cfg) + cfg->in_arena_bytes + 16 >= (1ull << 31)) return SSE_ERR_ARG;   // arena offsets are 31-bit
@@ -240,7 +284,7 @@ int sse_init(int device, const sse_config *cfg, sse_ctx **out) {
     CU(cudaSetDevice(device));
     sse_ctx *c = new (std::nothrow) sse_ctx();
     if (!c) return SSE_ERR_NOMEM;
-    c->device = device; c->cfg = *cfg;
+    c->device = device; c->cfg = *cfg; c->pool = pool;
     cudaDeviceProp prop;
     if (!cu_ok(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties")) { delete c; return SSE_ERR_CUDA; }
     c->sm_count = prop.multiProcessorCount;
@@ -260,6 +304,14 @@ int sse_init(int device, const sse_config *cfg, sse_ctx **out) {
     ok = ok && cu_ok(cudaMemset(c->d_conns, 0, (size_t)cfg->max_conns * sizeof(ConnState)), "cudaMemset");
     ok = ok && dalloc(c->d_tcache, sse_fused_tcache_words());
     ok = ok && cu_ok(cudaMemset(c->d_tcache, 0, (size_t)sse_fused_tcache_words() * sizeof(uint32_t)), "cudaMemset");
+    if (ok && pool.pool_pages) {
+        ok = ok && dalloc(c->d_pool, (size_t)pool.pool_pages * pool.page_bytes) && dalloc(c->d_pool_hdr, 1);
+        ok = ok && dalloc(c->d_pool_stack, pool.pool_pages) && dalloc(c->d_pool_next, pool.pool_pages);
+        ok = ok && dalloc(c->d_pool_chain, cfg->max_conns) && halloc(c->h_pool_hdr, 1);
+        ok = ok && cu_ok(cudaMemset(c->d_pool_hdr, 0, sizeof(PoolHdr)), "cudaMemset");
+        ok = ok && cu_ok((cudaError_t)sse_launch_pool_reset(pool_params(c), SSE_NONE, c->ctl_stream), "pool reset kernel");
+        ok = ok && cu_ok(cudaStreamSynchronize(c->ctl_stream), "cudaStreamSynchronize");
+    }
     c->slots.resize(cfg->n_slots);
     for (auto &s : c->slots) {
         if (!ok) break;
@@ -290,6 +342,8 @@ void sse_destroy(sse_ctx *c) {
     cudaDeviceSynchronize();
     for (auto &s : c->slots) free_slot(s);
     cudaFree(c->d_conns); cudaFree(c->d_carry); cudaFree(c->d_tcache);
+    cudaFree(c->d_pool); cudaFree(c->d_pool_hdr); cudaFree(c->d_pool_stack); cudaFree(c->d_pool_next); cudaFree(c->d_pool_chain);
+    cudaFreeHost(c->h_pool_hdr);
     if (c->ctl_stream) cudaStreamDestroy(c->ctl_stream);
     if (c->last_kernel) cudaEventDestroy(c->last_kernel);
     delete c;
@@ -350,7 +404,9 @@ int sse_reset_conn(sse_ctx *c, uint32_t conn) {
     if (!c || conn >= c->cfg.max_conns) return SSE_ERR_ARG;
     CU(cudaSetDevice(c->device));
     if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
-    CU(cudaMemsetAsync(c->d_conns + conn, 0, sizeof(ConnState), c->ctl_stream));
+    if (c->pool.pool_pages) {   // the connection's pages go back to the pool with its state
+        if (!cu_ok((cudaError_t)sse_launch_pool_reset(pool_params(c), conn, c->ctl_stream), "pool reset kernel")) return SSE_ERR_CUDA;
+    } else CU(cudaMemsetAsync(c->d_conns + conn, 0, sizeof(ConnState), c->ctl_stream));
     CU(cudaEventRecord(c->last_kernel, c->ctl_stream));   // later kernels are ordered after the reset
     c->have_last = true;
     return SSE_OK;
@@ -362,7 +418,21 @@ int sse_reset_all(sse_ctx *c, void *cuda_stream) {
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->ctl_stream;
     if (!cuda_stream && c->have_last) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
     CU(cudaMemsetAsync(c->d_conns, 0, (size_t)c->cfg.max_conns * sizeof(ConnState), st));
+    if (c->pool.pool_pages && !cu_ok((cudaError_t)sse_launch_pool_reset(pool_params(c), SSE_NONE, st), "pool reset kernel")) return SSE_ERR_CUDA;
     if (!cuda_stream) { CU(cudaEventRecord(c->last_kernel, st)); c->have_last = true; }
+    return SSE_OK;
+}
+
+int sse_line_pool_stats(sse_ctx *c, uint32_t *pages_in_use, uint32_t *pages_high_water) {
+    if (!c || !pages_in_use || !pages_high_water) return SSE_ERR_ARG;
+    *pages_in_use = *pages_high_water = 0;
+    if (!c->pool.pool_pages) return SSE_OK;
+    CU(cudaSetDevice(c->device));
+    if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
+    CU(cudaMemcpyAsync(c->h_pool_hdr, c->d_pool_hdr, sizeof(PoolHdr), cudaMemcpyDeviceToHost, c->ctl_stream));
+    CU(cudaStreamSynchronize(c->ctl_stream));
+    *pages_in_use = c->pool.pool_pages - c->h_pool_hdr->n_free;
+    *pages_high_water = c->h_pool_hdr->high_water;
     return SSE_OK;
 }
 

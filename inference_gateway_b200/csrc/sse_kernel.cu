@@ -7,7 +7,7 @@
 //   emit     frame table; a frame that stands in the input arena as it must be sent is a span of it (zero-copy), the others
 //            go through the warp-cooperative serializer into the out arena      (agent.go:195 / routes.go:613)
 //   items    a stub record + a 16-byte work item per line to decode (lines longer than the window are assembled in the carry
-//            slot and become work items too); sse_kernel2.cu sorts the items, decodes them (sse_decode_kernel) and resolves
+//            slot, past it in line-pool pages, and become work items too); sse_kernel2.cu sorts the items, decodes them (sse_decode_kernel) and resolves
 //            early termination (sse_finalize_kernel). The template parameter SPLIT is always true: the first-generation
 //            kernel that decoded in place (SPLIT = false) was removed in round 2.
 //   finish   carry update, per-segment result
@@ -118,8 +118,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     if (m) q = i0 + __ffs(m) - 1;
                 }
                 int take = (q < 0) ? (fill - base) : (q - base + 1);
-                if (clen + take > (int)P.carry_slot) { dead = true; break; }
-                copy_s2g_bytes(slot + clen, buf + base, take);
+                if (!hold_back(P, conn, slot, clen, buf + base, take)) { dead = true; break; }
                 clen += take;
                 __syncwarp();
                 if (q < 0) {
@@ -127,7 +126,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     if (consumed >= in_len) break;
                     continue;
                 }
-                if (!process_long_line(P, rc, slot, clen, mode, SPLIT ? (int)s : -1)) { overflow = true; break; }
+                if (!complete_long_line(P, rc, conn, slot, clen, mode, SPLIT ? (int)s : -1)) { overflow = true; break; }
                 __syncwarp();
                 in_long = false; clen = 0; pos = q + 1;
             }
@@ -370,6 +369,8 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
             if (terminated || overflow) break;
 
             const int tail = fill - pos;
+            // A tail is at most one window (BUF bytes) and sse_init refuses a carry slot shorter than BUF + 16, so the two slot
+            // checks below never fail: only a line assembled across windows (in_long, above) can outgrow the slot and go to the pool.
             if (consumed >= in_len) {          // segment exhausted: hold the unterminated tail back
                 if (tail > 0) {
                     if (tail > (int)P.carry_slot) { dead = true; break; }

@@ -1026,7 +1026,7 @@ __global__ void __launch_bounds__(SCATTER_TPB) sse_bucket_scatter_kernel(const K
 // ---------------------------------------------------------------- split pipeline, stage 3: early termination
 // One thread per segment: cut the segment's runs after the terminating chunk and mark the connection finished
 // (everything after it is never read by the reference, mcp/agent.go:235-242 and :169).
-__global__ void sse_finalize_kernel(const KParams P) {
+__global__ void sse_finalize_kernel(const __grid_constant__ KParams P) {
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= P.n_segs) return;
     const uint32_t trec = P.seg_term[s];
@@ -1047,8 +1047,30 @@ __global__ void sse_finalize_kernel(const KParams P) {
     r.flags |= SSE_SEG_TERMINATED;
     r.carry_len = 0;
     P.seg_results[s] = r;
+    const uint32_t conn = P.segs[s].conn;
+    // the produce stage kept reading after the terminating chunk and may have pooled a line that is never completed
+    if (P.pool_pages && ((volatile PoolChain *)P.pool_chain)[conn].n_pages) {
+        pool_lock(P.pool_hdr); pool_release_locked(P, conn); pool_unlock(P.pool_hdr);
+    }
     ConnState ns; ns.carry_len = 0; ns.flags = CONN_FINISHED;
-    P.conns[P.segs[s].conn] = ns;
+    P.conns[conn] = ns;
+}
+
+// Line pool reset: conn < max_conns returns that connection's pages and clears its state (sse_reset_conn); conn == SSE_NONE
+// rebuilds the free stack with every page free (sse_reset_all, context creation; the caller clears the connection states).
+__global__ void sse_pool_reset_kernel(const __grid_constant__ KParams P, uint32_t conn) {
+    if (conn != SSE_NONE) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            pool_lock(P.pool_hdr); pool_release_locked(P, conn); pool_unlock(P.pool_hdr);
+            ConnState z; z.carry_len = 0; z.flags = 0;
+            P.conns[conn] = z;
+        }
+        return;
+    }
+    const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
+    for (uint32_t i = tid; i < P.pool_pages; i += nt) P.pool_stack[i] = i;
+    for (uint32_t i = tid; i < P.max_conns; i += nt) { PoolChain z; z.first = z.last = SSE_NONE; z.n_pages = 0; z.pad = 0; P.pool_chain[i] = z; }
+    if (tid == 0) { P.pool_hdr->lock = 0; P.pool_hdr->n_free = P.pool_pages; }
 }
 
 DfaTables *g_tables_dev[16] = { nullptr };
@@ -1096,5 +1118,12 @@ int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int
     if (e != cudaSuccess) return (int)e;
     const int tpb = 256;
     sse_finalize_kernel<<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
+    return (int)cudaGetLastError();
+}
+
+int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream) {
+    const uint32_t n = p.pool_pages > p.max_conns ? p.pool_pages : p.max_conns;
+    const uint32_t grid = conn != SSE_NONE ? 1u : (n + 255u) / 256u < 1024u ? (n + 255u) / 256u : 1024u;
+    sse_pool_reset_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, conn);
     return (int)cudaGetLastError();
 }

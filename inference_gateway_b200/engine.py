@@ -89,17 +89,36 @@ class BatchResult:
         return self.text[off:off + length].tobytes() if in_text else self.at(off, length)
 
 
+def make_line_pool(pool_pages: int, page_bytes: int = 0, max_line_bytes: int = A.MAX_LINE_BYTES) -> A.LinePool:
+    """sse_line_pool: pool_pages pages of page_bytes (0: 64 KiB) shared by all connections for lines longer than the carry slot;
+    one connection's line may grow to max_line_bytes."""
+    return A.LinePool(C.sizeof(A.LinePool), page_bytes, pool_pages, max_line_bytes)
+
+
 class SseEngine:
-    def __init__(self, device: int = 0, max_conns: int = 1024, bytes_per_batch: int = 1 << 20, **overrides):
+    def __init__(self, device: int = 0, max_conns: int = 1024, bytes_per_batch: int = 1 << 20, line_pool: dict | None = None,
+                 **overrides):
+        """line_pool: keyword arguments of make_line_pool() (pool_pages, page_bytes, max_line_bytes), or None for no pool:
+        a line longer than carry_slot_bytes then fails its connection."""
         self.L = A.load()
         cfg = A.Config()
         self.L.sse_default_config(C.byref(cfg), max_conns, bytes_per_batch)
         for k, v in overrides.items():
             setattr(cfg, k, v)
-        self.cfg = cfg
         self._ctx = C.c_void_p()
-        A.check(self.L.sse_init(device, C.byref(cfg), C.byref(self._ctx)), "sse_init")
+        self.pool = make_line_pool(**line_pool) if line_pool is not None else None
+        pp = C.byref(self.pool) if self.pool is not None else None
+        A.check(self.L.sse_init_ex(device, C.byref(cfg), pp, C.byref(self._ctx)), "sse_init_ex")
+        if pp is not None:
+            self.L.sse_line_pool_config(C.byref(cfg), pp)   # the capacities the context allocated
+        self.cfg = cfg
         self.device = device
+
+    def pool_stats(self):
+        """(pages in use, high-water mark) of the line pool, after every batch submitted so far."""
+        used, hw = C.c_uint32(), C.c_uint32()
+        A.check(self.L.sse_line_pool_stats(self._ctx, C.byref(used), C.byref(hw)), "sse_line_pool_stats")
+        return used.value, hw.value
 
     def close(self):
         if self._ctx:

@@ -8,11 +8,16 @@ from . import _abi as A
 
 
 class Gateway:
-    def __init__(self, device: int = 0, max_conns: int = 256, bytes_per_batch: int = 1 << 20):
+    def __init__(self, device: int = 0, max_conns: int = 256, bytes_per_batch: int = 1 << 20, line_pool: dict | None = None):
+        """line_pool: keyword arguments of engine.make_line_pool() (pool_pages, page_bytes, max_line_bytes): lines longer than the
+        64 KiB carry slot continue in a shared device page pool instead of failing their stream."""
+        from .engine import make_line_pool
         self.L = L = A.load()
         vp, i32 = C.c_void_p, C.c_int
         L.ssegw_new.argtypes = [i32, C.c_uint32, C.c_uint32, C.POINTER(i32)]
         L.ssegw_new.restype = vp
+        L.ssegw_new_ex.argtypes = [i32, C.c_uint32, C.c_uint32, C.POINTER(A.LinePool), C.POINTER(i32)]
+        L.ssegw_new_ex.restype = vp
         L.ssegw_free.argtypes = [vp]
         L.ssegw_free.restype = None
         L.ssegw_stream_chat_completions.argtypes = [vp, C.c_uint8]
@@ -34,7 +39,11 @@ class Gateway:
         L.ssegw_agent_tool_calls.argtypes = [vp, i32, C.POINTER(A.ToolCall), C.c_size_t]
         L.ssegw_agent_tool_calls.restype = C.c_size_t
         st = i32()
-        self.g = L.ssegw_new(device, max_conns, bytes_per_batch, C.byref(st))
+        if line_pool is None:
+            self.g = L.ssegw_new(device, max_conns, bytes_per_batch, C.byref(st))
+        else:
+            self._pool = make_line_pool(**line_pool)
+            self.g = L.ssegw_new_ex(device, max_conns, bytes_per_batch, C.byref(self._pool), C.byref(st))
         if not self.g:
             raise A.SseError(st.value, "ssegw_new")
         self._buf = C.create_string_buffer(1 << 20)
@@ -65,6 +74,9 @@ class Gateway:
     def _recv(self, fn, sid):
         n = C.c_size_t()
         rc = fn(self.g, sid, self._buf, len(self._buf), C.byref(n))
+        if rc == A.SSE_ERR_ARG and n.value > len(self._buf):   # an element longer than the buffer (a pooled line): grow, retry
+            self._buf = C.create_string_buffer(n.value)
+            rc = fn(self.g, sid, self._buf, len(self._buf), C.byref(n))
         if rc == 1:
             return self._buf.raw[:n.value]
         if rc == 0:

@@ -15,7 +15,9 @@ import "C"
 import (
 	"errors"
 	"fmt"
+	"os"
 	"runtime"
+	"strconv"
 	"unsafe"
 )
 
@@ -39,16 +41,47 @@ func statusErr(where string, rc C.int) error {
 	return fmt.Errorf("%s: %s (%d)", where, msg, int(rc))
 }
 
+func envUint32(name string) uint32 {
+	v, err := strconv.ParseUint(os.Getenv(name), 10, 32)
+	if err != nil {
+		return 0
+	}
+	return uint32(v)
+}
+
 // NewContext fails when no CUDA device is present: there is no CPU fallback.
+//
+// GPU_LINE_POOL_PAGES > 0 gives the context a line pool of that many pages (GPU_LINE_POOL_PAGE_BYTES each, default 64 KiB),
+// shared by all connections: a line longer than the carry slot continues there instead of failing its stream, up to
+// GPU_LINE_POOL_MAX_LINE bytes per connection (default and ceiling SSE_MAX_LINE_BYTES, 16 MiB - 1).
 func NewContext(device int, maxConns, bytesPerBatch uint32) (*Context, error) {
 	runtime.LockOSThread()
 	var cfg C.sse_config
 	C.sse_default_config(&cfg, C.uint32_t(maxConns), C.uint32_t(bytesPerBatch))
 	var ctx *C.sse_ctx
+	if pages := envUint32("GPU_LINE_POOL_PAGES"); pages > 0 {
+		maxLine := envUint32("GPU_LINE_POOL_MAX_LINE")
+		if maxLine == 0 {
+			maxLine = uint32(C.SSE_MAX_LINE_BYTES)
+		}
+		pool := C.sse_line_pool{struct_size: C.uint32_t(unsafe.Sizeof(C.sse_line_pool{})),
+			page_bytes: C.uint32_t(envUint32("GPU_LINE_POOL_PAGE_BYTES")), pool_pages: C.uint32_t(pages), max_line_bytes: C.uint32_t(maxLine)}
+		if err := statusErr("sse_init_ex", C.sse_init_ex(C.int(device), &cfg, &pool, &ctx)); err != nil {
+			return nil, err
+		}
+		return &Context{c: ctx}, nil
+	}
 	if err := statusErr("sse_init", C.sse_init(C.int(device), &cfg, &ctx)); err != nil {
 		return nil, err
 	}
 	return &Context{c: ctx}, nil
+}
+
+// LinePoolStats returns the pages of the line pool held now and the most ever held at once.
+func (x *Context) LinePoolStats() (inUse, highWater uint32, err error) {
+	var u, h C.uint32_t
+	err = statusErr("sse_line_pool_stats", C.sse_line_pool_stats(x.c, &u, &h))
+	return uint32(u), uint32(h), err
 }
 
 func (x *Context) Close() { C.sse_destroy(x.c) }
