@@ -26,6 +26,11 @@ ssegw *ssegw_new(int device, uint32_t max_conns, uint32_t bytes_per_batch, int *
  * pool instead of failing their stream. Elements can then be longer than a receive buffer: ssegw_recv and friends return
  * SSE_ERR_ARG with *n set to the element's length and keep it queued, so the caller can grow the buffer and call again. */
 ssegw *ssegw_new_ex(int device, uint32_t max_conns, uint32_t bytes_per_batch, const sse_line_pool *pool, int *status);
+/* A gateway on any config (cfg->max_conns streams), e.g. sse_default_config with SSE_FLAG_DEFER: capacities sized for realistic
+ * traffic instead of the worst case, and a batch whose results do not fit them leaves the rest of a stream's bytes queued for the
+ * next tick (streams with deferred bytes are offered first) instead of failing every stream of the batch. ssegw_new and
+ * ssegw_new_ex use sse_worst_case_config. pool may be NULL. A bad config is refused (SSE_ERR_ARG) before a device is touched. */
+ssegw *ssegw_new_cfg(int device, const sse_config *cfg, const sse_line_pool *pool, int *status);
 void   ssegw_free(ssegw *g);
 int    ssegw_stream_chat_completions(ssegw *g, uint8_t mode);
 size_t ssegw_upstream_write(ssegw *g, int stream, const uint8_t *data, size_t n);

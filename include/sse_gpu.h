@@ -41,7 +41,7 @@ typedef enum {
     SSE_ERR_CUDA = -2,        /* a CUDA call failed; sse_last_cuda_error() has the text */
     SSE_ERR_ARG = -3,
     SSE_ERR_BUSY = -4,        /* no free batch slot / slot in wrong state */
-    SSE_ERR_OVERFLOW = -5,    /* a result arena was too small for this batch (config too small) */
+    SSE_ERR_OVERFLOW = -5,    /* a result arena was too small for this batch (config too small); never with SSE_FLAG_DEFER */
     SSE_ERR_NOMEM = -6,
     SSE_ERR_UNDECODED = -7    /* sse_agent_feed / sse_telemetry_feed: the segment holds a record flagged SSE_F_TOO_LONG or SSE_F_DEPTH_LIMIT, i.e. a
                                  line the reference would have decoded and this library did not: the fold took the rest, the caller must
@@ -78,6 +78,13 @@ typedef struct {
                                   caller's input arena exactly as the reference would send them (every mode P line, and a mode R
                                   "data: ...\n" line followed by a blank line) is returned as a span of the input arena and is
                                   neither copied on the device nor sent back over PCIe (see sse_at) */
+#define SSE_FLAG_DEFER 64u     /* a batch whose results do not fit the config's capacities is not failed (SSE_ERR_OVERFLOW never happens):
+                                  - out bytes / frames / records / runs: a segment stops at the start of the round of lines that does not
+                                    fit; its connection state describes exactly the bytes before that point, the segment is flagged
+                                    SSE_SEG_DEFERRED and sse_seg_result.consumed tells how many of its bytes the batch took. The caller
+                                    submits the rest (in[consumed:]) for that connection in a later batch, before any newer bytes.
+                                  - tool calls / usages / decoded text: sse_collect grows the slot's arenas and decodes the batch again.
+                                  sse_result.overflow reports the SSE_OVF_* bits of what was deferred or grown. Not with SSE_FLAG_KERNEL_FUSED. */
 
 /* One segment = the bytes read from ONE connection since the previous batch. in_off is 16-byte aligned. */
 typedef struct {
@@ -150,6 +157,7 @@ typedef struct { int64_t prompt_tokens, completion_tokens, total_tokens; } sse_u
 #define SSE_SEG_LINE_TOO_LONG 0x04u /* a line exceeded carry_slot_bytes and could not continue in the line pool (longer than
                                        max_line_bytes, or no free page): stream failed, connection dead until reset */
 #define SSE_SEG_DEAD         0x08u  /* connection is in the failed state */
+#define SSE_SEG_DEFERRED     0x10u  /* SSE_FLAG_DEFER: the result arenas were full: only the first `consumed` bytes were taken */
 
 /* A run: contiguous frames/recs produced by up to 64 consecutive lines of one segment. */
 typedef struct {
@@ -163,7 +171,8 @@ typedef struct {
     sse_run  run;          /* first run inline */
     uint32_t carry_len;    /* bytes held back (unterminated tail), carried to the next batch: carry slot plus line pool */
     uint32_t flags;        /* SSE_SEG_* */
-    uint32_t reserved;
+    uint32_t consumed;     /* this segment's input bytes the batch took: in_len unless SSE_SEG_DEFERRED (then resubmit in[consumed:]).
+                              A line that continues in the carry slot or line pool counts as taken; a deferred line does not */
 } sse_seg_result;
 
 typedef struct {
@@ -179,7 +188,9 @@ typedef struct {
     const sse_run        *runs;
     const sse_seg_result *segs;
     uint32_t n_decoded, n_derived;  /* statistics: lines decoded by the automaton; n_derived is reserved (0) */
-    uint32_t overflow;              /* SSE_OVF_* bits when status == SSE_ERR_OVERFLOW: which sse_config capacity to raise */
+    uint32_t overflow;              /* SSE_OVF_* bits: status == SSE_ERR_OVERFLOW: which sse_config capacity to raise; with
+                                       SSE_FLAG_DEFER (status SSE_OK): what this batch deferred (OUT, RUNS) or grew and decoded again
+                                       (TCS, USAGES, TEXT); 0 when everything fit */
     uint32_t in_base;               /* arena offsets >= in_base refer to in[off - in_base] */
     const uint8_t *in;              /* the batch's input arena (sse_batch.in_arena), lent until sse_release like out */
 } sse_result;
@@ -188,7 +199,7 @@ typedef struct {
  * off >= r->in_base ? r->in + (off - r->in_base) : r->out + off. */
 const uint8_t *sse_at(const sse_result *r, uint32_t off);
 
-#define SSE_OVF_OUT    0x01u  /* out_arena_bytes / max_frames / max_recs (bump-allocated together per round) */
+#define SSE_OVF_OUT    0x01u  /* out_arena_bytes / max_frames / max_recs / work items (bump-allocated together per round) */
 #define SSE_OVF_TCS    0x02u  /* max_tcs */
 #define SSE_OVF_USAGES 0x04u  /* max_usages */
 #define SSE_OVF_TEXT   0x08u  /* text_arena_bytes */
@@ -211,7 +222,8 @@ int  sse_abi_version(void);
 void sse_default_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_per_batch);
 /* Capacities under which NO input can overflow a result arena (a batch of bytes_per_batch bytes on max_conns connections):
  * memory grows to ~30x the batch size, meant for small batcher arenas (sse_gateway.h uses it). With sse_default_config the
- * capacities fit realistic SSE traffic and a pathological batch fails as a whole with SSE_ERR_OVERFLOW. */
+ * capacities fit realistic SSE traffic and a pathological batch fails as a whole with SSE_ERR_OVERFLOW, unless the context
+ * runs with SSE_FLAG_DEFER (then what does not fit waits for the next batch, or the decode arenas grow). */
 void sse_worst_case_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_per_batch);
 
 /* Line pool: pages in HBM shared by all connections of a context. A line that outgrows its connection's carry slot

@@ -8,7 +8,7 @@ from . import build as _build
 
 SSE_OK, SSE_ERR_NO_DEVICE, SSE_ERR_CUDA, SSE_ERR_ARG, SSE_ERR_BUSY, SSE_ERR_OVERFLOW, SSE_ERR_NOMEM, SSE_ERR_UNDECODED = 0, -1, -2, -3, -4, -5, -6, -7
 MODE_P, MODE_R, MODE_PARSE = 0, 1, 2
-FLAG_KERNEL_FUSED, FLAG_COPY_OUT, FLAG_TEMPLATES = 4, 8, 16
+FLAG_KERNEL_FUSED, FLAG_COPY_OUT, FLAG_TEMPLATES, FLAG_DEFER = 4, 8, 16, 64
 NONE = 0xFFFFFFFF
 MAX_LINE_BYTES = 16777215   # SSE_MAX_LINE_BYTES: decode work items carry a 24-bit payload length
 
@@ -17,7 +17,8 @@ F_DONE_LINE, F_DONE_EXACT, F_TERMINATES, F_DEPTH_LIMIT, F_TOO_LONG = 0x20, 0x40,
 F_FINISH_SHIFT, F_FINISH_MASK = 12, 0x7000
 TC_HAS_ID, TC_HAS_TYPE, TC_HAS_FUNC = 0x1, 0x2, 0x4
 TC_ID_TEXT, TC_TYPE_TEXT, TC_NAME_TEXT, TC_ARGS_TEXT = 0x10, 0x20, 0x40, 0x80
-SEG_TERMINATED, SEG_FINISHED, SEG_LINE_TOO_LONG, SEG_DEAD = 0x1, 0x2, 0x4, 0x8
+SEG_TERMINATED, SEG_FINISHED, SEG_LINE_TOO_LONG, SEG_DEAD, SEG_DEFERRED = 0x1, 0x2, 0x4, 0x8, 0x10
+OVF_OUT, OVF_TCS, OVF_USAGES, OVF_TEXT, OVF_RUNS = 0x1, 0x2, 0x4, 0x8, 0x10
 
 
 class Config(C.Structure):
@@ -61,7 +62,7 @@ class Run(C.Structure):
 
 
 class SegResult(C.Structure):
-    _fields_ = [("run", Run), ("carry_len", C.c_uint32), ("flags", C.c_uint32), ("reserved", C.c_uint32)]
+    _fields_ = [("run", Run), ("carry_len", C.c_uint32), ("flags", C.c_uint32), ("consumed", C.c_uint32)]
 
 
 class Result(C.Structure):

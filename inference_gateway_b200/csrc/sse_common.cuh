@@ -518,10 +518,14 @@ __device__ __forceinline__ void copy_s2g_vec(uint8_t *__restrict__ g_dst, const 
     if (lane < n - done) g_dst[done + lane] = sm_src[done + lane];
 }
 
+struct Resv { uint32_t ob, qb, fb, rb; };   // SSE_FLAG_DEFER: a long line's reservation (out offset, work item, frame, record)
+
 struct RunChain {           // lane-uniform bookkeeping of a segment's result runs
     sse_run first;
     bool have_first;
     uint32_t last_idx;      // index in runs[] of the last appended run (SSE_NONE: the inline one)
+    uint32_t pre;           // SSE_FLAG_DEFER: runs[] entry reserved for the next appended run (SSE_NONE: allocate it then)
+    Resv rv;                // SSE_FLAG_DEFER: where the long line being completed puts its results (reserve_long)
 };
 
 __device__ __noinline__ void append_run(const KParams &P, RunChain &rc, uint32_t ff, uint32_t fc, uint32_t rf, uint32_t rcnt) {
@@ -531,10 +535,13 @@ __device__ __noinline__ void append_run(const KParams &P, RunChain &rc, uint32_t
         rc.first.next = SSE_NONE; rc.have_first = true; rc.last_idx = SSE_NONE;
         return;
     }
-    uint32_t idx = 0;
-    if (lane_id() == 0) idx = atomicAdd(&P.ctr->n_runs, 1u);
-    idx = __shfl_sync(FULL, idx, 0);
-    if (idx >= P.cap_runs) { if (lane_id() == 0) sse_overflow(P.ctr, SSE_OVF_RUNS); return; }
+    uint32_t idx = rc.pre;
+    rc.pre = SSE_NONE;
+    if (idx == SSE_NONE) {
+        if (lane_id() == 0) idx = atomicAdd(&P.ctr->n_runs, 1u);
+        idx = __shfl_sync(FULL, idx, 0);
+        if (idx >= P.cap_runs) { if (lane_id() == 0) sse_overflow(P.ctr, SSE_OVF_RUNS); return; }
+    }
     if (lane_id() == 0) {
         sse_run r; r.frame_first = ff; r.frame_count = fc; r.rec_first = rf; r.rec_count = rcnt; r.next = SSE_NONE;
         P.runs[idx] = r;
@@ -544,12 +551,73 @@ __device__ __noinline__ void append_run(const KParams &P, RunChain &rc, uint32_t
     rc.last_idx = idx;
 }
 
+// ---------------------------------------------------------------- SSE_FLAG_DEFER: results that do not fit wait for a later batch
+// The produce stage allocates with plain atomicAdds (no compare-and-swap on the hot path), so a round or long line that does not
+// fit may leave its counters past a capacity (sse_download clamps them) and holes below it. Out bytes, frames and records in a hole
+// are never referenced by a run. Work items are read by the sort and decode stages whatever references them, so every work item a
+// deferred allocation got below cap_items becomes an empty item that decodes into the sink record recs[cap_recs], which is
+// allocated past the capacity and never returned.
+
+__device__ __noinline__ void empty_items(const KParams &P, uint32_t qb, uint32_t n) {
+    const uint32_t e = min(qb + n, P.cap_items);
+    for (uint32_t i = qb + lane_id(); i < e; i += 32) P.items[i] = make_uint4(0u, 0u, P.cap_recs, 0u);
+}
+
+// SSE_FLAG_DEFER: a round's allocation did not fit (!fits), or the round needs a runs[] entry, which is reserved before the round
+// writes anything. Returns true when the round may write its results; false: its allocation becomes a hole and the segment stops
+// before the round.
+__device__ __noinline__ bool admit_round(const KParams &P, RunChain &rc, bool fits, uint32_t qb, uint32_t nq, bool need_run) {
+    const uint32_t lane = lane_id();
+    uint32_t bits = SSE_OVF_OUT;
+    if (fits && need_run) {
+        uint32_t idx = 0;
+        if (lane == 0) idx = atomicAdd(&P.ctr->n_runs, 1u);
+        idx = __shfl_sync(FULL, idx, 0);
+        if (idx < P.cap_runs) { rc.pre = idx; return true; }
+        bits = SSE_OVF_RUNS;
+    }
+    empty_items(P, qb, nq);
+    if (lane == 0) atomicOr(&P.ctr->overflow, bits);     // reported, but the batch stays good (status untouched)
+    return false;
+}
+
+// SSE_FLAG_DEFER: everything a held line of L bytes ('\n' included) can need when it completes, or nothing: out bytes for the
+// line and the second '\n' of a mode R frame (a pooled line is gathered there and emitted in place), one frame, one record, one
+// work item and, after the segment's first run, one runs[] entry.
+__device__ __noinline__ bool reserve_long(const KParams &P, RunChain &rc, uint32_t L) {
+    const uint32_t lane = lane_id(), bytes = (L + 2u + 15u) & ~15u;
+    const bool need_run = rc.have_first;
+    uint32_t ob = 0, qb = 0, fb = 0, rb = 0, ri = 0;
+    if (lane == 0) {
+        const unsigned long long r0 = atomicAdd(reinterpret_cast<unsigned long long *>(&P.ctr->out_bytes), (unsigned long long)bytes | (1ull << 32));
+        const unsigned long long r1 = atomicAdd(reinterpret_cast<unsigned long long *>(&P.ctr->n_frames), 1ull | (1ull << 32));
+        ob = (uint32_t)r0; qb = (uint32_t)(r0 >> 32); fb = (uint32_t)r1; rb = (uint32_t)(r1 >> 32);
+        if (need_run) ri = atomicAdd(&P.ctr->n_runs, 1u);
+    }
+    ob = __shfl_sync(FULL, ob, 0); qb = __shfl_sync(FULL, qb, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0);
+    ri = __shfl_sync(FULL, ri, 0);
+    const bool run_ok = !need_run || ri < P.cap_runs;
+    const bool rest_ok = ob + bytes + 16u <= P.cap_out && qb < P.cap_items && fb < P.cap_frames && rb < P.cap_recs;
+    if (!run_ok || !rest_ok) {
+        empty_items(P, qb, 1u);
+        if (lane == 0) atomicOr(&P.ctr->overflow, (run_ok ? 0u : SSE_OVF_RUNS) | (rest_ok ? 0u : SSE_OVF_OUT));
+        return false;
+    }
+    // the work item stays empty unless the line turns out to have a payload to decode (process_long_line overwrites it)
+    if (lane == 0) P.items[qb] = make_uint4(0u, 0u, P.cap_recs, 0u);
+    rc.rv.ob = ob; rc.rv.qb = qb; rc.rv.fb = fb; rc.rv.rb = rb;
+    rc.pre = need_run ? ri : SSE_NONE;
+    return true;
+}
+
 // A line that never fit the window, assembled in the connection's carry slot (HBM): classified and emitted straight from
 // global memory. seg >= 0 (split pipeline): its payload becomes a work item like any other line's -- the decode kernel
 // reads payloads from the arenas, so a line of any length up to carry_slot_bytes is decoded. seg < 0 (first-generation
 // kernel): the payload is not decoded (SSE_F_TOO_LONG). at != SSE_NONE: the line already stands in the out arena at offset
 // `at` (a pooled line gathered there, one spare byte after it) and is emitted in place: frame, payload and the swallowed
-// line's materialised payload are spans of it, nothing is copied.
+// line's materialised payload are spans of it, nothing is copied. resv (SSE_FLAG_DEFER): the line's results go where reserve_long
+// put them (rc.rv), and what the line does not use of that reservation is left as a hole.
+template <bool RESV>
 __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, const uint8_t *line, int L, uint32_t mode, int seg = -1,
                                                uint32_t at = SSE_NONE) {
     const uint32_t lane = lane_id();
@@ -577,16 +645,20 @@ __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, c
     uint32_t nf = emit ? 1u : 0u, nr = parse ? 1u : 0u;
     const bool in_place = at != SSE_NONE;
     uint32_t ob = 0, fb = 0, rb = 0, qb = 0;
-    if (lane == 0) {
-        if ((nf || extra) && !in_place) ob = atomicAdd(&P.ctr->out_bytes, ((uint32_t)flen + extra + 15u) & ~15u);
-        if (nf) fb = atomicAdd(&P.ctr->n_frames, 1u);
-        if (nr) rb = atomicAdd(&P.ctr->n_recs, 1u);
-        if (item && !exact) qb = atomicAdd(&P.ctr->n_items, 1u);
+    if (RESV) {
+        ob = rc.rv.ob; fb = rc.rv.fb; rb = rc.rv.rb; qb = rc.rv.qb;
+    } else {
+        if (lane == 0) {
+            if ((nf || extra) && !in_place) ob = atomicAdd(&P.ctr->out_bytes, ((uint32_t)flen + extra + 15u) & ~15u);
+            if (nf) fb = atomicAdd(&P.ctr->n_frames, 1u);
+            if (nr) rb = atomicAdd(&P.ctr->n_recs, 1u);
+            if (item && !exact) qb = atomicAdd(&P.ctr->n_items, 1u);
+        }
+        ob = __shfl_sync(FULL, ob, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0); qb = __shfl_sync(FULL, qb, 0);
+        bool ovf = (!in_place && (nf || extra) && (ob + (uint32_t)flen + extra + 16u > P.cap_out)) || (nf && fb >= P.cap_frames) ||
+                   (nr && rb >= P.cap_recs) || (item && !exact && qb >= P.cap_items);
+        if (ovf) { if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT); return false; }
     }
-    ob = __shfl_sync(FULL, ob, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0); qb = __shfl_sync(FULL, qb, 0);
-    bool ovf = (!in_place && (nf || extra) && (ob + (uint32_t)flen + extra + 16u > P.cap_out)) || (nf && fb >= P.cap_frames) ||
-               (nr && rb >= P.cap_recs) || (item && !exact && qb >= P.cap_items);
-    if (ovf) { if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT); return false; }
     // frame and payload offsets in the out arena
     const uint32_t fo = in_place ? at + (uint32_t)((mode & SSE_MODE_R) ? a : 0) : ob;
     const uint32_t po = in_place ? at + (uint32_t)ps : (emit ? ob + (uint32_t)(ps - ((mode & SSE_MODE_R) ? a : 0)) : ob);
@@ -614,6 +686,7 @@ __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, c
         }
     }
     append_run(P, rc, fb, nf, rb, nr);
+    if (RESV) rc.pre = SSE_NONE;      // a reserved runs[] entry this line did not use stays a hole
     return true;
 }
 
@@ -715,15 +788,16 @@ __device__ __noinline__ bool pool_append(const KParams &P, uint32_t conn, const 
 }
 
 // A pooled line is complete (its last byte, the '\n', was appended): gathered from its pages into the out arena with 16-byte
-// copies, its pages returned to the pool, then classified and emitted in place by process_long_line.
+// copies, classified and emitted in place by process_long_line, then its pages are returned to the pool.
+template <bool RESV>
 __device__ __noinline__ bool pool_long_line(const KParams &P, RunChain &rc, uint32_t conn, int L, uint32_t mode, int seg) {
     const uint32_t lane = lane_id(), PB = P.page_bytes;
     const uint32_t bytes = ((uint32_t)L + 1u + 15u) & ~15u;    // + 1: mode R's frame ends in a second '\n'
     uint32_t ob = 0, pg = 0;
-    if (lane == 0) { ob = atomicAdd(&P.ctr->out_bytes, bytes); pg = ((volatile PoolChain *)P.pool_chain)[conn].first; }
-    ob = __shfl_sync(FULL, ob, 0); pg = __shfl_sync(FULL, pg, 0);
+    if (lane == 0) { if (!RESV) ob = atomicAdd(&P.ctr->out_bytes, bytes); pg = ((volatile PoolChain *)P.pool_chain)[conn].first; }
+    ob = RESV ? rc.rv.ob : __shfl_sync(FULL, ob, 0); pg = __shfl_sync(FULL, pg, 0);
     // on overflow the batch is discarded and the chain stays with the connection: its state still describes the line
-    if (ob + bytes + 16u > P.cap_out) { if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT); return false; }
+    if (!RESV && ob + bytes + 16u > P.cap_out) { if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT); return false; }
     for (uint32_t d = 0; d < (uint32_t)L; d += PB) {
         if (d) pg = pool_next_page(P, pg);
         const uint32_t nv = (min(PB, (uint32_t)L - d) + 15u) >> 4;
@@ -732,14 +806,11 @@ __device__ __noinline__ bool pool_long_line(const KParams &P, RunChain &rc, uint
         for (uint32_t i = lane; i < nv; i += 32) o[i] = __ldcg(s + i);
     }
     __syncwarp();
+    const bool ok = process_long_line<RESV>(P, rc, P.out + ob, L, mode, seg, ob);
+    __syncwarp();
     if (lane == 0) { pool_lock(P.pool_hdr); pool_release_locked(P, conn); pool_unlock(P.pool_hdr); }
     __syncwarp();
-    return process_long_line(P, rc, P.out + ob, L, mode, seg, ob);
-}
-
-// A line assembled outside the window is complete (clen bytes, '\n' included): in the carry slot, or in the pool.
-__device__ __noinline__ bool complete_long_line(const KParams &P, RunChain &rc, uint32_t conn, const uint8_t *slot, int clen, uint32_t mode, int seg) {
-    return clen > (int)P.carry_slot ? pool_long_line(P, rc, conn, clen, mode, seg) : process_long_line(P, rc, slot, clen, mode, seg);
+    return ok;
 }
 
 // Holds `take` bytes of the window back as the continuation of the connection's unterminated line: in the carry slot while
@@ -750,5 +821,53 @@ __device__ __forceinline__ bool hold_back(const KParams &P, uint32_t conn, uint8
     return true;
 }
 
+// SSE_FLAG_DEFER: the held line of clen bytes gives back its last byte, the '\n' just appended, so that the connection's state
+// describes the line without it. Only the pool can have changed: the '\n' may have taken a new last page, or moved the line
+// out of the carry slot. In the second case the slot holds only the bytes it had before this window (pool_append leaves them
+// there, but writes the window's bytes to the pages alone), so the line's keep bytes are copied back from the pages into the
+// slot before the pages go back.
+__device__ __noinline__ void drop_newline(const KParams &P, uint32_t conn, uint8_t *slot, int clen) {
+    const uint32_t keep = (uint32_t)clen - 1u, PB = P.page_bytes;
+    if (clen <= (int)P.carry_slot || (keep > P.carry_slot && keep % PB != 0)) return;
+    if (keep <= P.carry_slot) {
+        uint32_t pg = 0;
+        if (lane_id() == 0) pg = ((volatile PoolChain *)P.pool_chain)[conn].first;
+        pg = __shfl_sync(FULL, pg, 0);
+        for (uint32_t d = 0; d < keep; d += PB) {     // this warp wrote the pages (pool_append ends in __syncwarp)
+            if (d) pg = pool_next_page(P, pg);
+            const uint32_t n = min(PB, keep - d);
+            copy_g2g_bytes(slot + d, P.pool + (size_t)pg * PB, (int)n);
+        }
+        __syncwarp();
+    }
+    if (lane_id() == 0) {
+        pool_lock(P.pool_hdr);
+        if (keep <= P.carry_slot) pool_release_locked(P, conn);
+        else {
+            volatile PoolHdr *h = P.pool_hdr;
+            volatile PoolChain *c = P.pool_chain + conn;
+            const uint32_t k = c->n_pages;
+            uint32_t pg = c->first;
+            for (uint32_t i = 0; i + 2u < k; i++) pg = pool_next_page(P, pg);
+            const uint32_t n = h->n_free;
+            ((volatile uint32_t *)P.pool_stack)[n] = c->last;
+            h->n_free = n + 1u;
+            c->last = pg; c->n_pages = k - 1u;
+        }
+        pool_unlock(P.pool_hdr);
+    }
+    __syncwarp();
+}
+
+// A line assembled outside the window is complete (clen bytes, '\n' included): in the carry slot, or in the pool. false: its
+// results do not fit; without SSE_FLAG_DEFER the batch has failed. With SSE_FLAG_DEFER everything the line's results can need
+// is reserved before anything is written, and when that does not fit the line gives its '\n' back: the connection keeps the
+// line's other bytes (clen - 1) and the '\n' is the first byte the caller resubmits.
+template <bool DEFER>
+__device__ __noinline__ bool complete_long_line(const KParams &P, RunChain &rc, uint32_t conn, uint8_t *slot, int clen, uint32_t mode, int seg) {
+    if (DEFER && !reserve_long(P, rc, (uint32_t)clen)) { drop_newline(P, conn, slot, clen); return false; }
+    return clen > (int)P.carry_slot ? pool_long_line<DEFER>(P, rc, conn, clen, mode, seg)
+                                    : process_long_line<DEFER>(P, rc, slot, clen, mode, seg);
+}
 
 } // namespace

@@ -58,7 +58,7 @@ struct alignas(8) Counters {
     uint32_t item_ticket;  // split pipeline: next item batch for the decode kernel
     uint32_t n_tiles;      // fused pipeline: tiles written by the plan kernel
     uint32_t reserved1;
-    uint32_t overflow;     // SSE_OVF_* bits: which arena was too small
+    uint32_t overflow;     // SSE_OVF_* bits: which arena was too small (SSE_FLAG_DEFER: also what the produce stage deferred)
     uint32_t pad[2];
     // device-only tail (the host reads the struct up to here)
     uint32_t class_count[SSE_N_BUCKETS];  // split pipeline: items per bucket (see item_bucket)
@@ -113,6 +113,7 @@ __device__ __forceinline__ void sse_overflow(Counters *c, uint32_t which) {
 // launch wrappers (sse_kernel.cu)
 int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count);           // split pipeline, stage 1
 int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device);  // split pipeline, stages 2+3
+int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device);           // SSE_FLAG_DEFER: stage 2 again (grown arenas)
 int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream);              // line pool: reset one connection (SSE_NONE: all)
 int sse_v2_prepare(int device);                                                        // builds + uploads the automaton tables
 int sse_fused_prepare(int device);                                                     // fused pipeline: tables + kernel attributes

@@ -1640,7 +1640,7 @@ __device__ __noinline__ void finish_segment(const KParams &P, FSmem &S, uint32_t
         if (!(sg.state & FS_SKIP)) { ConnState ns; ns.carry_len = carry; ns.flags = cflags; P.conns[sg.conn] = ns; }
         sse_seg_result *r = &P.seg_results[gs];
         if (sg.nruns == 0) { sse_run z; z.frame_first = z.frame_count = z.rec_first = z.rec_count = 0; z.next = SSE_NONE; r->run = z; }
-        r->carry_len = carry; r->flags = flags; r->reserved = 0;
+        r->carry_len = carry; r->flags = flags; r->consumed = P.segs[gs].in_len;
     }
 }
 

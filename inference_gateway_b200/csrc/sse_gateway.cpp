@@ -38,6 +38,7 @@ struct Stream {
     bool terminated = false;    // mode R: agent loop left (finish_reason stop/tool_calls)
     sse_agent_fold *agent = nullptr;
     bool done_sent = false;
+    bool deferred = false;      // SSE_FLAG_DEFER: the last batch left bytes of this stream in `pending`; offered first next tick
 };
 
 } // namespace
@@ -57,14 +58,21 @@ ssegw *ssegw_new(int device, uint32_t max_conns, uint32_t bytes_per_batch, int *
 }
 
 ssegw *ssegw_new_ex(int device, uint32_t max_conns, uint32_t bytes_per_batch, const sse_line_pool *pool, int *status) {
-    ssegw *g = new ssegw();
     // worst-case result capacities: whatever the upstreams send (a flood of one-byte lines, of empty tool-call elements ...), a
     // batch cannot overflow, so one connection can never fail the batch of the others; a line pool grows them by its size
-    sse_worst_case_config(&g->cfg, max_conns, bytes_per_batch);
+    sse_config cfg;
+    sse_worst_case_config(&cfg, max_conns, bytes_per_batch);
+    return ssegw_new_cfg(device, &cfg, pool, status);
+}
+
+ssegw *ssegw_new_cfg(int device, const sse_config *cfg, const sse_line_pool *pool, int *status) {
+    if (!cfg || cfg->struct_size != sizeof(sse_config)) { if (status) *status = SSE_ERR_ARG; return nullptr; }
+    ssegw *g = new ssegw();
+    g->cfg = *cfg;
     int rc = sse_init_ex(device, &g->cfg, pool, &g->ctx);
     if (status) *status = rc;
     if (rc != SSE_OK) { delete g; return nullptr; }   // no CUDA device: error, never a CPU path
-    g->streams.resize(max_conns);
+    g->streams.resize(cfg->max_conns);
     return g;
 }
 
@@ -81,7 +89,7 @@ int ssegw_stream_chat_completions(ssegw *g, uint8_t mode) {
         Stream &s = g->streams[i];
         if (!s.open) {
             if (s.agent) sse_agent_reset(s.agent); else s.agent = sse_agent_new();
-            s = Stream{ true, false, false, mode, {}, {}, false, s.agent, false };
+            s = Stream{ true, false, false, mode, {}, {}, false, s.agent, false, false };
             if (sse_reset_conn(g->ctx, (uint32_t)i) != SSE_OK) return -1;
             return (int)i;
         }
@@ -112,9 +120,12 @@ int ssegw_pump(ssegw *g) {
     uint32_t off = 0, n = 0;
     const size_t ns = g->streams.size();
     const size_t start = ns ? g->rr++ % ns : 0;
+    // streams whose bytes a batch deferred (SSE_FLAG_DEFER) go first, so that a flood on other streams cannot keep them waiting
+    for (int pass = 0; pass < 2; pass++)
     for (size_t q = 0; q < ns && n < b.max_segs; q++) {
         const size_t i = (start + q) % ns;
         Stream &s = g->streams[i];
+        if (s.deferred != (pass == 0)) continue;
         if (!s.open || s.closed || s.pending.empty()) continue;
         if (s.chan.size() >= CHAN_CAP) continue;                      // receiver is slow: leave the bytes queued
         // a stream takes what fits: the rest stays queued for the next tick (the carry state on the device makes any cut legal)
@@ -124,7 +135,6 @@ int ssegw_pump(ssegw *g) {
         memcpy(b.in_arena + off, s.pending.data(), take);
         b.segs[n] = sse_seg{ (uint32_t)i, off, (uint32_t)take, s.mode, 0, 0 };
         off = (off + (uint32_t)take + 15u) & ~15u;
-        s.pending.erase(0, take);
         who.push_back((uint32_t)i);
         n++;
     }
@@ -134,13 +144,17 @@ int ssegw_pump(ssegw *g) {
         sse_result res;
         if (rc == SSE_OK) rc = sse_collect(g->ctx, slot, &res);
         if (rc != SSE_OK) {
-            // a failed batch fails its streams: the client sees EOF, exactly like an upstream read error (provider.go:323-330)
+            // a failed batch fails its streams: the client sees EOF, exactly like an upstream read error (provider.go:323-330).
+            // With SSE_FLAG_DEFER a batch does not fail for want of arena space, only on a CUDA or allocation error.
             for (uint32_t i : who) g->streams[i].closed = true;
             sse_release(g->ctx, slot);
             return rc;
         }
         for (uint32_t k = 0; k < n; k++) {
             Stream &s = g->streams[who[k]];
+            // only the bytes the batch took leave the queue: a deferred rest is submitted again, before anything newer
+            s.pending.erase(0, res.segs[k].consumed);
+            s.deferred = (res.segs[k].flags & SSE_SEG_DEFERRED) != 0;
             const sse_run *run = &res.segs[k].run;
             for (;;) {
                 for (uint32_t f = run->frame_first; f < run->frame_first + run->frame_count; f++) {

@@ -46,6 +46,7 @@ struct Slot {
     uint4 *d_items2 = nullptr;                                 // items ordered for the decode kernel
     uint2 *d_tiles = nullptr;                                  // fused pipeline: tile list of the plan kernel
     uint32_t n_segs = 0, in_bytes = 0;
+    uint32_t cap_tcs = 0, cap_usages = 0, cap_text = 0;        // decode-stage capacities (SSE_FLAG_DEFER grows them per slot)
 };
 
 } // namespace
@@ -95,9 +96,9 @@ KParams make_params(sse_ctx *c, Slot &s, uint32_t n_segs) {
     p.out = s.d_out; p.cap_out = c->cfg.out_arena_bytes; p.in_base = in_base_of(c->cfg);
     p.frames = s.d_frames; p.cap_frames = c->cfg.max_frames;
     p.recs = s.d_recs; p.cap_recs = c->cfg.max_recs;
-    p.tcs = s.d_tcs; p.cap_tcs = c->cfg.max_tcs;
-    p.usages = s.d_usages; p.cap_usages = c->cfg.max_usages;
-    p.text = s.d_text; p.cap_text = c->cfg.text_arena_bytes;
+    p.tcs = s.d_tcs; p.cap_tcs = s.cap_tcs;
+    p.usages = s.d_usages; p.cap_usages = s.cap_usages;
+    p.text = s.d_text; p.cap_text = s.cap_text;
     p.runs = s.d_runs; p.cap_runs = c->cfg.max_runs;
     p.seg_results = s.d_segres; p.ctr = s.d_ctr;
     p.items = s.d_items; p.cap_items = c->cfg.max_recs; p.seg_term = s.d_segterm;
@@ -157,17 +158,99 @@ int do_launch(sse_ctx *c, Slot &s, uint32_t n_segs, cudaStream_t st) {
     return SSE_OK;
 }
 
+// Upper bounds of what one batch can ask of the decode stage's arenas. Every payload the decode stage reads stands in the batch's
+// input arena or in its out arena (lines completed from the carry slot or the line pool), so the bounds are sse_worst_case_config's
+// rules applied to both arenas together (the out arena already includes the line pool's growth): a tool-call element takes at
+// least 3 payload bytes ("{},"), a decoded string at most 4 text bytes per payload byte (U+FFFD for every invalid byte, 4-byte
+// aligned allocations), and there is at most one usage per record.
+sse_config worst_decode_caps(const sse_ctx *c) {
+    sse_config w = c->cfg;
+    const uint64_t payload = (uint64_t)w.in_arena_bytes + w.out_arena_bytes, cap = 0xF0000000ull;
+    auto clamp = [&](uint64_t v) { return (uint32_t)(v > cap ? cap : v); };
+    w.max_usages = w.max_recs;
+    w.max_tcs = clamp(payload / 3 + 64);
+    w.text_arena_bytes = clamp(4 * payload + 65536);
+    return w;
+}
+
+// One decode-stage arena of a slot grows from *cap to want elements of T, device and pinned (the slot's stream is idle).
+template <class T> int grow_arena(T *&d, T *&h, uint32_t &cap, uint32_t want) {
+    T *nd = nullptr, *nh = nullptr;
+    if (cudaMalloc((void **)&nd, (size_t)want * sizeof(T)) != cudaSuccess) { cudaGetLastError(); return SSE_ERR_NOMEM; }
+    if (cudaHostAlloc((void **)&nh, (size_t)want * sizeof(T), cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); cudaFree(nd); return SSE_ERR_NOMEM; }
+    cudaFree(d); cudaFreeHost(h);
+    d = nd; h = nh; cap = want;
+    return SSE_OK;
+}
+
+// SSE_FLAG_DEFER: the decode stage ran out of tool-call, usage or text arena (k: its counters, which count on past a capacity, so
+// they say what the batch needs, less what the records that failed earlier could not ask for). Grows each arena that ran out to at
+// least what was counted, and to twice its size where that stays within worst_decode_caps, then runs the decode stage again over the
+// same sorted work items; repeats until the batch fits. Every pass grows an arena past its count, so the loop ends, at the latest
+// when an allocation fails (SSE_ERR_NOMEM). The finalize stage is not run again: where a segment terminates does not depend on these
+// arenas, and it already ran, so connection state and line-pool pages are never touched twice. Later batches may have been
+// submitted meanwhile: the pass is ordered after them (the template cache is shared) and they after it.
+int redecode(sse_ctx *c, Slot &s, Counters &k, cudaStream_t st, uint32_t &grown) {
+    const sse_config w = worst_decode_caps(c);
+    auto want = [](uint32_t cap, uint32_t need, uint32_t worst) {
+        uint64_t v = (uint64_t)cap * 2u;
+        if (v > worst) v = worst;
+        if (v < need) v = need;
+        return (uint32_t)(v > 0xF0000000ull ? 0xF0000000ull : v);
+    };
+    auto grow = [&](auto *&d, auto *&h, uint32_t &cap, uint32_t need, uint32_t worst) {
+        const uint32_t n = want(cap, need, worst);
+        return n > cap ? grow_arena(d, h, cap, n) : (int)SSE_ERR_NOMEM;
+    };
+    while (k.status == SSE_ERR_OVERFLOW) {
+        const uint32_t ovf = k.overflow & (SSE_OVF_TCS | SSE_OVF_USAGES | SSE_OVF_TEXT);
+        if (!ovf) return SSE_ERR_OVERFLOW;   // not reachable: with SSE_FLAG_DEFER only the decode stage fails a batch
+        int rc = SSE_OK;
+        if (ovf & SSE_OVF_TCS) rc = grow(s.d_tcs, s.h_tcs, s.cap_tcs, k.n_tcs, w.max_tcs);
+        if (rc == SSE_OK && (ovf & SSE_OVF_USAGES)) rc = grow(s.d_usages, s.h_usages, s.cap_usages, k.n_usages, w.max_usages);
+        if (rc == SSE_OK && (ovf & SSE_OVF_TEXT)) rc = grow(s.d_text, s.h_text, s.cap_text, k.text_bytes, w.text_arena_bytes);
+        if (rc != SSE_OK) return rc;
+        grown |= ovf;
+        k.n_tcs = k.n_usages = k.text_bytes = 0; k.item_ticket = 0; k.status = SSE_OK; k.overflow = 0;
+        *s.h_ctr = k;
+        CU(cudaMemcpyAsync(s.d_ctr, s.h_ctr, offsetof(Counters, class_count), cudaMemcpyHostToDevice, st));
+        if (c->have_last) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
+        const int e = sse_launch_decode(make_params(c, s, s.n_segs), (void *)st, c->sm_count, c->device);
+        if (e != 0) { cu_ok((cudaError_t)e, "decode kernel launch"); return SSE_ERR_CUDA; }
+        c->launches += 1;
+        CU(cudaEventRecord(c->last_kernel, st));
+        c->have_last = true;
+        CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        k = *s.h_ctr;
+    }
+    return SSE_OK;
+}
+
 int do_download(sse_ctx *c, Slot &s, sse_result *res, cudaStream_t st) {
     CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    const Counters k = *s.h_ctr;
+    Counters k = *s.h_ctr;
     memset(res, 0, sizeof *res);
-    res->status = k.status;
     res->n_segs = s.n_segs;
+    uint32_t bits = 0;
+    if (c->cfg.flags & SSE_FLAG_DEFER) {
+        // the produce stage reports what it deferred in k.overflow without failing the batch; only the decode stage sets status
+        bits = k.overflow;
+        const int rc = redecode(c, s, k, st, bits);
+        if (rc != SSE_OK) { res->status = rc; res->overflow = bits | k.overflow; return rc; }
+    }
+    res->status = k.status;
     if (k.status != SSE_OK) {   // overflow: the batch result is unusable, report loudly
         res->overflow = k.overflow;
         return k.status;
     }
+    res->overflow = bits;
+    // a deferred allocation may leave a produce-stage counter past its capacity (the holes below it are never referenced)
+    auto lim = [](uint32_t n, uint32_t cap) { return n < cap ? n : cap; };
+    k.n_frames = lim(k.n_frames, c->cfg.max_frames); k.n_recs = lim(k.n_recs, c->cfg.max_recs); k.n_runs = lim(k.n_runs, c->cfg.max_runs);
+    k.out_bytes = lim(k.out_bytes, c->cfg.out_arena_bytes); k.n_items = lim(k.n_items, c->cfg.max_recs);
+    k.n_tcs = lim(k.n_tcs, s.cap_tcs); k.n_usages = lim(k.n_usages, s.cap_usages); k.text_bytes = lim(k.text_bytes, s.cap_text);
     res->n_frames = k.n_frames; res->n_recs = k.n_recs; res->n_tcs = k.n_tcs; res->n_usages = k.n_usages;
     res->n_runs = k.n_runs; res->out_bytes = k.out_bytes; res->text_bytes = k.text_bytes;
     res->n_decoded = k.n_items; res->n_derived = 0;
@@ -275,7 +358,13 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
     if (cfg->n_slots < 1 || cfg->n_slots > 8 || cfg->max_conns == 0 || cfg->max_segs == 0 ||
         (cfg->in_arena_bytes & 15u) || cfg->carry_slot_bytes < 8192 + 16 || (cfg->carry_slot_bytes & 15u)) return SSE_ERR_ARG;
     if ((uint64_t)in_base_of(*cfg) + cfg->in_arena_bytes + 16 >= (1ull << 31)) return SSE_ERR_ARG;   // arena offsets are 31-bit
-    if (cfg->flags & ~(SSE_FLAG_KERNEL_FUSED | SSE_FLAG_COPY_OUT | SSE_FLAG_TEMPLATES)) return SSE_ERR_ARG;          // unknown engine flag
+    if (cfg->flags & ~(SSE_FLAG_KERNEL_FUSED | SSE_FLAG_COPY_OUT | SSE_FLAG_TEMPLATES | SSE_FLAG_DEFER)) return SSE_ERR_ARG;   // unknown engine flag
+    if ((cfg->flags & SSE_FLAG_DEFER) && (cfg->flags & SSE_FLAG_KERNEL_FUSED)) return SSE_ERR_ARG;   // the tile kernel does not defer
+    // with SSE_FLAG_DEFER a segment alone in a batch must always get somewhere: one round of up to 64 lines (at most a window of
+    // bytes plus a '\n' per line), and the longest line a connection may hold, must fit an empty batch
+    if ((cfg->flags & SSE_FLAG_DEFER) &&
+        (cfg->max_frames < 64 || cfg->max_recs < 64 || cfg->out_arena_bytes < 8192 + 1024 ||
+         (uint64_t)cfg->out_arena_bytes < (uint64_t)(pool.pool_pages ? pool.max_line_bytes : cfg->carry_slot_bytes) + 64)) return SSE_ERR_ARG;
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0 || device < 0 || device >= n) {
         cu_ok(cudaGetLastError(), "cudaGetDeviceCount");
@@ -324,7 +413,9 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
         ok = ok && dalloc(s.d_segs, cfg->max_segs);
         ok = ok && dalloc(s.d_out, (size_t)in_base_of(*cfg) + cfg->in_arena_bytes + 16);
         if (ok) s.d_in = s.d_out + in_base_of(*cfg);
-        ok = ok && dalloc(s.d_frames, cfg->max_frames) && dalloc(s.d_recs, cfg->max_recs);
+        // recs[max_recs]: the sink record of the empty work items a deferred allocation leaves (SSE_FLAG_DEFER), never returned
+        ok = ok && dalloc(s.d_frames, cfg->max_frames) && dalloc(s.d_recs, (size_t)cfg->max_recs + 1);
+        s.cap_tcs = cfg->max_tcs; s.cap_usages = cfg->max_usages; s.cap_text = cfg->text_arena_bytes;
         ok = ok && dalloc(s.d_tcs, cfg->max_tcs) && dalloc(s.d_usages, cfg->max_usages) && dalloc(s.d_text, cfg->text_arena_bytes);
         ok = ok && dalloc(s.d_runs, cfg->max_runs) && dalloc(s.d_segres, cfg->max_segs) && dalloc(s.d_ctr, 1);
         ok = ok && dalloc(s.d_items, cfg->max_recs) && dalloc(s.d_segterm, cfg->max_segs);

@@ -24,7 +24,8 @@ namespace {
 #ifndef SSE_V1_MINB
 #define SSE_V1_MINB 2
 #endif
-template <bool SPLIT>
+// DEFER: SSE_FLAG_DEFER (its own instantiation: the cold deferral paths do not weigh on the default kernel's registers)
+template <bool SPLIT, bool DEFER>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, SSE_V1_MINB)
 sse_stream_kernel(const __grid_constant__ KParams P) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -60,7 +61,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
         const uint32_t conn = seg.conn;
         ConnState cst = P.conns[conn];
         uint8_t *slot = P.carry + (size_t)conn * P.carry_slot;
-        RunChain rc; rc.have_first = false; rc.last_idx = SSE_NONE;
+        RunChain rc; rc.have_first = false; rc.last_idx = SSE_NONE; rc.pre = SSE_NONE;
         rc.first.frame_first = rc.first.frame_count = rc.first.rec_first = rc.first.rec_count = 0; rc.first.next = SSE_NONE;
         uint32_t seg_flags = 0;
         if (SPLIT && lane == 0) P.seg_term[s] = SSE_NONE;
@@ -68,7 +69,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
         if (cst.flags & (CONN_FINISHED | CONN_DEAD)) {
             if (lane == 0) {
                 sse_seg_result r; r.run = rc.first; r.carry_len = cst.carry_len;
-                r.flags = (cst.flags & CONN_DEAD) ? SSE_SEG_DEAD : SSE_SEG_FINISHED; r.reserved = 0;
+                r.flags = (cst.flags & CONN_DEAD) ? SSE_SEG_DEAD : SSE_SEG_FINISHED; r.consumed = seg.in_len;
                 P.seg_results[s] = r;
             }
             continue;
@@ -87,6 +88,9 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
         int consumed = 0;
         const int in_len = (int)seg.in_len;
         const uint8_t *src = P.in + seg.in_off;
+        // overflow: the segment stops. Without SSE_FLAG_DEFER the batch has failed; with it the rest of the segment is deferred
+        // and `consumed` becomes the input-arena offset of the first byte not taken (before seg.in_off: that line starts in the
+        // carried tail)
         bool terminated = false, dead = false, overflow = false;
 
         for (;;) {   // windows
@@ -126,7 +130,10 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     if (consumed >= in_len) break;
                     continue;
                 }
-                if (!complete_long_line(P, rc, conn, slot, clen, mode, SPLIT ? (int)s : -1)) { overflow = true; break; }
+                if (!complete_long_line<DEFER>(P, rc, conn, slot, clen, mode, SPLIT ? (int)s : -1)) {
+                    consumed = q + in_delta; clen--;   // (SSE_FLAG_DEFER) the segment stops at the line's '\n'
+                    overflow = true; break;
+                }
                 __syncwarp();
                 in_long = false; clen = 0; pos = q + 1;
             }
@@ -262,10 +269,20 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     ob = (uint32_t)r0; qb = (uint32_t)(r0 >> 32); fb = (uint32_t)r1; rb = (uint32_t)(r1 >> 32);
                 }
                 ob = __shfl_sync(FULL, ob, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0); qb = __shfl_sync(FULL, qb, 0);
-                if (ob + tot_b + 16 > P.cap_out || fb + tot_f > P.cap_frames || rb + tot_r > P.cap_recs ||
-                    (SPLIT && qb + tot_q > P.cap_items)) {
-                    if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT);
-                    overflow = true; break;
+                if (!DEFER) {
+                    if (ob + tot_b + 16 > P.cap_out || fb + tot_f > P.cap_frames || rb + tot_r > P.cap_recs ||
+                        (SPLIT && qb + tot_q > P.cap_items)) {
+                        if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT);
+                        overflow = true; break;
+                    }
+                } else {
+                    const bool fits = !(ob + tot_b + 16 > P.cap_out || fb + tot_f > P.cap_frames || rb + tot_r > P.cap_recs ||
+                                        (SPLIT && qb + tot_q > P.cap_items));
+                    const bool need_run = rc.have_first && (tot_f | tot_r) != 0u;
+                    if ((!fits || need_run) && !admit_round(P, rc, fits, qb, tot_q, need_run)) {
+                        consumed = pos + in_delta;   // the segment stops before this round
+                        overflow = true; break;
+                    }
                 }
                 // frame table
                 #pragma unroll
@@ -408,12 +425,21 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
 
         if (terminated) seg_flags |= SSE_SEG_TERMINATED;
         if (dead) seg_flags |= SSE_SEG_LINE_TOO_LONG | SSE_SEG_DEAD;
+        const bool deferred = DEFER && overflow;
+        if (deferred) seg_flags |= SSE_SEG_DEFERRED;
         if (lane == 0) {
             ConnState ns;
-            ns.carry_len = (terminated || dead) ? 0u : (uint32_t)clen;
-            ns.flags = (terminated ? CONN_FINISHED : 0u) | (dead ? CONN_DEAD : 0u) | ((in_long && !terminated && !dead) ? CONN_LONG : 0u);
-            P.conns[conn] = ns;
-            sse_seg_result r; r.run = rc.first; r.carry_len = ns.carry_len; r.flags = seg_flags; r.reserved = 0;
+            if (deferred) consumed -= (int)P.segs[s].in_off;
+            if (deferred && consumed < 0) {
+                // deferred at the first line, which starts in the carried tail: the connection is left exactly as it was
+                ns = P.conns[conn]; consumed = 0;
+            } else {
+                ns.carry_len = (terminated || dead) ? 0u : (uint32_t)clen;
+                ns.flags = (terminated ? CONN_FINISHED : 0u) | (dead ? CONN_DEAD : 0u) | ((in_long && !terminated && !dead) ? CONN_LONG : 0u);
+                P.conns[conn] = ns;
+            }
+            sse_seg_result r; r.run = rc.first; r.carry_len = ns.carry_len; r.flags = seg_flags;
+            r.consumed = deferred ? (uint32_t)consumed : seg.in_len;
             P.seg_results[s] = r;
         }
         __syncwarp();
@@ -422,16 +448,16 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
 
 } // namespace
 
-template <bool SPLIT>
+template <bool SPLIT, bool DEFER>
 static int launch_v1(const KParams &p, void *stream, int sm_count) {
     static bool attr_set = false;
     static int ctas_per_sm = 0;
     const size_t smem = sizeof(CtaSmem);
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(sse_stream_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(sse_stream_kernel<SPLIT, DEFER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return (int)e;
         int n = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sse_stream_kernel<SPLIT>, WARPS_PER_CTA * 32, smem);
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sse_stream_kernel<SPLIT, DEFER>, WARPS_PER_CTA * 32, smem);
         if (e != cudaSuccess) return (int)e;
         ctas_per_sm = n > 0 ? n : 1;
         attr_set = true;
@@ -439,8 +465,10 @@ static int launch_v1(const KParams &p, void *stream, int sm_count) {
     int grid = sm_count * ctas_per_sm;   // persistent: one resident wave, warps pull segments by ticket
     int need = (int)((p.n_segs + WARPS_PER_CTA - 1) / WARPS_PER_CTA);
     if (need < grid) grid = need > 0 ? need : 1;
-    sse_stream_kernel<SPLIT><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(p);
+    sse_stream_kernel<SPLIT, DEFER><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(p);
     return (int)cudaGetLastError();
 }
 
-int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count) { return launch_v1<true>(p, stream, sm_count); }
+int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count) {
+    return (p.flags & SSE_FLAG_DEFER) ? launch_v1<true, true>(p, stream, sm_count) : launch_v1<true, false>(p, stream, sm_count);
+}

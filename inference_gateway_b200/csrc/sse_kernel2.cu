@@ -747,8 +747,11 @@ __device__ __noinline__ void t_build(const KParams &P, TCtx &X, const TRec &R, u
     T[1] = litb | (tflags << 16) | (tc_count << 24); T[2] = rec_static; T[3] = n_choices | (n_items << 16);
     uint32_t *items = T + T_HDR, *tcs = items + n_items, *lw = tcs + (tc_count ? 4u : 0u);
     if (tc_count) {
-        uint32_t w4[4] = { 0, 0, 0, 0 }, t = tc_first;
-        for (uint32_t j = 0; j < tc_count && t != SSE_NONE; j++) { w4[j >> 2] |= (P.tcs[t].flags & 7u) << ((j & 3u) * 8u); t = P.tcs[t].next; }
+        uint32_t w4[4] = { 0, 0, 0, 0 }, t = tc_first, j = 0;
+        for (; j < tc_count && t != SSE_NONE; j++) { w4[j >> 2] |= (P.tcs[t].flags & 7u) << ((j & 3u) * 8u); t = P.tcs[t].next; }
+        // a chain shorter than tc_count: the tool-call arena was full (the batch is decoded again after it grows, SSE_FLAG_DEFER);
+        // the flags of the missing elements are unknown, so no template
+        if (j < tc_count) return;
         tcs[0] = w4[0]; tcs[1] = w4[1]; tcs[2] = w4[2]; tcs[3] = w4[3];
     }
     prev = ps;
@@ -1025,7 +1028,10 @@ __global__ void __launch_bounds__(SCATTER_TPB) sse_bucket_scatter_kernel(const K
 
 // ---------------------------------------------------------------- split pipeline, stage 3: early termination
 // One thread per segment: cut the segment's runs after the terminating chunk and mark the connection finished
-// (everything after it is never read by the reference, mcp/agent.go:235-242 and :169).
+// (everything after it is never read by the reference, mcp/agent.go:235-242 and :169). A finished segment has nothing left to
+// resubmit: bytes its batch deferred (SSE_FLAG_DEFER) would be ignored, so the whole segment counts as consumed. Where the
+// segment terminates does not depend on the tool-call, usage and text arenas, so this stage is complete even when the decode
+// stage ran out of them (and is decoded again by sse_launch_decode).
 __global__ void sse_finalize_kernel(const __grid_constant__ KParams P) {
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= P.n_segs) return;
@@ -1044,8 +1050,9 @@ __global__ void sse_finalize_kernel(const __grid_constant__ KParams P) {
         if (run->next == SSE_NONE) break;
         run = &P.runs[run->next];
     }
-    r.flags |= SSE_SEG_TERMINATED;
+    r.flags = (r.flags | SSE_SEG_TERMINATED) & ~SSE_SEG_DEFERRED;
     r.carry_len = 0;
+    r.consumed = P.segs[s].in_len;
     P.seg_results[s] = r;
     const uint32_t conn = P.segs[s].conn;
     // the produce stage kept reading after the terminating chunk and may have pooled a line that is never completed
@@ -1118,6 +1125,15 @@ int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int
     if (e != cudaSuccess) return (int)e;
     const int tpb = 256;
     sse_finalize_kernel<<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
+    return (int)cudaGetLastError();
+}
+
+// SSE_FLAG_DEFER, after the tool-call / usage / text arenas of a batch grew: the decode stage again over the items the sort left
+// in items_sorted (the caller has reset the decode counters). Records are rewritten whole, so a second pass gives the records a
+// single pass with large enough arenas gives.
+int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device) {
+    if (p.tcache) sse_decode_kernel<true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), (cudaStream_t)stream>>>(p, g_tables_dev[device]);
+    else sse_decode_kernel<false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), (cudaStream_t)stream>>>(p, g_tables_dev[device]);
     return (int)cudaGetLastError();
 }
 

@@ -32,7 +32,7 @@ USAGE_DT = np.dtype([("prompt", "<i8"), ("completion", "<i8"), ("total", "<i8")]
 RUN_DT = np.dtype([("frame_first", "<u4"), ("frame_count", "<u4"), ("rec_first", "<u4"), ("rec_count", "<u4"),
                    ("next", "<u4")])
 SEGRES_DT = np.dtype([("frame_first", "<u4"), ("frame_count", "<u4"), ("rec_first", "<u4"), ("rec_count", "<u4"),
-                      ("next", "<u4"), ("carry_len", "<u4"), ("flags", "<u4"), ("reserved", "<u4")])
+                      ("next", "<u4"), ("carry_len", "<u4"), ("flags", "<u4"), ("consumed", "<u4")])
 SEG_DT = np.dtype([("conn", "<u4"), ("in_off", "<u4"), ("in_len", "<u4"), ("mode", "u1"), ("provider", "u1"),
                    ("reserved", "<u2")])
 assert FRAME_DT.itemsize == 8 and REC_DT.itemsize == 32 and TC_DT.itemsize == 48 and SEGRES_DT.itemsize == 32
@@ -87,6 +87,15 @@ class BatchResult:
 
     def span(self, off: int, length: int, in_text: bool) -> bytes:
         return self.text[off:off + length].tobytes() if in_text else self.at(off, length)
+
+    def consumed(self, i: int) -> int:
+        """Input bytes of segment i the batch took: its whole length unless it was deferred (SSE_FLAG_DEFER, SEG_DEFERRED)."""
+        return int(self.segs[i]["consumed"])
+
+    @property
+    def overflow(self) -> int:
+        """SSE_OVF_* bits of what this batch deferred or grew (SSE_FLAG_DEFER); 0 when everything fit."""
+        return int(self.raw.overflow)
 
 
 def make_line_pool(pool_pages: int, page_bytes: int = 0, max_line_bytes: int = A.MAX_LINE_BYTES) -> A.LinePool:
@@ -215,3 +224,34 @@ class SseEngine:
         self.submit(slot, n, nbytes)
         r = self.collect(slot)
         return slot, r
+
+    def process_all(self, items, on_batch=None) -> int:
+        """items: list of (conn, mode, bytes), at most one per connection, run to the end on an engine with SSE_FLAG_DEFER: the
+        part of a segment a batch deferred is submitted again, from its first byte not taken, in the next batch, until every
+        byte was taken. on_batch(result, conns) sees every batch before its slot is released (conns[i]: the connection of
+        segment i). A batch in which no segment got anywhere (segments competing for arenas that fit each of them alone) is
+        followed by one that carries only the first remaining segment, which always fits an empty batch. Returns the number
+        of batches."""
+        pending = [(c, m, bytes(d)) for c, m, d in items]
+        n_batches = 0
+        alone = False
+        while pending:
+            batch = pending[:1] if alone else pending
+            slot, res = self.process(batch)
+            try:
+                if on_batch is not None:
+                    on_batch(res, [c for c, _, _ in batch])
+                left, progress = [], False
+                for i, (conn, mode, data) in enumerate(batch):
+                    took = res.consumed(i)
+                    if int(res.segs[i]["flags"]) & A.SEG_DEFERRED:
+                        left.append((conn, mode, data[took:]))
+                    progress = progress or took > 0 or not int(res.segs[i]["flags"]) & A.SEG_DEFERRED
+            finally:
+                self.release(slot)
+            if alone and not progress:
+                raise RuntimeError("a segment alone in a batch was deferred without progress: capacities below one round")
+            pending = left + pending[len(batch):]
+            alone = not progress
+            n_batches += 1
+        return n_batches

@@ -8,9 +8,12 @@ from . import _abi as A
 
 
 class Gateway:
-    def __init__(self, device: int = 0, max_conns: int = 256, bytes_per_batch: int = 1 << 20, line_pool: dict | None = None):
+    def __init__(self, device: int = 0, max_conns: int = 256, bytes_per_batch: int = 1 << 20, line_pool: dict | None = None,
+                 config: A.Config | None = None):
         """line_pool: keyword arguments of engine.make_line_pool() (pool_pages, page_bytes, max_line_bytes): lines longer than the
-        64 KiB carry slot continue in a shared device page pool instead of failing their stream."""
+        64 KiB carry slot continue in a shared device page pool instead of failing their stream.
+        config: an sse_config to run on (ssegw_new_cfg; max_conns and bytes_per_batch are then ignored), e.g. default capacities
+        with FLAG_DEFER; None: the worst-case config."""
         from .engine import make_line_pool
         self.L = L = A.load()
         vp, i32 = C.c_void_p, C.c_int
@@ -18,6 +21,8 @@ class Gateway:
         L.ssegw_new.restype = vp
         L.ssegw_new_ex.argtypes = [i32, C.c_uint32, C.c_uint32, C.POINTER(A.LinePool), C.POINTER(i32)]
         L.ssegw_new_ex.restype = vp
+        L.ssegw_new_cfg.argtypes = [i32, C.POINTER(A.Config), C.POINTER(A.LinePool), C.POINTER(i32)]
+        L.ssegw_new_cfg.restype = vp
         L.ssegw_free.argtypes = [vp]
         L.ssegw_free.restype = None
         L.ssegw_stream_chat_completions.argtypes = [vp, C.c_uint8]
@@ -39,10 +44,12 @@ class Gateway:
         L.ssegw_agent_tool_calls.argtypes = [vp, i32, C.POINTER(A.ToolCall), C.c_size_t]
         L.ssegw_agent_tool_calls.restype = C.c_size_t
         st = i32()
-        if line_pool is None:
+        self._pool = make_line_pool(**line_pool) if line_pool is not None else None
+        if config is not None:
+            self.g = L.ssegw_new_cfg(device, C.byref(config), C.byref(self._pool) if self._pool is not None else None, C.byref(st))
+        elif line_pool is None:
             self.g = L.ssegw_new(device, max_conns, bytes_per_batch, C.byref(st))
         else:
-            self._pool = make_line_pool(**line_pool)
             self.g = L.ssegw_new_ex(device, max_conns, bytes_per_batch, C.byref(self._pool), C.byref(st))
         if not self.g:
             raise A.SseError(st.value, "ssegw_new")

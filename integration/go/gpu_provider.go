@@ -21,6 +21,8 @@ import (
 // (carry state and FIFO order are per device). One goroutine per GPU, locked to its OS thread, runs:
 //   acquire -> drain pending reads of its connections into the batch (<= GPU_BATCH_USEC or GPU_BATCH_BYTES) ->
 //   submit -> collect -> fan frames out to the per-stream channels -> release.
+// With GPU_DEFER=1 (see NewContext) a segment can come back Deferred: its unconsumed tail goes back to the head of that
+// connection's queue, and connections with such a tail are drained first into the next batch.
 type Batcher interface {
 	// Open registers a new upstream stream; the returned id addresses its slot until Close.
 	Open(mode uint8) (conn uint32, frames <-chan []byte)

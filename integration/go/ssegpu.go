@@ -54,10 +54,18 @@ func envUint32(name string) uint32 {
 // GPU_LINE_POOL_PAGES > 0 gives the context a line pool of that many pages (GPU_LINE_POOL_PAGE_BYTES each, default 64 KiB),
 // shared by all connections: a line longer than the carry slot continues there instead of failing its stream, up to
 // GPU_LINE_POOL_MAX_LINE bytes per connection (default and ceiling SSE_MAX_LINE_BYTES, 16 MiB - 1).
+//
+// GPU_DEFER=1 sets SSE_FLAG_DEFER: a batch whose results do not fit the default capacities no longer fails (which would close
+// every stream in it); what does not fit waits for the next batch. The batcher must then keep the unconsumed tail of a
+// deferred segment (data[res.Consumed(i):], see Result.Deferred) at the head of that connection's queue and submit it before
+// any newer bytes of the connection.
 func NewContext(device int, maxConns, bytesPerBatch uint32) (*Context, error) {
 	runtime.LockOSThread()
 	var cfg C.sse_config
 	C.sse_default_config(&cfg, C.uint32_t(maxConns), C.uint32_t(bytesPerBatch))
+	if os.Getenv("GPU_DEFER") == "1" {
+		cfg.flags |= C.SSE_FLAG_DEFER
+	}
 	var ctx *C.sse_ctx
 	if pages := envUint32("GPU_LINE_POOL_PAGES"); pages > 0 {
 		maxLine := envUint32("GPU_LINE_POOL_MAX_LINE")
@@ -160,4 +168,15 @@ func (r *Result) Frames(i uint32, fn func(line []byte)) (terminated bool) {
 		run = runs[run.next]
 	}
 	return segs[i].flags&C.SSE_SEG_TERMINATED != 0
+}
+
+// Deferred reports whether the batch took only the first Consumed(i) bytes of segment i (SSE_FLAG_DEFER): the rest has to be
+// submitted again, first in the connection's queue.
+func (r *Result) Deferred(i uint32) bool {
+	return unsafe.Slice(r.r.segs, int(r.r.n_segs))[i].flags&C.SSE_SEG_DEFERRED != 0
+}
+
+// Consumed is the number of segment i's bytes the batch took (its whole length unless Deferred).
+func (r *Result) Consumed(i uint32) uint32 {
+	return uint32(unsafe.Slice(r.r.segs, int(r.r.n_segs))[i].consumed)
 }
