@@ -290,7 +290,11 @@ __device__ bool v2_action(const KParams &P, const DfaTables &T, Lane &L, LaneScr
                     break;
                 case TG_FINISH:
                     if (len == 0) L.finish = SSE_FIN_NONE;
-                    else if (!d2) { uint32_t nm = T.accept[L.km]; uint32_t fv = nm != 0xFFu ? T.finmap[nm] : 0xFFu; L.finish = fv != 0xFFu ? fv : (uint32_t)SSE_FIN_OTHER; }
+                    else if (!d2) {
+                        // the trie folds ASCII case (it matches keys); finish_reason values compare exactly, and all are lower-case
+                        uint32_t nm = (L.sf & SF_UPPER) ? 0xFFu : T.accept[L.km];
+                        uint32_t fv = nm != 0xFFu ? T.finmap[nm] : 0xFFu; L.finish = fv != 0xFFu ? fv : (uint32_t)SSE_FIN_OTHER;
+                    }
                     else {
                         uint8_t tmp[40];
                         uint32_t n = json_unquote(P.out, (int)start, (int)L.p, tmp, 32);

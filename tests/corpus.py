@@ -82,3 +82,166 @@ def mutate(rng, doc: bytes) -> bytes:
     return bytes(b).replace(b"\n", b" ")
 
 
+# ------------------------------------------------------------------ strings at every alignment
+# One string per document, in each field the decoder captures. The decode stage skips plain string bytes 16 at a time, a
+# lane at most 4 windows (64 bytes) per round, a whole warp 512 bytes per step, and unquotes in 32-byte steps; its item sort
+# puts every payload of 4,064 bytes or more in one bucket.
+STRING_FIELDS = {
+    "content": b'{"choices":[{"index":0,"delta":{"content":"%s"},"finish_reason":null}]}',
+    "id": b'{"choices":[{"index":0,"delta":{"tool_calls":[{"index":0,"id":"%s","type":"function","function":{"name":"f","arguments":""}}]}}]}',
+    "name": b'{"choices":[{"index":0,"delta":{"tool_calls":[{"index":0,"id":"c","type":"function","function":{"name":"%s","arguments":""}}]}}]}',
+    "arguments": b'{"choices":[{"index":0,"delta":{"tool_calls":[{"index":0,"function":{"arguments":"%s"}}]}}]}',
+    "finish_reason": b'{"choices":[{"index":0,"delta":{},"finish_reason":"%s"}]}',
+    "thought_signature": b'{"choices":[{"index":0,"delta":{"tool_calls":[{"index":0,"id":"c","extra_content":{"google":{"thought_signature":"%s"}}}]}}]}',
+}
+STRING_LENGTHS = (16, 32, 64, 512, 4096, 8192)
+# what stands at offset k of the string: None = the closing quote, b"EOF" = the payload ends there, anything else is inserted
+STRING_EVENTS = (
+    None, b"EOF",
+    b"\\\\", b'\\"', b"\\n", b"\\u00e9",
+    b"\\ud83d\\ude00", b"\\ud83d", b"\\ude00",                        # a pair, a lone high and a lone low surrogate
+    "é".encode(), "漢".encode(), "😀".encode(),                         # raw UTF-8 of 2, 3 and 4 bytes
+    b"\xe6\xbc", b"\xc0\xaf", b"\xed\xa0\x80", b"\xf4\x90\x80\x80",   # truncated, overlong, surrogate-encoded, above U+10FFFF
+    b"\x01", b"\x1f", b"\x7f",                                        # raw control bytes (invalid JSON), and DEL (valid)
+)
+
+
+def _plain(n: int) -> bytes:
+    from inference_gateway_b200.synth import _WORDS
+    words = b" ".join(w.encode() for w in _WORDS)
+    return (words * (n // len(words) + 1))[:n]
+
+
+def string_offsets(length: int) -> list:
+    """Offsets k of the event in a string of about `length` bytes: 0-33, 480-544 and the last 33 bytes. The 480-544 band is
+    left out at 8,192, where it repeats what 4,096 puts there."""
+    ks = set(range(34)) | set(range(max(0, length - 33), length + 1))
+    if length < 8192:
+        ks |= set(range(480, 545))
+    return sorted(k for k in ks if k <= length)
+
+
+def string_alignment_docs() -> list:
+    """Deterministic: every event of STRING_EVENTS at every offset of string_offsets(L), for each L of STRING_LENGTHS; the
+    field cycles through STRING_FIELDS so that each of them sees every event and every length."""
+    plain = _plain(max(STRING_LENGTHS) + 64)
+    fields = list(STRING_FIELDS.values())
+    docs = []
+    for li, length in enumerate(STRING_LENGTHS):
+        for ei, ev in enumerate(STRING_EVENTS):
+            for k in string_offsets(length):
+                tpl = fields[(li + ei + k) % len(fields)]
+                if ev is None:
+                    docs.append(tpl % plain[:k])
+                elif ev == b"EOF":
+                    docs.append(tpl[:tpl.index(b"%s")] + plain[:k])
+                else:
+                    docs.append(tpl % (plain[:k] + ev + plain[k:max(k, length - len(ev))]))
+    return docs
+
+
+# ------------------------------------------------------------------ skeleton-template near-misses
+# A template is a learnt line with its string bodies and integers cut out (wildcards); a line replays it when everything else
+# is byte for byte the same and every wildcard is again a well-formed string body or integer. The variants below differ from
+# a canonical chunk in one place; whichever way the decoder takes them, the record must be the reference's.
+STRING_VARIANTS = (b"a\\nb", "café".encode(), b"\xff", b"x\x01y", b"5", b"null", b"{}")        # unterminated: built apart
+INT_VARIANTS = (b"01", b"-0", b"-", b"1.0", b"1e2", b"9223372036854775807", b"9223372036854775808",
+                b"-9223372036854775808", b"-9223372036854775809", b"12345678901234567890", b'"1"')
+
+
+def _wildcards(doc: bytes) -> list:
+    """(start, end, kind) of every string value and integer of a JSON document outside strings; a string's span includes
+    its quotes."""
+    out, i, n = [], 0, len(doc)
+    prev = b""                                  # last significant byte outside strings
+    while i < n:
+        c = doc[i:i + 1]
+        if c == b'"':
+            j = i + 1
+            while doc[j:j + 1] != b'"':
+                j += 2 if doc[j:j + 1] == b"\\" else 1
+            if prev in (b":", b"["):
+                out.append((i, j + 1, "str"))
+            elif prev == b"," and _in_array(doc, i):
+                out.append((i, j + 1, "str"))
+            prev = b'"'
+            i = j + 1
+        elif c in b"-0123456789":
+            j = i + 1
+            while j < n and doc[j:j + 1] in b"0123456789.eE+-":
+                j += 1
+            if all(ch in b"-0123456789" for ch in doc[i:j]):
+                out.append((i, j, "int"))
+            prev = b"0"
+            i = j
+        else:
+            if c not in b" \t\r\n":
+                prev = c
+            i += 1
+    return out
+
+
+def _in_array(doc: bytes, i: int) -> bool:
+    depth = 0
+    for j in range(i - 1, -1, -1):
+        ch = doc[j:j + 1]
+        if ch in b"]}":
+            depth += 1
+        elif ch in b"[{":
+            if depth == 0:
+                return ch == b"["
+            depth -= 1
+    return False
+
+
+def canonical_chunks() -> list:
+    """Deterministic: every data payload of one synth stream per flavour, with tool-call chunks and a usage chunk."""
+    from inference_gateway_b200.synth import MODELS, StreamSpec, Synth
+    g = Synth(0x7E3)
+    out = []
+    for fl in MODELS:
+        for tool in (0, 5):
+            body, _ = g.stream(StreamSpec(flavour=fl, n_content=4, tool_run=tool, usage_chunk=True, with_done=False))
+            out += [ev[6:] for ev in body.split(b"\n\n") if ev.startswith(b"data: {")]
+    return out
+
+
+def template_near_misses() -> tuple:
+    """Deterministic: (canonical chunks, near-misses). Per wildcard of every canonical chunk: string bodies with an escape,
+    non-ASCII, invalid UTF-8, a control byte, left unterminated, or a number / null / object in their place; integers with a
+    leading zero, -0, a lone '-', a fraction, an exponent, int64 max / max+1 / min / min-1, 20 digits or a string; the line cut
+    just before and just after the wildcard. Per chunk: the first occurrence of a key name with another case or a Unicode
+    folding (K = Kelvin sign, ſ = long s) -- that is the value in "finish_reason":"tool_calls", which must then compare
+    exactly --, a duplicated key, extra whitespace, and a key changed in the middle so the line keeps its last two bytes."""
+    canon = canonical_chunks()
+    miss = []
+    for doc in canon:
+        for s, e, kind in _wildcards(doc):
+            if kind == "str":
+                miss += [doc[:s + 1] + v + doc[e - 1:] for v in STRING_VARIANTS[:4]]
+                miss += [doc[:s] + v + doc[e:] for v in STRING_VARIANTS[4:]]
+                miss.append(doc[:e - 1] + doc[e:])                       # the closing quote is gone
+            else:
+                miss += [doc[:s] + v + doc[e:] for v in INT_VARIANTS]
+            miss += [doc[:s], doc[:e]]
+        keys = [(m, m + len(k)) for k in (b'"index"', b'"content"', b'"choices"', b'"id"', b'"tool_calls"', b'"arguments"',
+                                          b'"prompt_tokens"', b'"finish_reason"') for m in [doc.find(k)] if m >= 0]
+        for s, e in keys:
+            key = doc[s:e]
+            miss.append(doc[:s] + key.upper() + doc[e:])
+            if b"k" in key:
+                miss.append(doc[:s] + key.replace(b"k", "K".encode(), 1) + doc[e:])
+            if b"s" in key:
+                miss.append(doc[:s] + key.replace(b"s", "ſ".encode(), 1) + doc[e:])
+            # the key and its value once more, right behind it
+            v = next(((a, b) for a, b, _ in _wildcards(doc) if a > e), None)
+            if v is not None and doc[e:v[0]].strip() == b":":
+                miss.append(doc[:v[1]] + b"," + doc[s:v[1]] + doc[v[1]:])
+            miss.append(doc[:e] + b" " + doc[e:])
+        miss.append(doc[:-1] + b" " + doc[-1:])
+        # a letter of a key, the one nearest the middle, replaced
+        wild = _wildcards(doc)
+        letters = [i for i in range(len(doc)) if chr(doc[i]).isalpha() and not any(s <= i < e for s, e, _ in wild)]
+        m = min(letters, key=lambda i: abs(i - len(doc) // 2))
+        miss.append(doc[:m] + (b"y" if doc[m:m + 1] == b"x" else b"x") + doc[m + 1:])
+    return canon, miss

@@ -5,14 +5,11 @@ Two kinds of checks:
     whole body -- as per-connection 64-bit digests of the canonical byte string both sides produce (oracle/orc_check.c; the
     field list is check_stream's), plus frame / record counts, termination and the held-back tail length;
   * size-independent properties: exact byte identities between input and output, record/frame accounting, idempotence."""
-import os
-
 import numpy as np
 import pytest
 
 from inference_gateway_b200 import SseEngine, _abi as A, synth
-from oracle import orc
-from tests.util import check_stream, run_streams
+from tests.util import check_stream, cut_bounds, digest_run, oracle_digests, run_streams
 
 pytestmark = pytest.mark.gpu
 N = 65536
@@ -26,75 +23,53 @@ def workload():
 
 
 @pytest.fixture(scope="module")
-def eng(workload):
-    e = SseEngine(device=0, max_conns=N, bytes_per_batch=sum(map(len, workload)), n_slots=1, carry_slot_bytes=16384)
-    yield e
-    e.close()
+def engines(workload):
+    """engines(flags): the full-size context with those engine flags; one context lives at a time."""
+    live = {}
+
+    def get(flags):
+        if flags not in live:
+            for e in live.values():
+                e.close()
+            live.clear()
+            live[flags] = SseEngine(device=0, max_conns=N, bytes_per_batch=sum(map(len, workload)), n_slots=1,
+                                    carry_slot_bytes=16384, flags=flags)
+        return live[flags]
+    yield get
+    for e in live.values():
+        e.close()
+
+
+@pytest.fixture
+def eng(engines):
+    return engines(0)
 
 
 # ------------------------------------------------------------------ oracle parity at full size
-def _digest_run(eng, bodies, mode, n_batches, seed):
-    """Feeds every body in n_batches randomly cut pieces (empty pieces included) and folds every batch result into
-    per-connection digests. Returns (digests, carry_len, seg_flags)."""
-    n = len(bodies)
-    rng = np.random.default_rng(seed)
-    lens = np.fromiter((len(b) for b in bodies), dtype=np.int64, count=n)
-    cuts = np.sort((rng.random((n, n_batches - 1)) * (lens[:, None] + 1)).astype(np.int64), axis=1) if n_batches > 1 else np.zeros((n, 0), np.int64)
-    bounds = np.concatenate([np.zeros((n, 1), np.int64), np.minimum(cuts, lens[:, None]), lens[:, None]], axis=1)
-    d = orc.new_digests(n)
-    carry = np.zeros(n, dtype=np.uint32)
-    flags = np.zeros(n, dtype=np.uint32)
-    conn = np.arange(n, dtype=np.uint32)
-    eng.reset_all()
-    for b in range(n_batches):
-        plen = bounds[:, b + 1] - bounds[:, b]
-        aligned = (plen + 15) & ~15
-        offs = np.zeros(n, dtype=np.int64)
-        offs[1:] = np.cumsum(aligned)[:-1]
-        slot, arena, segs = eng.acquire()
-        for i in range(n):
-            if plen[i]:
-                arena[offs[i]:offs[i] + plen[i]] = np.frombuffer(bodies[i], dtype=np.uint8, count=int(plen[i]), offset=int(bounds[i, b]))
-        segs["conn"][:n] = conn
-        segs["in_off"][:n] = offs
-        segs["in_len"][:n] = plen
-        segs["mode"][:n] = mode
-        segs["provider"][:n] = 0
-        segs["reserved"][:n] = 0
-        eng.submit(slot, n, int(offs[-1] + aligned[-1]))
-        res = eng.collect(slot)
-        try:
-            assert orc.digest_result(res.raw, conn, d, carry, flags) == n
-        finally:
-            eng.release(slot)
-    return d, carry, flags
-
-
-def _oracle_digests(bodies, mode):
-    n = len(bodies)
-    lens = np.fromiter((len(b) for b in bodies), dtype=np.uint32, count=n)
-    offs = np.zeros(n, dtype=np.uint64)
-    offs[1:] = np.cumsum(lens.astype(np.uint64))[:-1]
-    arena = np.frombuffer(b"".join(bodies) + b"\0", dtype=np.uint8)
-    modes = np.full(n, mode, dtype=np.uint8)
-    return orc.digest_streams(arena, offs, lens, modes, max(1, len(os.sched_getaffinity(0))))
-
-
 def _explain(eng, bodies, mode, i, n_batches, seed):
     """A digest differed: rerun that stream alone through the field-by-field checker for a readable message."""
     outs = run_streams(eng, [bodies[i]], [mode], n_batches=n_batches, seed=seed)
     check_stream(bodies[i], mode, outs[0], label=f"stream {i}")
 
 
-@pytest.mark.parametrize("name,n_streams,mode,n_batches", [
-    ("C2", 4096, A.MODE_P, 4), ("C2", 4096, A.MODE_P | A.MODE_PARSE, 5),
-    ("C3", 16384, R, 1), ("C3", 16384, R, 4),
-    ("C4", 65536, R, 1), ("C4", 65536, R, 4), ("C4", 65536, A.MODE_P | A.MODE_PARSE, 6)])
-def test_oracle_parity_at_full_size(eng, workload, name, n_streams, mode, n_batches):
+# the default engine on every case; skeleton templates, COPY_OUT, the tile kernel and the tile kernel with templates on the
+# mode R cases (grouped by engine: one context is built per group)
+ENGINES = {"templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT, "fused": A.FLAG_KERNEL_FUSED,
+           "fused_templates": A.FLAG_KERNEL_FUSED | A.FLAG_TEMPLATES}
+FULLSIZE = [("C2", 4096, A.MODE_P, 4), ("C2", 4096, A.MODE_P | A.MODE_PARSE, 5),
+            ("C3", 16384, R, 1), ("C3", 16384, R, 4),
+            ("C4", 65536, R, 1), ("C4", 65536, R, 4), ("C4", 65536, A.MODE_P | A.MODE_PARSE, 6)]
+
+
+@pytest.mark.parametrize("name,n_streams,mode,n_batches,eng_flags", [
+    pytest.param(*c, 0, id="-".join(map(str, c))) for c in FULLSIZE] + [
+    pytest.param(*c, f, id="-".join(map(str, c)) + "-" + e) for e, f in ENGINES.items() for c in FULLSIZE if c[0] != "C2" and c[2] == R])
+def test_oracle_parity_at_full_size(engines, workload, name, n_streams, mode, n_batches, eng_flags):
+    eng = engines(eng_flags)
     bodies = workload if name == "C4" else [b for b, _, _ in synth.make_config(name, n_streams=n_streams)[0]]
     assert len(bodies) == n_streams
-    od, oterm, otail = _oracle_digests(bodies, mode)
-    gd, carry, flags = _digest_run(eng, bodies, mode, n_batches, seed=1000 + n_batches)
+    od, oterm, otail = oracle_digests(bodies, mode)
+    gd, carry, flags = digest_run(eng, bodies, mode, cut_bounds(bodies, n_batches, seed=1000 + n_batches))
     assert int(gd["inexact"].sum()) == 0                                   # no record left undecoded (TOO_LONG / DEPTH_LIMIT)
     for key in ("n_frames", "frame_bytes", "frames_h", "n_recs", "recs_h"):
         bad = np.nonzero(gd[key] != od[key])[0]
@@ -113,14 +88,14 @@ def test_oracle_parity_at_full_size(eng, workload, name, n_streams, mode, n_batc
 def test_digest_checker_sees_a_single_flipped_bit(eng, workload):
     """The digests are only as good as their sensitivity: corrupt one byte of one body on the oracle side only."""
     bodies = list(workload[:2048])
-    od, _, _ = _oracle_digests(bodies, R)
+    od, _, _ = oracle_digests(bodies, R)
     k = bodies[777].find(b'"content":"') + 12
     twisted = bodies[777][:k] + bytes([bodies[777][k] ^ 1]) + bodies[777][k + 1:]
     bodies2 = bodies[:777] + [twisted] + bodies[778:]
-    od2, _, _ = _oracle_digests(bodies2, R)
+    od2, _, _ = oracle_digests(bodies2, R)
     diff = np.nonzero((od["frames_h"] != od2["frames_h"]) | (od["recs_h"] != od2["recs_h"]))[0]
     assert list(diff) == [777]
-    gd, _, _ = _digest_run(eng, bodies, R, 3, seed=5)
+    gd, _, _ = digest_run(eng, bodies, R, cut_bounds(bodies, 3, seed=5))
     assert np.array_equal(gd["frames_h"], od["frames_h"]) and np.array_equal(gd["recs_h"], od["recs_h"])
     assert gd["recs_h"][777] != od2["recs_h"][777]
 

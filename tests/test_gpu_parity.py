@@ -392,6 +392,17 @@ def test_provider_hint_only_schedules(engine):
         assert got[0][i][0] == [l.out for l in v.lines if l.kind == orc.L_EMITTED]
 
 
+def test_finish_reason_is_case_sensitive(engine):
+    """Keys match case-insensitively, finish_reason values do not: "STOP" or "Tool_Calls" is some other reason, and does not end
+    the stream (agent.go:235-242 compares with "stop" / "tool_calls")."""
+    after = b'data: {"choices":[{"delta":{"content":"after"}}]}\n\n'
+    bodies = [b'data: {"choices":[{"delta":{},"finish_reason":"%s"}]}\n\n' % f + after
+              for f in (b"STOP", b"Stop", b"TOOL_CALLS", b"Tool_Calls", b"LENGTH", b"stop")]
+    outs, _ = _run_and_check(engine, bodies, [R] * len(bodies))
+    assert [o.terminated for o in outs] == [False] * 5 + [True]
+    assert [r["finish"] for o in outs[:5] for r in o.recs[:1]] == [7] * 5
+
+
 def test_done_marker_at_every_alignment(engine):
     """agent.go:181 is a substring test: "[DONE]" anywhere in the trimmed line swallows it. The produce scan finds candidates
     16 bytes per lane ('[' followed by 'D', with the chunk's last byte handled conservatively): every alignment of the

@@ -6,7 +6,8 @@ import pytest
 from inference_gateway_b200 import synth
 from oracle import orc
 from tests import go_model
-from tests.corpus import TRICKY, mutate
+from tests.corpus import (STRING_EVENTS, STRING_LENGTHS, TRICKY, mutate, string_alignment_docs, string_offsets,
+                          template_near_misses)
 from tests.util import chunk_to_dict
 
 
@@ -29,6 +30,32 @@ def test_mutation_fuzz(seed):
         assert orc.json_valid(d) == go_model.parse(d)[0], d
         n_ok += a["json_ok"]
     assert 1000 < n_ok < 5900      # the corpus exercises both outcomes
+
+
+def test_string_alignment_corpus():
+    """The GPU occupancy tests take the oracle as truth on this corpus: pin it here first, on every document."""
+    docs = string_alignment_docs()
+    assert docs == string_alignment_docs()                        # deterministic
+    assert len(docs) == len(STRING_EVENTS) * sum(len(string_offsets(n)) for n in STRING_LENGTHS)
+    n_ok = 0
+    for d in docs:
+        a = chunk_to_dict(orc.unmarshal(d))
+        assert a == go_model.unmarshal(d), d[:200]
+        n_ok += a["json_ok"]
+    assert 0 < n_ok < len(docs)
+
+
+def test_template_near_miss_corpus():
+    canon, miss = template_near_misses()
+    assert (canon, miss) == template_near_misses()
+    for d in canon:
+        assert chunk_to_dict(orc.unmarshal(d))["json_ok"], d
+    n_ok = 0
+    for d in canon + miss:
+        a = chunk_to_dict(orc.unmarshal(d))
+        assert a == go_model.unmarshal(d), d
+        n_ok += a["json_ok"]
+    assert len(canon) < n_ok < len(canon) + len(miss)
 
 
 def test_trim_space_matches_unicode_isspace():

@@ -3,6 +3,7 @@ every frame and every side-band record with the CPU oracle (oracle/ is the check
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -65,6 +66,17 @@ def chunk_to_dict(ck: orc.ChunkView) -> dict:
     return d
 
 
+def fold_segment(o: ConnOut, res, i: int):
+    """Appends segment i of a batch result to its connection's output."""
+    o.frames.extend(res.seg_frames(i))
+    o.recs.extend(rec_to_dict(res, ri) for ri in res.seg_recs(i))
+    sr = res.segs[i]
+    o.carry_len = int(sr["carry_len"])
+    o.flags |= int(sr["flags"])
+    if int(sr["flags"]) & A.SEG_TERMINATED:
+        o.terminated = True
+
+
 def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False):
     """streams: list of bytes (one upstream body per connection); modes: list of mode bits.
     Feeds every stream in n_batches randomly cut pieces (simulated TCP segmentation), one micro-batch per
@@ -93,19 +105,99 @@ def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False):
         try:
             for i, c in enumerate(who):
                 o = outs[c]
-                o.frames.extend(res.seg_frames(i))
-                o.recs.extend(rec_to_dict(res, ri) for ri in res.seg_recs(i))
-                sr = res.segs[i]
-                o.carry_len = int(sr["carry_len"])
-                o.flags |= int(sr["flags"])
-                if int(sr["flags"]) & A.SEG_TERMINATED:
-                    o.terminated = True
+                fold_segment(o, res, i)
                 if with_folds:
                     A.check(L.sse_agent_feed(o.agent, C.byref(res.raw), i), "sse_agent_feed")
                     A.check(L.sse_telemetry_feed(o.tele, C.byref(res.raw), i), "sse_telemetry_feed")
         finally:
             engine.release(slot)
     return outs
+
+
+# ------------------------------------------------------------------ digest parity at scale
+def cut_bounds(bodies, n_batches: int, seed: int) -> np.ndarray:
+    """Seeded random cut positions: row i holds the n_batches + 1 piece boundaries of bodies[i] (empty pieces included)."""
+    n = len(bodies)
+    rng = np.random.default_rng(seed)
+    lens = np.fromiter((len(b) for b in bodies), dtype=np.int64, count=n)
+    cuts = np.sort((rng.random((n, n_batches - 1)) * (lens[:, None] + 1)).astype(np.int64), axis=1) if n_batches > 1 else np.zeros((n, 0), np.int64)
+    return np.concatenate([np.zeros((n, 1), np.int64), np.minimum(cuts, lens[:, None]), lens[:, None]], axis=1)
+
+
+def digest_run(eng, bodies, modes, bounds, providers=None, on_batch=None):
+    """Feeds body i in the pieces bounds[i] gives (one micro-batch per piece index, every connection in every batch, empty
+    pieces included) and folds every batch result into per-connection digests. modes: one mode for all connections or one per
+    connection; providers: the sse_seg.provider hint per connection (default 0). on_batch(batch index, result) sees every
+    result before its slot is released. Returns (digests, carry_len, seg_flags)."""
+    n = len(bodies)
+    n_batches = bounds.shape[1] - 1
+    d = orc.new_digests(n)
+    carry = np.zeros(n, dtype=np.uint32)
+    flags = np.zeros(n, dtype=np.uint32)
+    conn = np.arange(n, dtype=np.uint32)
+    eng.reset_all()
+    for b in range(n_batches):
+        plen = bounds[:, b + 1] - bounds[:, b]
+        aligned = (plen + 15) & ~15
+        offs = np.zeros(n, dtype=np.int64)
+        offs[1:] = np.cumsum(aligned)[:-1]
+        slot, arena, segs = eng.acquire()
+        for i in range(n):
+            if plen[i]:
+                arena[offs[i]:offs[i] + plen[i]] = np.frombuffer(bodies[i], dtype=np.uint8, count=int(plen[i]), offset=int(bounds[i, b]))
+        segs["conn"][:n] = conn
+        segs["in_off"][:n] = offs
+        segs["in_len"][:n] = plen
+        segs["mode"][:n] = modes
+        segs["provider"][:n] = 0 if providers is None else providers
+        segs["reserved"][:n] = 0
+        eng.submit(slot, n, int(offs[-1] + aligned[-1]))
+        res = eng.collect(slot)
+        try:
+            assert orc.digest_result(res.raw, conn, d, carry, flags) == n
+            if on_batch is not None:
+                on_batch(b, res)
+        finally:
+            eng.release(slot)
+    return d, carry, flags
+
+
+def oracle_digests(bodies, modes):
+    """The oracle's digests of whole bodies (modes: one for all or one per body). Returns (digests, terminated, tail_len)."""
+    n = len(bodies)
+    lens = np.fromiter((len(b) for b in bodies), dtype=np.uint32, count=n)
+    offs = np.zeros(n, dtype=np.uint64)
+    offs[1:] = np.cumsum(lens.astype(np.uint64))[:-1]
+    arena = np.frombuffer(b"".join(bodies) + b"\0", dtype=np.uint8)
+    modes = np.ascontiguousarray(np.broadcast_to(np.asarray(modes, dtype=np.uint8), (n,)))
+    return orc.digest_streams(arena, offs, lens, modes, max(1, len(os.sched_getaffinity(0))))
+
+
+def decode_shape(n_items: int, sm_count: int) -> int:
+    """Work items a warp of sse_decode_kernel pulls at a time for a batch of n_items decoded lines (csrc/sse_kernel2.cu:823-832).
+    The kernel runs one CTA of 32 warps per SM. A batch with fewer items than 32 per warp spreads them over every warp, 8 or 16
+    per pull, and then runs the whole warp over any lane left inside a long string (coop_max 32); above 16 per warp the pull
+    is 32 items and the warp helps only when at most SSE_COOP (8) lanes are."""
+    warps = sm_count * 32
+    if n_items >= 32 * warps:
+        return 32
+    per = -(-n_items // warps)
+    return 8 if per <= 8 else (16 if per <= 16 else 32)
+
+
+def item_class(rel: int, provider: int) -> int:
+    """Sort class of a decoded line (csrc/sse_kernel.cu:336-337): its rank among the decoded lines of its produce round (7 and
+    up alike; the second line sorts first) and the segment's provider hint. A line longer than the produce window is class 0
+    (csrc/sse_common.cuh:683)."""
+    o = min(rel, 7)
+    return ((0 if o == 1 else (1 if o == 0 else o)) << 2) | (provider & 3)
+
+
+def item_sort_key(payload_len: int, cls: int) -> int:
+    """Bucket of a work item in the decode kernel's item sort (item_bucket, csrc/sse_kernel2.cu:968-971): payload length in
+    32-byte steps, longest first, every payload of 4,064 bytes or more in the last one; then the class. Items of one bucket
+    keep about the order the produce kernel allocated them in, which follows the segment order."""
+    return ((127 - min(payload_len >> 5, 127)) << 5) | cls
 
 
 def _bytes(b: A.Bytes) -> bytes:
