@@ -41,7 +41,8 @@ class Chunk(C.Structure):
 
 class Line(C.Structure):
     _fields_ = [("line_off", C.c_uint32), ("line_len", C.c_uint32), ("out_off", C.c_uint32),
-                ("out_len", C.c_uint32), ("kind", C.c_uint32), ("chunk", C.c_uint32)]
+                ("out_len", C.c_uint32), ("kind", C.c_uint32), ("chunk", C.c_uint32), ("pay_off", C.c_uint32),
+                ("pay_len", C.c_uint32)]
 
 
 class Result(C.Structure):
@@ -63,6 +64,8 @@ class Usage(C.Structure):
 
 
 L_DROPPED, L_EMITTED, L_DONE, L_UNREAD, L_DONE_EXACT = 0, 1, 2, 3, 4
+JSON_OK, JSON_SYNTAX, JSON_DEPTH = 0, 1, 2
+DEPTH_LIMIT = 128
 FIN_NONE, FIN_STOP, FIN_TOOL_CALLS, FIN_LENGTH, FIN_CONTENT_FILTER, FIN_FUNCTION_CALL, FIN_OTHER = 0, 1, 2, 3, 4, 5, 7
 
 _lib = None
@@ -78,6 +81,8 @@ def lib():
         _lib.orc_trim_space.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
         _lib.orc_json_valid.argtypes = [C.c_char_p, C.c_size_t]
         _lib.orc_json_valid.restype = C.c_int
+        _lib.orc_json_scan.argtypes = [C.c_char_p, C.c_size_t, C.c_int]
+        _lib.orc_json_scan.restype = C.c_int
         _lib.orc_unmarshal_chunk.argtypes = [C.POINTER(Result), C.c_char_p, C.c_size_t]
         _lib.orc_unmarshal_chunk.restype = C.c_uint32
         _lib.orc_passthrough.argtypes = [C.POINTER(Result), C.c_char_p, C.c_size_t, C.c_int]
@@ -99,6 +104,8 @@ def lib():
         _lib.orc_digest_streams.restype = None
         _lib.orc_digest_result.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.orc_digest_result.restype = C.c_uint32
+        _lib.orc_check_result.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]
+        _lib.orc_check_result.restype = C.c_uint32
     return _lib
 
 
@@ -131,6 +138,16 @@ class LineView:
     kind: int
     out: bytes
     chunk: ChunkView | None
+    payload: bytes = b""        # what the line handed to json.Unmarshal (the "[DONE]" a DONE_EXACT line did not decode)
+
+    @property
+    def payload_len(self) -> int:
+        return len(self.payload)
+
+    @property
+    def depth_limited(self) -> bool:
+        """The payload hits the product's documented nesting limit (DESIGN.md §5, deviation 2)."""
+        return self.chunk is not None and json_scan(self.payload, DEPTH_LIMIT) == JSON_DEPTH
 
 
 @dataclass
@@ -179,6 +196,12 @@ def json_valid(payload: bytes) -> bool:
     return bool(lib().orc_json_valid(payload, len(payload)))
 
 
+def json_scan(payload: bytes, max_depth: int = 10000) -> int:
+    """checkValid with a nesting limit: JSON_OK, JSON_SYNTAX, or JSON_DEPTH when a container opens while max_depth are open
+    before the first syntax error."""
+    return lib().orc_json_scan(payload, len(payload), max_depth)
+
+
 def trim_space(s: bytes) -> bytes:
     a, b = C.c_size_t(), C.c_size_t()
     lib().orc_trim_space(s, len(s), C.byref(a), C.byref(b))
@@ -193,7 +216,8 @@ def _stream_view(L, rp, data: bytes, with_builder: bool) -> StreamView:
         ln = r.lines[i]
         lines.append(LineView(data[ln.line_off:ln.line_off + ln.line_len], ln.kind,
                               out[ln.out_off:ln.out_off + ln.out_len],
-                              _chunk_view(r, ln.chunk) if ln.chunk != 0xFFFFFFFF else None))
+                              _chunk_view(r, ln.chunk) if ln.chunk != 0xFFFFFFFF else None,
+                              data[ln.pay_off:ln.pay_off + ln.pay_len]))
     b = b""
     if with_builder:
         n = C.c_size_t()
@@ -294,3 +318,14 @@ def digest_result(raw_result, conn, digests, carry_len, seg_flags) -> int:
     """Folds one sse_result (ctypes struct of the product's C ABI, passed by reference) into per-connection digests."""
     return lib().orc_digest_result(C.addressof(raw_result), conn.ctypes.data, digests.ctypes.data, carry_len.ctypes.data,
                                    seg_flags.ctypes.data)
+
+
+def check_result(raw_result, segs, flags: int, max_line: int) -> tuple[int, str]:
+    """Structural check of one sse_result (ctypes struct, by reference) against the submitted sse_seg descriptors (a numpy
+    array of sse_seg records, at least n_segs long) of an engine with sse_config.flags `flags` whose longest line is max_line.
+    Returns (number of violations, description of the first)."""
+    import numpy as np
+    segs = np.ascontiguousarray(segs)
+    msg = C.create_string_buffer(512)
+    n = lib().orc_check_result(C.addressof(raw_result), segs.ctypes.data, flags, max_line, msg, len(msg))
+    return n, msg.value.decode()

@@ -111,7 +111,7 @@ static int has_prefix(const uint8_t *s, size_t n, const char *p) {
  * Go's scanner (encoding/json/scanner.go): RFC 8259 grammar, whitespace = SP HT CR LF,
  * raw bytes < 0x20 illegal in strings, bytes >= 0x80 unchecked, nesting limit 10000. */
 #define ORC_MAX_DEPTH 10000
-typedef struct { const uint8_t *s; size_t n, p; } jscan;
+typedef struct { const uint8_t *s; size_t n, p; int max_depth, depth_hit; } jscan;
 static void js_ws(jscan *j) {
     while (j->p < j->n) {
         uint8_t c = j->s[j->p];
@@ -172,7 +172,7 @@ static int js_value(jscan *j, int depth) {
     if (j->p >= j->n) return 0;
     uint8_t c = j->s[j->p];
     if (c == '{') {
-        if (depth + 1 > ORC_MAX_DEPTH) return 0;
+        if (depth + 1 > j->max_depth) { j->depth_hit = 1; return 0; }
         j->p++; js_ws(j);
         if (j->p < j->n && j->s[j->p] == '}') { j->p++; return 1; }
         for (;;) {
@@ -191,7 +191,7 @@ static int js_value(jscan *j, int depth) {
         }
     }
     if (c == '[') {
-        if (depth + 1 > ORC_MAX_DEPTH) return 0;
+        if (depth + 1 > j->max_depth) { j->depth_hit = 1; return 0; }
         j->p++; js_ws(j);
         if (j->p < j->n && j->s[j->p] == ']') { j->p++; return 1; }
         for (;;) {
@@ -210,12 +210,13 @@ static int js_value(jscan *j, int depth) {
     if (c == 'n') return js_lit(j, "null");
     return 0;
 }
-int orc_json_valid(const uint8_t *s, size_t n) {
-    jscan j = { s, n, 0 };
-    if (!js_value(&j, 0)) return 0;
+int orc_json_scan(const uint8_t *s, size_t n, int max_depth) {
+    jscan j = { s, n, 0, max_depth, 0 };
+    if (!js_value(&j, 0)) return j.depth_hit ? ORC_JSON_DEPTH : ORC_JSON_SYNTAX;
     js_ws(&j);
-    return j.p == n;
+    return j.p == n ? ORC_JSON_OK : ORC_JSON_SYNTAX;
 }
+int orc_json_valid(const uint8_t *s, size_t n) { return orc_json_scan(s, n, ORC_MAX_DEPTH) == ORC_JSON_OK; }
 
 /* ------------------------------------------------------------------ encoding/json: unquote
  * decode.go unquoteBytes: escapes, surrogate pairs, lone surrogate -> U+FFFD, invalid UTF-8 ->
@@ -363,10 +364,10 @@ typedef struct {
 static void d_ws(dec *d) {
     while (d->p < d->n) { uint8_t c = d->s[d->p]; if (c == ' ' || c == '\t' || c == '\r' || c == '\n') d->p++; else break; }
 }
-static void d_skip(dec *d) { jscan j = { d->s, d->n, d->p }; js_value(&j, 0); d->p = j.p; }
+static void d_skip(dec *d) { jscan j = { d->s, d->n, d->p, ORC_MAX_DEPTH, 0 }; js_value(&j, 0); d->p = j.p; }
 /* reads a string literal at d->p, returns body span */
 static void d_strbody(dec *d, size_t *a, size_t *b) {
-    jscan j = { d->s, d->n, d->p }; js_string(&j);
+    jscan j = { d->s, d->n, d->p, ORC_MAX_DEPTH, 0 }; js_string(&j);
     *a = d->p + 1; *b = j.p - 1; d->p = j.p;
 }
 /* foldName (encoding/json/fold.go, Go >= 1.21): ASCII upper-cases; U+212A -> 'K', U+017F -> 'S' */
@@ -564,7 +565,7 @@ static void d_value(dec *d, int ty, int sub, int ety, int esub, int tgt, int liv
         return;
     }
     if (c == '-' || (c >= '0' && c <= '9')) {
-        jscan j = { d->s, d->n, d->p }; js_number(&j);
+        jscan j = { d->s, d->n, d->p, ORC_MAX_DEPTH, 0 }; js_number(&j);
         const uint8_t *num = d->s + d->p; size_t nn = j.p - d->p;
         d->p = j.p;
         if (ty == TY_INT) {
@@ -667,6 +668,7 @@ static void p_line(void *u, const uint8_t *line, size_t n, size_t off) {
     l->out_off = out_put(c->r, line, n);      /* routes.go:613 w.Write(line) */
     l->out_len = (uint32_t)n;
     if (c->parse && has_prefix(line, n, "data: ")) {
+        l->pay_off = (uint32_t)off + 6; l->pay_len = (uint32_t)n - 7;
         uint32_t ci = orc_unmarshal_chunk(c->r, line + 6, n - 7);
         c->r->lines[c->r->n_lines - 1].chunk = ci;
     }
@@ -692,6 +694,7 @@ static void r_line(void *u, const uint8_t *line, size_t n, size_t off) {
         /* what parseStreamingToolCalls (:377-402) will see for this builder line */
         const uint8_t *dd = t; size_t dn = tn; int pref = 0;
         if (has_prefix(t, tn, "data: ")) { dd = t + 6; dn = tn - 6; pref = 1; }
+        l->pay_off = (uint32_t)(off + (size_t)(dd - line)); l->pay_len = (uint32_t)dn;
         /* A6 breaks only on `data: [DONE]` (:385-396: data == "[DONE]" after the "data: " case); a bare `[DONE]` line
          * takes the switch's default branch (line == "[DONE]" fails case 2) and is skipped, like any unparsable line */
         if (pref && dn == 6 && !memcmp(dd, "[DONE]", 6)) l->kind = ORC_L_DONE_EXACT; /* exact: A6 breaks here */
@@ -702,6 +705,7 @@ static void r_line(void *u, const uint8_t *line, size_t n, size_t off) {
     const uint8_t *pay = t + 6; size_t pn = tn - 6;                               /* :190 */
     if (pn == 0) { l->kind = ORC_L_DROPPED; return; }                             /* :191-193 */
     l->kind = ORC_L_EMITTED;                                                      /* :195-197 */
+    l->pay_off = (uint32_t)(off + (size_t)(pay - line)); l->pay_len = (uint32_t)pn;
     l->out_off = out_put(r, "data: ", 6); out_put(r, pay, pn); out_put(r, "\n\n", 2);
     l->out_len = (uint32_t)(pn + 8);
     buf_put(&g_builder, r->out + l->out_off, l->out_len);

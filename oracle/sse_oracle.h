@@ -75,6 +75,8 @@ typedef struct {
     uint32_t out_off, out_len;     /* emitted bytes in out[] (0 len: nothing emitted) */
     uint32_t kind;                 /* ORC_L_* */
     uint32_t chunk;                /* index into chunks[] or 0xFFFFFFFF */
+    uint32_t pay_off, pay_len;     /* input bytes handed to orc_unmarshal_chunk (when chunk != 0xFFFFFFFF, and for a
+                                      DONE_EXACT line the "[DONE]" it did not decode) */
 } orc_line;
 
 enum { ORC_L_DROPPED = 0,     /* R: not "data: "-prefixed / empty payload */
@@ -105,6 +107,12 @@ void orc_result_clear(orc_result *r);
 void orc_trim_space(const uint8_t *s, size_t n, size_t *a, size_t *b);
 /* encoding/json checkValid: 1 valid, 0 invalid */
 int orc_json_valid(const uint8_t *s, size_t n);
+/* checkValid with a nesting limit, and why it stopped: ORC_JSON_DEPTH when the scan opens a container while max_depth are
+ * open, before the document's first syntax error. max_depth 128 restates the product's documented limit (DESIGN.md §5,
+ * deviation 2: such a line is reported not JSON_OK and flagged SSE_F_DEPTH_LIMIT); Go's own limit is 10000. */
+enum { ORC_JSON_OK = 0, ORC_JSON_SYNTAX = 1, ORC_JSON_DEPTH = 2 };
+#define ORC_DEPTH_LIMIT 128
+int orc_json_scan(const uint8_t *s, size_t n, int max_depth);
 
 /* json.Unmarshal(data, &CreateChatCompletionStreamResponse); appends one orc_chunk. */
 uint32_t orc_unmarshal_chunk(orc_result *r, const uint8_t *data, size_t n);

@@ -1,4 +1,5 @@
 """JSON documents that exercise every decode rule, and a byte-level mutator (shared by CPU and GPU tests)."""
+import numpy as np
 
 TRICKY = [
     b'{}', b'null', b' null ', b'[]', b'"x"', b'5', b'true', b'', b' ', b'{', b'}', b'{"a"}', b'{"a":}', b'{"a":1,}',
@@ -245,3 +246,84 @@ def template_near_misses() -> tuple:
         m = min(letters, key=lambda i: abs(i - len(doc) // 2))
         miss.append(doc[:m] + (b"y" if doc[m:m + 1] == b"x" else b"x") + doc[m + 1:])
     return canon, miss
+
+
+# ------------------------------------------------------------------ nesting at the 128-level limit (DESIGN.md §5, deviation 2)
+NEST_DEPTHS = (127, 128, 129, 130)
+# (name, text before the nested value, text after it, containers open around it)
+NEST_PLACES = [
+    ("top", b"", b"", 0),
+    ("unknown_key", b'{"choices":[{"delta":{"content":"x"}}],"unknown":', b"}", 1),
+    ("content", b'{"choices":[{"delta":{"content":', b"}}]}", 4),
+    ("arguments", b'{"choices":[{"delta":{"tool_calls":[{"index":0,"function":{"name":"f","arguments":', b"}}]}}]}", 7),
+    ("usage", b'{"choices":[],"usage":{"prompt_tokens":1,"x":', b"}}", 2),
+    ("finish_reason", b'{"choices":[{"delta":{},"finish_reason":', b"}]}", 3),
+]
+
+
+def nest_kinds(n: int, pattern: str) -> list:
+    """Container kinds ('[' or '{') of n nested levels: all arrays, all objects, alternating, or seeded random."""
+    if pattern == "arr":
+        return ["["] * n
+    if pattern == "obj":
+        return ["{"] * n
+    if pattern == "alt":
+        return ["[{"[i & 1] for i in range(n)]
+    rng = np.random.default_rng(n)
+    return ["[{"[int(b)] for b in rng.integers(0, 2, size=n)]
+
+
+def _open(k: str) -> bytes:
+    return b"[" if k == "[" else b'{"k":'
+
+
+def _close(k: str) -> bytes:
+    return b"]" if k == "[" else b"}"
+
+
+def nested(kinds, leaf: bytes = b"1") -> bytes:
+    return b"".join(_open(k) for k in kinds) + leaf + b"".join(_close(k) for k in reversed(kinds))
+
+
+def nesting_docs() -> list:
+    """Payloads around the nesting limit: (name, payload, shallow twin). The twin has the payload's text with the nested value
+    shallow, so a template engine has seen the line's shape when the deep one comes.
+    - every depth of NEST_DEPTHS at top level, under an unknown key and inside each captured field, in four kinds of nesting;
+      brackets inside a string at those depths (they do not count);
+    - each depth with a syntax error just before and just after the 129th opener;
+    - a mismatched closer at every depth 1-129, where the nesting opens to that depth, and where it opens to 128 and closes
+      down to it, so both 64-bit words of the container-type stack and their boundary are read;
+    - the same behind a 4,208-byte string, so the deep part starts after many 16-byte windows and a long-string skip."""
+    out = []
+    long_head = b'{"choices":[{"delta":{"content":"' + b"abcdefghijklmnop" * 263 + b'"}}],"x":'
+    for d in NEST_DEPTHS:
+        for name, pre, post, around in NEST_PLACES:
+            for pat in ("arr", "obj", "alt", "rnd"):
+                kinds = nest_kinds(d - around, pat)
+                out.append((f"{name}-{pat}-d{d}", pre + nested(kinds) + post, pre + nested(kinds[:2]) + post))
+        s = b'{"choices":[{"delta":{"content":"' + b"[{" * d + b'"}}]}'
+        out.append((f"in_string-d{d}", s, b'{"choices":[{"delta":{"content":"[{"}}]}'))
+        for where in ("before", "after"):
+            kinds = nest_kinds(d, "alt")
+            at = 128 if where == "before" else min(129, d)         # openers before the bad byte
+            body = b"".join(_open(k) for k in kinds[:at]) + b"\x01" + b"".join(_open(k) for k in kinds[at:]) + b"1" + \
+                b"".join(_close(k) for k in reversed(kinds))
+            out.append((f"syntax_{where}-d{d}", body, nested(kinds[:2])))
+            out.append((f"syntax_{where}-long-d{d}", long_head + body + b"}", long_head + nested(kinds[:2]) + b"}"))
+    for k in range(1, 130):
+        for pat in ("alt", "rnd"):
+            kinds = nest_kinds(k, pat)
+            wrong = b"}" if kinds[-1] == "[" else b"]"
+            # opens to depth k and closes level k with the other closer
+            inner = b"".join(_open(x) for x in kinds) + b"1" + wrong + b"".join(_close(x) for x in reversed(kinds[:-1]))
+            # opens to 128, closes down to level k + 1, then level k with the other closer
+            full = nest_kinds(128, pat)[:k - 1] + kinds[-1:] + nest_kinds(128 - k, "obj") if k <= 128 else None
+            docs = [("open", inner)]
+            if full is not None:
+                wrong = b"}" if full[k - 1] == "[" else b"]"
+                docs.append(("deep", b"".join(_open(x) for x in full) + b"1" + b"".join(_close(x) for x in reversed(full[k:])) +
+                             wrong + b"".join(_close(x) for x in reversed(full[:k - 1]))))
+            for how, body in docs:
+                out.append((f"mismatch_{how}-{pat}-k{k}", body, nested(kinds[:1])))
+                out.append((f"mismatch_{how}-long-{pat}-k{k}", long_head + body + b"}", long_head + nested(kinds[:1]) + b"}"))
+    return out

@@ -352,3 +352,38 @@ def unmarshal(payload: bytes) -> dict:
         out["tcs"] = st["tcs"]
         out["tc_valid"] = any(t["id"] is not None or (t["function"] and (t["name"] or t["args"])) for t in st["tcs"])
     return out
+
+
+DEPTH_LIMIT = 128
+
+
+def depth_limited(payload: bytes, limit: int = DEPTH_LIMIT) -> bool:
+    """The product's documented nesting limit (DESIGN.md §5, deviation 2), restated independently of oracle/sse_oracle.c: True
+    when a container opens while `limit` are open, before the payload's first syntax error. The error position is the one
+    CPython's json reports; depth is a bracket count outside strings up to it. Payloads with NaN / Infinity literals (which
+    CPython reports without a position) are outside this model."""
+    s = payload.decode("utf-8", errors="surrogateescape")
+    try:
+        json.loads(s, object_pairs_hook=Obj, strict=True)
+        err = len(s)
+    except json.JSONDecodeError as e:
+        err = e.pos
+    assert "NaN" not in s and "Infinity" not in s
+    depth, in_str, esc = 0, False, False
+    for ch in s[:err]:
+        if in_str:
+            if esc:
+                esc = False
+            elif ch == "\\":
+                esc = True
+            elif ch == '"':
+                in_str = False
+        elif ch == '"':
+            in_str = True
+        elif ch in "[{":
+            if depth >= limit:
+                return True
+            depth += 1
+        elif ch in "]}":
+            depth -= 1
+    return False

@@ -177,6 +177,28 @@ def parse_streaming_tool_calls(builder: bytes):
     return [m[i] for i in range(len(m)) if i in m]
 
 
+def decoded_payloads(body: bytes, mode_r: bool):
+    """The bytes each decoded line hands to json.Unmarshal, in line order. Mode R (agent.go:169-248 up to the terminating
+    chunk): an emitted line's chunk_data; a swallowed line containing "[DONE]" as parseStreamingToolCalls (:385-402) sees it,
+    the trimmed line without its "data: " prefix, or the bare trimmed line. Mode P with parsing: line[6:len-1] of every line
+    that starts with "data: " (the telemetry tap's per-line decode)."""
+    if not mode_r:
+        return [line[6:-1] for line in lines(body) if line.startswith(b"data: ")]
+    out = []
+    for line in lines(body):
+        trimmed = trim_space(line)
+        if b"[DONE]" in trimmed:
+            out.append(trimmed[6:] if trimmed.startswith(b"data: ") else trimmed)
+            continue
+        if not trimmed.startswith(b"data: ") or trimmed[6:] == b"":
+            continue
+        out.append(trimmed[6:])
+        ck = gm.unmarshal(trimmed[6:])
+        if ck["json_ok"] and ck["n_choices"] > 0 and ck["finish"] in (gm.FIN["stop"], gm.FIN["tool_calls"]):
+            break
+    return out
+
+
 def telemetry(body: bytes):
     pieces = body.split(b"\n\n")
     usage = (0, 0, 0)

@@ -11,7 +11,7 @@ from inference_gateway_b200.gateway import Gateway
 from inference_gateway_b200.synth import random_cuts
 from oracle import orc
 from tests.corpus import TRICKY, mutate
-from tests.util import ConnOut, agent_results, check_stream, rec_to_dict, telemetry_results
+from tests.util import ConnOut, agent_results, check_stream, fold_segment, process_all_checked, process_checked, telemetry_results
 
 pytestmark = pytest.mark.gpu
 
@@ -40,20 +40,15 @@ def run_deferred(eng, bodies, modes, n_batches=1, seed=0, with_folds=False, n_fo
         stats["overflow"] |= res.overflow
         for i, c in enumerate(conns):
             o = outs[c]
-            o.frames.extend(res.seg_frames(i))
-            o.recs.extend(rec_to_dict(res, ri) for ri in res.seg_recs(i))
-            fl = int(res.segs[i]["flags"])
-            o.carry_len = int(res.segs[i]["carry_len"])
-            o.flags |= fl
-            o.terminated |= bool(fl & A.SEG_TERMINATED)
-            stats["deferred"] += bool(fl & A.SEG_DEFERRED)
+            fold_segment(o, res, i)
+            stats["deferred"] += bool(int(res.segs[i]["flags"]) & A.SEG_DEFERRED)
             if o.agent is not None:
                 A.check(L.sse_agent_feed(o.agent, C.byref(res.raw), i), "sse_agent_feed")
                 A.check(L.sse_telemetry_feed(o.tele, C.byref(res.raw), i), "sse_telemetry_feed")
 
     for b in range(max(len(p) for p in pieces)):
         items = [(c, modes[c], pieces[c][b]) for c in range(len(bodies)) if b < len(pieces[c])]
-        stats["batches"] += eng.process_all(items, on_batch)
+        stats["batches"] += process_all_checked(eng, items, on_batch)
     return outs, stats
 
 
@@ -90,7 +85,8 @@ N_C4 = 160
 
 def mixed_bodies(seed, n_c4=N_C4, n_adv=60):
     """C4 streams, then adversarial ones (nesting past the 128-level limit among them: those records are flagged
-    SSE_F_DEPTH_LIMIT and the folds refuse them, so only the C4 streams are folded)."""
+    SSE_F_DEPTH_LIMIT, which check_stream compares with the oracle's restatement of the limit, and the folds refuse them, so
+    only the C4 streams are folded)."""
     streams, _ = synth.make_config("C4", n_streams=n_c4)
     bodies = [b for b, _, _ in streams] + adversarial_bodies(np.random.default_rng(seed), n_adv)
     modes = [(P, R, PP)[i % 3] for i in range(len(bodies))]
@@ -166,7 +162,7 @@ def test_deferral_at_a_first_line_that_starts_in_the_carried_tail():
         bodies = [head + rest for _ in range(48)]
         outs = [ConnOut() for _ in bodies]
         e.reset_all()
-        slot, res = e.process([(c, PP, head) for c in range(len(bodies))])
+        slot, res = process_checked(e, [(c, PP, head) for c in range(len(bodies))])
         try:
             assert all(int(res.segs[i]["carry_len"]) == len(head) for i in range(len(bodies)))
         finally:
@@ -178,11 +174,8 @@ def test_deferral_at_a_first_line_that_starts_in_the_carried_tail():
                 fl = int(res.segs[i]["flags"])
                 if fl & A.SEG_DEFERRED and not outs[c].frames and res.consumed(i) == 0:
                     seen.append(int(res.segs[i]["carry_len"]))
-                outs[c].frames.extend(res.seg_frames(i))
-                outs[c].recs.extend(rec_to_dict(res, ri) for ri in res.seg_recs(i))
-                outs[c].carry_len = int(res.segs[i]["carry_len"])
-                outs[c].flags |= fl
-        e.process_all([(c, PP, rest) for c in range(len(bodies))], on_batch)
+                fold_segment(outs[c], res, i)
+        process_all_checked(e, [(c, PP, rest) for c in range(len(bodies))], on_batch)
         assert len(seen) >= len(bodies) - 2 and set(seen) == {len(head)}
         for i, (b, o) in enumerate(zip(bodies, outs)):
             check_stream(b, PP, o, label=f"carry stream {i}")
@@ -199,7 +192,7 @@ def test_terminating_chunk_before_deferred_bytes_finishes_the_connection():
         more = b'data: {"choices":[{"index":0,"delta":{"content":"never read"},"finish_reason":null}]}\n\n' * 100
         body = stop + more
         e.reset_all()
-        slot, res = e.process([(0, R, body)])
+        slot, res = process_checked(e, [(0, R, body)])
         try:
             fl = int(res.segs[0]["flags"])
             assert fl & A.SEG_TERMINATED and not fl & A.SEG_DEFERRED and res.consumed(0) == len(body)
@@ -207,7 +200,7 @@ def test_terminating_chunk_before_deferred_bytes_finishes_the_connection():
             assert res.seg_frames(0) == [stop]
         finally:
             e.release(slot)
-        slot, res = e.process([(0, R, more)])
+        slot, res = process_checked(e, [(0, R, more)])
         try:
             assert int(res.segs[0]["flags"]) & A.SEG_FINISHED and res.seg_frames(0) == [] and res.consumed(0) == len(more)
         finally:
@@ -241,13 +234,9 @@ def test_pooled_line_whose_completion_does_not_fit_waits_at_its_newline():
                 fl = int(res.segs[i]["flags"])
                 if fl & A.SEG_DEFERRED:
                     stops.append(res.consumed(i))
-                outs[c].frames.extend(res.seg_frames(i))
-                outs[c].recs.extend(rec_to_dict(res, ri) for ri in res.seg_recs(i))
-                outs[c].carry_len = int(res.segs[i]["carry_len"])
-                outs[c].flags |= fl
-                outs[c].terminated |= bool(fl & A.SEG_TERMINATED)
-        assert e.process_all(first, on_batch) == 1 and e.pool_stats()[0] > 0
-        n = e.process_all(second, on_batch)
+                fold_segment(outs[c], res, i)
+        assert process_all_checked(e, first, on_batch) == 1 and e.pool_stats()[0] > 0
+        n = process_all_checked(e, second, on_batch)
         # one line waited, at its '\n' (consumed 0); the other completed, and what followed it may have waited too (the failed
         # reservation left the out-arena counter past the capacity)
         assert n == 2 and stops.count(0) == 1 and all(c in (0, 1) for c in stops)
@@ -293,16 +282,13 @@ def test_line_whose_newline_would_leave_the_carry_slot_keeps_its_bytes_when_defe
                         assert taken[c] + res.consumed(i) == keep - 10000, (c, taken[c], res.consumed(i))
                         waited.add(c)
                     taken[c] += res.consumed(i)
-                outs[c].frames.extend(frames)
-                outs[c].recs.extend(rec_to_dict(res, ri) for ri in res.seg_recs(i))
-                outs[c].carry_len = int(res.segs[i]["carry_len"])
-                outs[c].flags |= fl
+                fold_segment(outs[c], res, i)
         e.reset_all()
         # 10,000 bytes without a '\\n': more than a window, so the line is assembled in the slot (not yet in the pool)
-        assert e.process_all([(c, PP, b[:10000]) for c, b in enumerate(bodies)], on_batch) == 1
+        assert process_all_checked(e, [(c, PP, b[:10000]) for c, b in enumerate(bodies)], on_batch) == 1
         assert all(o.carry_len == 10000 for o in outs) and e.pool_stats()[0] == 0
         second[0] = True
-        assert e.process_all([(c, PP, b[10000:]) for c, b in enumerate(bodies)], on_batch) >= 8
+        assert process_all_checked(e, [(c, PP, b[10000:]) for c, b in enumerate(bodies)], on_batch) >= 8
         assert len(waited) >= 7 and taken == [len(b) - 10000 for b in bodies]
         for i, (b, o) in enumerate(zip(bodies, outs)):
             check_stream(b, PP, o, label=f"keep={keep} stream {i}")

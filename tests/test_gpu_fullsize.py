@@ -70,7 +70,7 @@ def test_oracle_parity_at_full_size(engines, workload, name, n_streams, mode, n_
     assert len(bodies) == n_streams
     od, oterm, otail = oracle_digests(bodies, mode)
     gd, carry, flags = digest_run(eng, bodies, mode, cut_bounds(bodies, n_batches, seed=1000 + n_batches))
-    assert int(gd["inexact"].sum()) == 0                                   # no record left undecoded (TOO_LONG / DEPTH_LIMIT)
+    assert int(gd["inexact"].sum()) == 0                                   # no record left undecoded (TOO_LONG) or with a broken tool-call chain
     for key in ("n_frames", "frame_bytes", "frames_h", "n_recs", "recs_h"):
         bad = np.nonzero(gd[key] != od[key])[0]
         if bad.size:

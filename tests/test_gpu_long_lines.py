@@ -7,7 +7,7 @@ import pytest
 
 from inference_gateway_b200 import SseEngine, _abi as A, synth
 from oracle import orc
-from tests.util import agent_results, check_stream, run_streams, telemetry_results
+from tests.util import agent_results, check_stream, run_pieces, run_streams, telemetry_results
 
 pytestmark = pytest.mark.gpu
 
@@ -295,27 +295,6 @@ def test_long_lines_with_small_odd_pages(small_pages, length, n_batches):
     test_long_line_lengths(small_pages, length, n_batches)
 
 
-def _run_pieces(e, pieces, modes):
-    """Like run_streams, with the pieces of every connection given (empty pieces are submitted as empty segments)."""
-    from tests.util import ConnOut, rec_to_dict
-    outs = [ConnOut() for _ in pieces]
-    e.reset_all()
-    for b in range(max(map(len, pieces))):
-        who = [c for c in range(len(pieces)) if b < len(pieces[c])]
-        slot, res = e.process([(c, modes[c], pieces[c][b]) for c in who])
-        try:
-            for i, c in enumerate(who):
-                o = outs[c]
-                o.frames.extend(res.seg_frames(i))
-                o.recs.extend(rec_to_dict(res, ri) for ri in res.seg_recs(i))
-                o.carry_len = int(res.segs[i]["carry_len"])
-                o.flags |= int(res.segs[i]["flags"])
-                o.terminated |= bool(int(res.segs[i]["flags"]) & A.SEG_TERMINATED)
-        finally:
-            e.release(slot)
-    return outs
-
-
 @pytest.mark.parametrize("page", [SMALL_PAGE, PAGE], ids=["page4112", "page65536"])
 def test_empty_segments_while_a_line_is_held(page):
     """An empty segment for a connection whose held-back line fills its slot or its pages exactly (a whole number of pages,
@@ -331,12 +310,12 @@ def test_empty_segments_while_a_line_is_held(page):
             pieces = [body[:cut], b"", body[cut:cut + 5000], b"", b"", body[cut + 5000:]]
             if held % page == 0 and held > SLOT:       # the pooled prefix is a whole number of pages when the empty segment comes
                 pieces = [body[:cut], b"", b"", body[cut:]]
-            outs = _run_pieces(e, [pieces] * 3, list(MODES))
+            outs = run_pieces(e, [pieces] * 3, list(MODES))
             _check_all([body] * 3, list(MODES), outs, f"held={held} page={page}")
             assert not any(o.flags & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG) for o in outs), held
             assert e.pool_stats()[0] == 0
         # a pooled line of exactly k pages, then only empty segments: still held, its pages still owned
-        outs = _run_pieces(e, [[body[:start + 8 * page], b"", b""]], [P])
+        outs = run_pieces(e, [[body[:start + 8 * page], b"", b""]], [P])
         assert not outs[0].flags & A.SEG_DEAD and outs[0].carry_len == 8 * page
         assert e.pool_stats()[0] == 8
         e.reset_conn(0)

@@ -80,3 +80,27 @@ def test_number_rules():
     assert lp(b"-9999.0") and lp(b"3.4028234e38") and lp(b"3.40282356e38") and lp(b"1e-999")
     assert not lp(b"3.4028236e38") and not lp(b"1e39") and not lp(b"-4e38")
     assert lp(b"340282356779733661637539395458142568447") and not lp(b"340282356779733661637539395458142568448")
+
+
+def test_depth_limit_rule_matches_independent_scan():
+    """The oracle's restatement of the nesting limit (orc_json_scan at 128 levels) against a bracket count up to CPython's
+    first syntax error (tests/go_model.py::depth_limited), on the nesting corpus and on every corpus document."""
+    from tests.corpus import nesting_docs
+    docs = nesting_docs()
+    n_limited = 0
+    for name, d, twin in docs:
+        lim = orc.json_scan(d, orc.DEPTH_LIMIT) == orc.JSON_DEPTH
+        assert lim == go_model.depth_limited(d), name
+        assert not go_model.depth_limited(twin), name
+        n_limited += lim
+    for d in TRICKY:
+        assert (orc.json_scan(d, orc.DEPTH_LIMIT) == orc.JSON_DEPTH) == go_model.depth_limited(d), d
+    names = {n for n, _, _ in docs}
+    assert len(docs) > 1000 and 200 < n_limited < len(docs) - 200
+    # the shape of the rule at its edges
+    assert {n: orc.json_scan(d, orc.DEPTH_LIMIT) for n, d, _ in docs if n.startswith("top-arr")} == \
+        {"top-arr-d127": 0, "top-arr-d128": 0, "top-arr-d129": 2, "top-arr-d130": 2}
+    by = {n: orc.json_scan(d, orc.DEPTH_LIMIT) for n, d, _ in docs}
+    assert by["syntax_before-d130"] == orc.JSON_SYNTAX and by["syntax_after-d130"] == orc.JSON_DEPTH
+    assert by["mismatch_open-alt-k64"] == orc.JSON_SYNTAX and by["mismatch_open-alt-k129"] == orc.JSON_DEPTH
+    assert by["in_string-d130"] == orc.JSON_OK and "mismatch_deep-rnd-k65" in names

@@ -98,3 +98,18 @@ def test_passthrough_and_telemetry_model_match_oracle():
         assert got == sm.telemetry(v.out), body[:120]
         n_usage += got[0] != (0, 0, 0)
     assert n_usage > 50
+
+
+def test_decoded_payload_lengths_match_model():
+    """orc_line's payload span: what each decoded line hands to json.Unmarshal (sse_rec.payload_len on the GPU side)."""
+    n_done = n_exact = 0
+    for body in BODIES:
+        v = orc.reframe(body)
+        got = [ln.payload for ln in v.lines if ln.kind in (orc.L_EMITTED, orc.L_DONE, orc.L_DONE_EXACT)]
+        assert got == sm.decoded_payloads(body, True), body[:120]
+        n_done += sum(ln.kind == orc.L_DONE for ln in v.lines)
+        n_exact += sum(ln.kind == orc.L_DONE_EXACT for ln in v.lines)
+        assert all(ln.payload_len == 6 for ln in v.lines if ln.kind == orc.L_DONE_EXACT)
+        v = orc.passthrough(body, parse=True)
+        assert [ln.payload for ln in v.lines if ln.chunk is not None] == sm.decoded_payloads(body, False), body[:120]
+    assert n_done > 100 and n_exact > 0

@@ -4,6 +4,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from unittest import mock
 
 import numpy as np
 
@@ -67,14 +68,59 @@ def chunk_to_dict(ck: orc.ChunkView) -> dict:
 
 
 def fold_segment(o: ConnOut, res, i: int):
-    """Appends segment i of a batch result to its connection's output."""
-    o.frames.extend(res.seg_frames(i))
-    o.recs.extend(rec_to_dict(res, ri) for ri in res.seg_recs(i))
+    """Appends segment i of a batch result to its connection's output. A record's frame link becomes the ordinal of the linked
+    frame among the connection's frames (A.NONE: no frame; -1: a frame outside the record's own run)."""
+    for ff, fc, rf, rc in res.seg_runs(i):
+        base = len(o.frames)
+        o.frames.extend(res.at(int(f["off"]), int(f["len"])) for f in res.frames[ff:ff + fc])
+        for ri in range(rf, rf + rc):
+            d = rec_to_dict(res, ri)
+            if d["frame"] != A.NONE:
+                d["frame"] = base + d["frame"] - ff if 0 <= d["frame"] - ff < fc else -1
+            o.recs.append(d)
     sr = res.segs[i]
     o.carry_len = int(sr["carry_len"])
     o.flags |= int(sr["flags"])
     if int(sr["flags"]) & A.SEG_TERMINATED:
         o.terminated = True
+
+
+# ------------------------------------------------------------------ structural check of every batch result
+CHECKED = [0]     # batch results orc_check_result has passed in this process
+
+
+def line_limit(eng) -> int:
+    """The longest line one connection of the engine may hold: the line pool's max_line_bytes, else the carry slot."""
+    return int(eng.pool.max_line_bytes) if eng.pool is not None and eng.pool.pool_pages else int(eng.cfg.carry_slot_bytes)
+
+
+def check_result(eng, res, segs):
+    """orc_check_result on one batch result: runs, frame / record ranges, links, chains, spans, flags (oracle/orc_check.c).
+    segs: the sse_seg descriptors the batch was submitted with."""
+    n, msg = orc.check_result(res.raw, segs[:int(res.raw.n_segs)], int(eng.cfg.flags), line_limit(eng))
+    assert n == 0, f"batch result breaks {n} structural rule(s); first: {msg}"
+    CHECKED[0] += 1
+
+
+def process_checked(eng, items):
+    """SseEngine.process (acquire, fill, submit, collect) with the structural check of the result. Returns (slot, result); the
+    caller releases the slot."""
+    slot, arena, segs = eng.acquire()
+    try:
+        n, nbytes = eng.fill(arena, segs, items)
+        eng.submit(slot, n, nbytes)
+        res = eng.collect(slot)
+        check_result(eng, res, segs[:n].copy())
+    except BaseException:
+        eng.release(slot)
+        raise
+    return slot, res
+
+
+def process_all_checked(eng, items, on_batch=None) -> int:
+    """SseEngine.process_all with every batch it submits checked by process_checked."""
+    with mock.patch.object(eng, "process", lambda batch: process_checked(eng, batch)):
+        return eng.process_all(items, on_batch)
 
 
 def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False):
@@ -101,7 +147,7 @@ def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False):
                 who.append(c)
         if not items:
             continue
-        slot, res = engine.process(items)
+        slot, res = process_checked(engine, items)
         try:
             for i, c in enumerate(who):
                 o = outs[c]
@@ -111,6 +157,22 @@ def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False):
                     A.check(L.sse_telemetry_feed(o.tele, C.byref(res.raw), i), "sse_telemetry_feed")
         finally:
             engine.release(slot)
+    return outs
+
+
+def run_pieces(eng, pieces, modes):
+    """Like run_streams, with the pieces of every connection given: pieces[c][b] goes to connection c in batch b (empty pieces
+    are submitted as empty segments). Returns list[ConnOut]."""
+    outs = [ConnOut() for _ in pieces]
+    eng.reset_all()
+    for b in range(max(map(len, pieces))):
+        who = [c for c in range(len(pieces)) if b < len(pieces[c])]
+        slot, res = process_checked(eng, [(c, modes[c], pieces[c][b]) for c in who])
+        try:
+            for i, c in enumerate(who):
+                fold_segment(outs[c], res, i)
+        finally:
+            eng.release(slot)
     return outs
 
 
@@ -154,6 +216,7 @@ def digest_run(eng, bodies, modes, bounds, providers=None, on_batch=None):
         eng.submit(slot, n, int(offs[-1] + aligned[-1]))
         res = eng.collect(slot)
         try:
+            check_result(eng, res, segs[:n])
             assert orc.digest_result(res.raw, conn, d, carry, flags) == n
             if on_batch is not None:
                 on_batch(b, res)
@@ -226,31 +289,37 @@ def telemetry_results(L, fold):
     return rc, (u.prompt_tokens, u.completion_tokens, u.total_tokens), calls
 
 
+def _expect(l, frame: int, done: bool, mode_r: bool) -> dict:
+    """The record the oracle's line l should give: its decoded fields (none past the nesting limit, DESIGN.md §5 deviation 2),
+    the ordinal of its frame among the connection's frames (A.NONE: none), the bytes handed to json.Unmarshal, termination."""
+    depth = l.depth_limited
+    d = dict(json_ok=False) if depth else chunk_to_dict(l.chunk)
+    d.update(done=done, done_exact=False, depth_limit=depth, frame=frame, payload_len=l.payload_len,
+             terminates=mode_r and not done and d["json_ok"] and d["n_choices"] > 0 and d["finish"] in (orc.FIN_STOP, orc.FIN_TOOL_CALLS))
+    return d
+
+
 def check_stream(body: bytes, mode: int, o: ConnOut, label=""):
     """Bit-exact comparison of one connection's GPU output with the oracle."""
     if mode & A.MODE_R:
         v = orc.reframe(body)
         exp_frames = [l.out for l in v.lines if l.kind == orc.L_EMITTED]
         exp_recs = []
+        n_frames = 0
         for l in v.lines:
-            if l.kind == orc.L_EMITTED or l.kind == orc.L_DONE:
-                d = chunk_to_dict(l.chunk)
-                d["done"] = l.kind == orc.L_DONE
-                d["done_exact"] = False
-                exp_recs.append(d)
+            if l.kind == orc.L_EMITTED:
+                exp_recs.append(_expect(l, n_frames, False, True))
+                n_frames += 1
+            elif l.kind == orc.L_DONE:
+                exp_recs.append(_expect(l, A.NONE, True, True))
             elif l.kind == orc.L_DONE_EXACT:
-                exp_recs.append(dict(json_ok=False, done=True, done_exact=True))
+                exp_recs.append(dict(json_ok=False, done=True, done_exact=True, depth_limit=False, frame=A.NONE, payload_len=6,
+                                     terminates=False))
         assert o.terminated == v.terminated, f"{label}: terminated {o.terminated} != {v.terminated}"
     else:
         v = orc.passthrough(body, parse=bool(mode & A.MODE_PARSE))
         exp_frames = [l.out for l in v.lines]
-        exp_recs = []
-        for l in v.lines:
-            if l.chunk is not None:
-                d = chunk_to_dict(l.chunk)
-                d["done"] = False
-                d["done_exact"] = False
-                exp_recs.append(d)
+        exp_recs = [_expect(l, k, False, False) for k, l in enumerate(v.lines) if l.chunk is not None]
         assert b"".join(o.frames) == v.out, f"{label}: passthrough bytes differ"
     assert len(o.frames) == len(exp_frames), f"{label}: {len(o.frames)} frames, oracle {len(exp_frames)}"
     for i, (g, e) in enumerate(zip(o.frames, exp_frames)):
@@ -258,9 +327,6 @@ def check_stream(body: bytes, mode: int, o: ConnOut, label=""):
     assert len(o.recs) == len(exp_recs), f"{label}: {len(o.recs)} recs, oracle {len(exp_recs)}"
     for i, (g, e) in enumerate(zip(o.recs, exp_recs)):
         assert not g["too_long"], f"{label}: rec {i} was not decoded (SSE_F_TOO_LONG)"
-        if g["depth_limit"]:      # nesting deeper than 128 levels: the documented limit (DESIGN.md 6), reported as not JSON_OK
-            assert not g["json_ok"]
-            continue
         for k, ev in e.items():
             assert g[k] == ev, f"{label}: rec {i} field {k}: gpu={g[k]!r} ref={ev!r}"
     if not o.terminated and not (o.flags & A.SEG_DEAD):
