@@ -2,7 +2,8 @@
 //
 // The table-driven automaton (v2_round / v2_action / v2_finish_line): one lane per line steps a pushdown automaton over the
 // payload it reads through a 16-byte register window. Syntax, type compatibility and field capture follow json.Unmarshal into
-// CreateChatCompletionStreamResponse; keys are matched by a case-folding trie walked alongside; rare cases (escaped keys,
+// CreateChatCompletionStreamResponse; the plain bytes of strings and digit runs are taken a window at a time, and a key is matched
+// at its closing quote by a perfect hash of its case-folded bytes; rare cases (escaped keys,
 // int/float range checks) fall to the sequential helpers of sse_common.cuh; strings that need unquoting are queued and decoded
 // by the whole warp.
 //
@@ -51,7 +52,7 @@ struct TCtx {                      // per CTA, shared memory
 
 struct LaneScratch {               // cold per-lane state (usage ints, the tool-call element being assembled)
     int64_t u_prompt, u_completion, u_total, tc_index;
-    uint32_t tc_flags, tc_dec;
+    uint32_t tc_flags, tc_dec, tc_prev;   // tc_prev: the line's last tool-call record (valid once the lane's tc_first is set)
     uint32_t id_off, id_len, type_off, type_len, name_off, name_len, args_off, args_len;
     TRec *recp;                    // the automaton records this line's wildcards here (nullptr: not recording)
     uint32_t rec, frame, slot, plen;   // the work item: record index, frame index, segment, payload length (read at the line's end only)
@@ -65,16 +66,16 @@ __device__ __forceinline__ void rec_event(LaneScratch &S, uint32_t kind, uint32_
 template <bool REC>
 __device__ __forceinline__ void rec_nonsimple(LaneScratch &S) { if (REC && S.recp) S.recp->nonsimple = 1; }
 // per-string flags (cleared outside strings) and per-line flags
-constexpr uint32_t SF_ESC = 1, SF_HI = 2, SF_UPPER = 4, SF_BAD = 8, SF_STRMASK = 15;
+constexpr uint32_t SF_ESC = 1, SF_HI = 2, SF_BAD = 8, SF_STRMASK = SF_ESC | SF_HI | SF_BAD;
 constexpr uint32_t SF_SYN = 0x100, SF_TYPE = 0x200, SF_DEPTH = 0x400, SF_GBAD = 0x800, SF_USAGE = 0x1000,
                    SF_TCNONNIL = 0x2000, SF_TCOPEN = 0x4000, SF_TCVALID = 0x8000, SF_CDEC = 0x10000, SF_RMODE = 0x20000, SF_CBAD = 0x40000, SF_CSET = 0x80000, SF_DONELINE = 0x100000;
 
 struct Lane {
     uint32_t p, pe;                // out-arena offsets of the payload being decoded
     uint4 win;                     // the 16 bytes containing p
-    uint32_t st, depth, skip, sd, cur, km, slen, sf, choices_count, n_choices, finish;
+    uint32_t st, depth, skip, sd, cur, slen, sf, choices_count, n_choices, finish;
     unsigned long long ct, ct1, sstk;   // container-type bit stack (1 = array), 128 levels
-    uint32_t content_off, content_len, tc_count, tc_first, tc_prev;
+    uint32_t content_off, content_len, tc_count, tc_first;
     bool busy;
 };
 
@@ -97,6 +98,21 @@ __device__ __forceinline__ void value_done(Lane &L) {
     const uint32_t d = L.depth - 1;
     const unsigned long long bits = d < 64 ? L.ct : L.ct1;
     L.st = ((bits >> (d & 63u)) & 1ull) ? (uint32_t)S_AFTA : (uint32_t)S_AFTO;
+}
+
+__device__ __forceinline__ uint32_t gload4(const uint8_t *base, uint32_t off) {
+    const uint32_t *w = reinterpret_cast<const uint32_t *>(base + (off & ~3u));
+    return __funnelshift_r(__ldg(w), __ldg(w + 1), (off & 3u) * 8u);
+}
+// 0x80 in every byte that is not '0'..'9' (exact for the lowest flagged byte only: a byte >= 0x80 may flag the one above it)
+__device__ __forceinline__ uint32_t nondigit4(uint32_t w4) {
+    return (~((w4 | 0x80808080u) - 0x30303030u) | (w4 + 0x46464646u) | w4) & 0x80808080u;
+}
+// name id of the unescaped string body [s, s + n) of the payload arena (name_lookup), | 0x100 when it has an upper-case letter
+__device__ __noinline__ uint32_t body_name(const uint8_t *base, const DfaTables &T, uint32_t s, uint32_t n) {
+    bool upper = false;
+    const uint32_t id = name_lookup(T, n, [&](uint32_t i) { return gload4(base, s + i); }, upper);
+    return id | (upper ? 0x100u : 0u);
 }
 
 // Span of a captured string: without escapes it is the payload's own bytes (no call, nothing through local memory); the
@@ -125,8 +141,8 @@ __device__ void v2_flush_tc(const KParams &P, Lane &L, LaneScratch &S, LaneJobs 
     o.id_off = id.off; o.id_len = id.len; o.type_off = ty.off; o.type_len = ty.len;
     o.name_off = nm.off; o.name_len = nm.len; o.args_off = ar.off; o.args_len = ar.len;
     *rec = o;            // queued unquote jobs overwrite the *_len fields when the warp drains them
-    if (L.tc_first == SSE_NONE) L.tc_first = idx; else P.tcs[L.tc_prev].next = idx;
-    L.tc_prev = idx;
+    if (L.tc_first == SSE_NONE) L.tc_first = idx; else P.tcs[S.tc_prev].next = idx;
+    S.tc_prev = idx;
 }
 
 __device__ void v2_elem_begin(const KParams &P, Lane &L, LaneScratch &S, LaneJobs *J) {
@@ -157,11 +173,11 @@ __device__ void v2_null(Lane &L, LaneScratch &S) {
     case TG_CHOICES:
         L.n_choices = 0; L.choices_count = 0; L.finish = SSE_FIN_NONE; L.content_off = L.content_len = 0;
         L.sf &= ~(SF_CDEC | SF_CBAD | SF_CSET | SF_TCNONNIL | SF_TCOPEN | SF_TCVALID);
-        L.tc_count = 0; L.tc_first = L.tc_prev = SSE_NONE;
+        L.tc_count = 0; L.tc_first = SSE_NONE;
         break;
     case TG_USAGE: L.sf &= ~SF_USAGE; S.u_prompt = S.u_completion = S.u_total = 0; break;
     case TG_TOOLCALLS:
-        if (lane_live(L)) { L.sf &= ~(SF_TCNONNIL | SF_TCOPEN | SF_TCVALID); L.tc_count = 0; L.tc_first = L.tc_prev = SSE_NONE; }
+        if (lane_live(L)) { L.sf &= ~(SF_TCNONNIL | SF_TCOPEN | SF_TCVALID); L.tc_count = 0; L.tc_first = SSE_NONE; }
         break;
     case TG_TC_ID: if ((L.sf & SF_TCOPEN) && lane_live(L)) { S.tc_flags &= ~SSE_TC_HAS_ID; S.id_off = S.id_len = 0; S.tc_dec &= ~3u; } break;
     case TG_TC_TYPE: if ((L.sf & SF_TCOPEN) && lane_live(L)) { S.tc_flags &= ~SSE_TC_HAS_TYPE; S.type_off = S.type_len = 0; S.tc_dec &= ~12u; } break;
@@ -228,7 +244,7 @@ __device__ bool v2_action(const KParams &P, const DfaTables &T, Lane &L, LaneScr
                     else if (tgt == TG_CHOICES) { if (L.n_choices || L.choices_count) rec_nonsimple<REC>(S); L.choices_count = 0; }
                     else if (tgt == TG_TOOLCALLS) {
                         if (live && (L.sf & SF_TCNONNIL)) rec_nonsimple<REC>(S);
-                        if (live) { L.sf = (L.sf | SF_TCNONNIL) & ~(SF_TCOPEN | SF_TCVALID); L.tc_count = 0; L.tc_first = L.tc_prev = SSE_NONE; }
+                        if (live) { L.sf = (L.sf | SF_TCNONNIL) & ~(SF_TCOPEN | SF_TCVALID); L.tc_count = 0; L.tc_first = SSE_NONE; }
                     }
                 }
                 if (sub == N_GOOGLE) L.sf &= ~SF_GBAD;
@@ -260,10 +276,10 @@ __device__ bool v2_action(const KParams &P, const DfaTables &T, Lane &L, LaneScr
                 int f = (n <= 64) ? match_field(c_schema, (int)node, tmp, (int)n) : -1;
                 if (f >= 0) cur = c_schema.f[f].ty | ((uint32_t)c_schema.f[f].sub << 4) | ((uint32_t)c_schema.f[f].tgt << 9);
             } else {
-                const uint32_t name = T.accept[L.km];
+                const uint32_t nm = body_name(P.out, T, L.p - L.slen, L.slen), name = nm & 0xFFu;
                 if (name != 0xFFu) {
                     uint32_t f = T.field[node * NNAMES + name];
-                    if ((f & FIELD_VALID) && !(node == N_GOOGLE && (L.sf & SF_UPPER))) cur = f & 0x1FFFu;
+                    if ((f & FIELD_VALID) && !(node == N_GOOGLE && (nm & 0x100u))) cur = f & 0x1FFFu;
                 }
             }
         }
@@ -291,9 +307,10 @@ __device__ bool v2_action(const KParams &P, const DfaTables &T, Lane &L, LaneScr
                 case TG_FINISH:
                     if (len == 0) L.finish = SSE_FIN_NONE;
                     else if (!d2) {
-                        // the trie folds ASCII case (it matches keys); finish_reason values compare exactly, and all are lower-case
-                        uint32_t nm = (L.sf & SF_UPPER) ? 0xFFu : T.accept[L.km];
-                        uint32_t fv = nm != 0xFFu ? T.finmap[nm] : 0xFFu; L.finish = fv != 0xFFu ? fv : (uint32_t)SSE_FIN_OTHER;
+                        // the lookup folds ASCII case (it matches keys); finish_reason values compare exactly, and all are lower-case
+                        const uint32_t nm = body_name(P.out, T, start, len);      // 0x1xx: upper-case, no finish value
+                        const uint32_t fv = nm < 0xFFu ? T.finmap[nm] : 0xFFu;
+                        L.finish = fv != 0xFFu ? fv : (uint32_t)SSE_FIN_OTHER;
                     }
                     else {
                         uint8_t tmp[40];
@@ -429,17 +446,22 @@ __device__ __forceinline__ void coop_string_skip(const KParams &P, Lane &L, unsi
 template <bool RO, bool REC>
 __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, Lane &L, LaneScratch &S, LaneJobs *J, const uint32_t coop_max) {
     uint32_t pend = 0;                       // action | cls << 8 | in_str << 16 | in_tok << 17
-    // phase A (once per round, only the lanes inside a long string value): jump to the next '"', '\\', control or non-ASCII
-    // byte, up to SKIPW windows. Keeping it out of the step loop means a warp whose lanes are not all in the same phase
-    // executes this path once per round, not once per step.
-    bool more = false;                       // still inside the plain bytes of the string after SKIPW windows
-    if (L.p < L.pe && L.st == S_VSTR && L.km == TRIE_DEAD) {
+    // phase A (once per round, only the lanes inside a string or a digit run): jump over the plain bytes -- to the next '"',
+    // '\\', control or non-ASCII byte of a key or value string, or to the next non-digit of an integer, fraction or exponent --
+    // up to SKIPW windows. The automaton would walk those bytes without changing its state or flags; the key's or value's
+    // bytes are read again where its end needs them (A_KEY_END, finish_reason). Keeping it out of the step loop means a warp
+    // whose lanes are not all in the same phase executes this path once per round, not once per step.
+    bool more = false;                       // still inside the plain bytes of a string after SKIPW windows
+    const bool str_run = L.st == S_VSTR || L.st == S_KSTR;
+    if (L.p < L.pe && (str_run || L.st == S_NINT || L.st == S_NFRAC || L.st == S_NEXP)) {
         int w = 0;
         #pragma unroll 1
         for (; w < SKIPW; w++) {
             const uint32_t i = L.p & 15u;
-            const uint32_t s0 = special_mask4(L.win.x), s1 = special_mask4(L.win.y), s2 = special_mask4(L.win.z), s3 = special_mask4(L.win.w);
-            if (i == 0 && (s0 | s1 | s2 | s3) == 0 && L.p + 16u <= L.pe) {      // a whole window of plain string bytes
+            uint32_t s0, s1, s2, s3;
+            if (str_run) { s0 = special_mask4(L.win.x); s1 = special_mask4(L.win.y); s2 = special_mask4(L.win.z); s3 = special_mask4(L.win.w); }
+            else { s0 = nondigit4(L.win.x); s1 = nondigit4(L.win.y); s2 = nondigit4(L.win.z); s3 = nondigit4(L.win.w); }
+            if (i == 0 && (s0 | s1 | s2 | s3) == 0 && L.p + 16u <= L.pe) {      // a whole window of plain bytes
                 L.p += 16u; L.slen += 16u;
                 if (L.p >= L.pe) break;
                 L.win = ldwin16<RO>(P.out, L.p);
@@ -455,7 +477,7 @@ __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, L
             if ((L.p & 15u) != 0 || L.p >= L.pe) break;     // stopped at a special byte or at the end of the payload
             L.win = ldwin16<RO>(P.out, L.p);
         }
-        more = w == SKIPW;
+        more = str_run && w == SKIPW;
     }
     if (SSE_COOP) {
         const unsigned mm = __ballot_sync(FULL, more);
@@ -474,7 +496,6 @@ __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, L
             const bool in_str = L.st >= S_KSTR, in_tok = L.st >= S_NMINUS;
             const uint32_t t = T.tr[L.st * NCLS + cls];
             if (t < A_FIRST) {
-                L.km = in_str ? (uint32_t)T.kt[L.km * NSYM + ((e >> 8) & 31u)] : (uint32_t)TRIE_ROOT;
                 L.sf = in_str ? (L.sf | (e >> 13)) : (L.sf & ~SF_STRMASK);
                 L.slen = in_tok ? L.slen + 1 : 0;
                 L.st = t;
@@ -492,7 +513,6 @@ __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, L
             if (t < A_FIRST) { L.st = t; break; }
         }
         const bool in_str = (pend & 0x10000u) != 0;
-        L.km = in_str ? (uint32_t)TRIE_DEAD : (uint32_t)TRIE_ROOT;
         const uint32_t nf = (cls == C_BSLASH ? SF_ESC : 0u) | (cls >= C_H80 ? SF_HI : 0u);
         L.sf = in_str ? (L.sf | nf) : (L.sf & ~SF_STRMASK);
         L.slen = (pend & 0x20000u) ? L.slen + 1 : 0;
@@ -524,13 +544,6 @@ constexpr int V3_WARPS = SSE_V3_WARPS;
 //   then the runs (each starts on a word)
 constexpr uint32_t T_LIT_MAX = 1024, TF_HAS_USAGE = 1, TF_SIMPLE = 2, T_HDR = 6;
 
-__device__ __forceinline__ uint32_t gload4(const uint8_t *base, uint32_t off) {
-    const uint32_t *w = reinterpret_cast<const uint32_t *>(base + (off & ~3u));
-    return __funnelshift_r(__ldg(w), __ldg(w + 1), (off & 3u) * 8u);
-}
-__device__ __forceinline__ uint32_t nondigit4(uint32_t w4) {      // 0x80 in every byte that is not '0'..'9'
-    return (~((w4 | 0x80808080u) - 0x30303030u) | (w4 + 0x46464646u) | w4) & 0x80808080u;
-}
 // body of a string value from fp (just behind the opening quote): position of the closing quote, or SSE_NONE when the body
 // is not well formed (control byte, bad escape, no closing quote). d2: bit 0 escapes, bit 1 invalid UTF-8.
 // 0x80 in some byte of w iff w holds a '"', a '\\', a byte < 0x20 or a byte >= 0x80 (which byte: special_mask4)
@@ -832,8 +845,8 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
     const uint32_t coop_max = batch < 32u ? 32u : (uint32_t)SSE_COOP;      // see coop_string_skip
 
     Lane L; L.busy = false; L.p = L.pe = 0; L.win = make_uint4(0, 0, 0, 0);
-    L.st = S_END; L.depth = L.skip = L.sd = 0; L.cur = 0; L.km = TRIE_ROOT; L.slen = 0; L.sf = 0; L.choices_count = L.n_choices = 0;
-    L.finish = 0; L.ct = L.ct1 = L.sstk = 0; L.content_off = L.content_len = 0; L.tc_count = 0; L.tc_first = L.tc_prev = SSE_NONE;
+    L.st = S_END; L.depth = L.skip = L.sd = 0; L.cur = 0; L.slen = 0; L.sf = 0; L.choices_count = L.n_choices = 0;
+    L.finish = 0; L.ct = L.ct1 = L.sstk = 0; L.content_off = L.content_len = 0; L.tc_count = 0; L.tc_first = SSE_NONE;
     S.rec = S.frame = S.slot = S.plen = 0;
 
     for (;;) {
@@ -847,10 +860,10 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
             const uint4 it = P.items_sorted[idx];
             L.p = it.x; S.plen = it.y & 0x00FFFFFFu; L.pe = it.x + S.plen; S.rec = it.z; S.slot = it.w;   // slot: segment index
             S.frame = P.recs[it.z].frame;
-            L.st = S_VAL; L.depth = L.skip = L.sd = 0; L.cur = TY_ROOT | (N_ROOT << 4); L.km = TRIE_ROOT; L.slen = 0;
+            L.st = S_VAL; L.depth = L.skip = L.sd = 0; L.cur = TY_ROOT | (N_ROOT << 4); L.slen = 0;
             L.sf = ((it.y & 0x80000000u) ? SF_RMODE : 0u) | ((it.y & 0x40000000u) ? SF_DONELINE : 0u);
             L.choices_count = L.n_choices = 0; L.finish = SSE_FIN_NONE; L.ct = L.ct1 = L.sstk = 0;
-            L.content_off = L.content_len = 0; L.tc_count = 0; L.tc_first = L.tc_prev = SSE_NONE;
+            L.content_off = L.content_len = 0; L.tc_count = 0; L.tc_first = SSE_NONE;
             S.u_prompt = S.u_completion = S.u_total = 0;
             S.recp = nullptr;
             L.busy = true;
@@ -873,7 +886,7 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
             const bool full = toff && !simple;
             if (__any_sync(FULL, full)) {              // usage / tool-call / range-check ops: a second walk runs them
                 if (full) {
-                    L.tc_count = 0; L.tc_first = L.tc_prev = SSE_NONE; L.finish = SSE_FIN_NONE; L.content_off = L.content_len = 0;
+                    L.tc_count = 0; L.tc_first = SSE_NONE; L.finish = SSE_FIN_NONE; L.content_off = L.content_len = 0;
                     L.sf &= ~(SF_CDEC | SF_CBAD);
                     if ((Tm[1] >> 16) & TF_HAS_USAGE) L.sf |= SF_USAGE;
                 }

@@ -1,5 +1,5 @@
 // sse_tables.h -- lookup tables of the v2 decoder: a byte-class table, the JSON pushdown automaton's transition
-// table (scanner.go grammar + utf8.DecodeRune validity), a case-folding trie over every struct-tag name of
+// table (scanner.go grammar + utf8.DecodeRune validity), a perfect hash over every struct-tag name of
 // providers/types/common_types.go (:271-297,:300-346,:349-371,:384-393,:451-478,:686-698) plus the finish_reason
 // values (:33-39), and the (struct, name) -> field table. Built on the host at sse_init, copied to shared memory
 // by each CTA. This is the "table-driven field map" of the design: all 11 providers use the identity table
@@ -35,11 +35,9 @@ enum : uint8_t {
     C_H80, C_H90, C_HA0, C_HC2, C_HE0, C_HE1, C_HED, C_HF0, C_HF1, C_HF4, C_HINV,
     NCLS
 };
-constexpr int NSYM = 28;          // a-z, '_', other
-constexpr int SYM_OTHER = 27;
-constexpr int NTRIE = 320;        // >= number of trie nodes (checked at build time)
-constexpr uint16_t TRIE_DEAD = 0, TRIE_ROOT = 1;
-constexpr uint16_t CLS_ESC = 0x2000, CLS_HI = 0x4000, CLS_UPPER = 0x8000;   // clssym flags: backslash, byte >= 0x80, ASCII upper-case (>> 13 gives the per-string flag bits)
+constexpr uint16_t CLS_ESC = 0x2000, CLS_HI = 0x4000;   // clssym flags: backslash, byte >= 0x80 (>> 13 gives the per-string flag bits)
+constexpr int NAME_WORDS = 5, NAME_LEN_MAX = 4 * NAME_WORDS;   // longest name: 20 bytes
+constexpr int NHASH_BITS = 7;
 
 // schema enums (same values as sse_common.cuh)
 enum : uint8_t { TTY_SKIP, TTY_STR, TTY_PSTR, TTY_INT, TTY_F32, TTY_STRUCT, TTY_PSTRUCT, TTY_SLICE, TTY_PSLICE,
@@ -49,18 +47,59 @@ constexpr int NNAMES = 40;
 constexpr uint16_t FIELD_VALID = 0x8000;   // field entry: ty | sub << 4 | tgt << 9 | FIELD_VALID
 
 struct DfaTables {
-    uint16_t clssym[256];              // class | sym << 8 | CLS_UPPER
-    uint8_t  tr[NST * NCLS + 3];       // next state or action
-    uint16_t kt[NTRIE * NSYM];         // trie transitions
-    uint8_t  accept[NTRIE];            // name id at a terminal node, 0xFF otherwise
-    uint16_t field[N_NODES * NNAMES];  // (node, name) -> packed field
-    uint8_t  finmap[NNAMES];           // name id -> SSE_FIN_* (0xFF: not a finish_reason value)
-    uint8_t  pad[8];
+    uint32_t nword[NNAMES][NAME_WORDS];  // name bytes, zero padded
+    uint32_t nhash_mul;                  // name_hash multiplier
+    uint16_t clssym[256];                // class | CLS_ESC | CLS_HI
+    uint8_t  tr[NST * NCLS + 3];         // next state or action
+    uint16_t field[N_NODES * NNAMES];    // (node, name) -> packed field
+    uint8_t  nhash[1 << NHASH_BITS];     // name_hash slot -> name id (0xFF: empty)
+    uint8_t  nlen[NNAMES];               // name length
+    uint8_t  finmap[NNAMES];             // name id -> SSE_FIN_* (0xFF: not a finish_reason value)
 };
+
+#ifdef __CUDACC__
+#define SSETAB_HD __host__ __device__ __forceinline__
+#else
+#define SSETAB_HD inline
+#endif
+// Names are looked up by a perfect hash of (first four bytes with ASCII letters lower-cased, length), then compared word by
+// word with the folded bytes of the key or finish_reason value.
+SSETAB_HD uint32_t name_hash(uint32_t mul, uint32_t w0, uint32_t len) { return (w0 * mul + len * 0x9E3779B1u) >> (32 - NHASH_BITS); }
+// w with 'A'..'Z' lower-cased; up collects 0x80 in each byte that was upper-case. Bytes >= 0x80 are left alone.
+SSETAB_HD uint32_t fold_ascii4(uint32_t w, uint32_t &up) {
+    const uint32_t x = w & 0x7F7F7F7Fu;
+    const uint32_t u = (x + 0x3F3F3F3Fu) & ~(x + 0x25252525u) & ~w & 0x80808080u;
+    up |= u;
+    return w | (u >> 2);
+}
+// Name id of an n-byte string body with its ASCII letters case-folded (0xFF: none); upper: the body has an ASCII upper-case
+// letter. load4(i) gives body bytes i..i+3 as a little-endian word (what lies past the body does not matter). The body has no
+// escapes. Names are [a-z_] only, so a match without upper-case letters is an exact match.
+template <class Load4>
+SSETAB_HD uint32_t name_lookup(const DfaTables &T, uint32_t n, Load4 load4, bool &upper) {
+    if (n == 0 || n > (uint32_t)NAME_LEN_MAX) return 0xFFu;
+    uint32_t up = 0, w = load4(0u);
+    if (n < 4u) w &= (1u << (n * 8u)) - 1u;
+    const uint32_t k = fold_ascii4(w, up);
+    const uint32_t id = T.nhash[name_hash(T.nhash_mul, k, n)];
+    if (id == 0xFFu || T.nlen[id] != n) return 0xFFu;
+    uint32_t diff = k ^ T.nword[id][0];
+#ifdef __CUDA_ARCH__
+    #pragma unroll 1
+#endif
+    for (uint32_t i = 4; i < n; i += 4u) {
+        w = load4(i);
+        if (n - i < 4u) w &= (1u << ((n - i) * 8u)) - 1u;
+        diff |= fold_ascii4(w, up) ^ T.nword[id][i >> 2];
+    }
+    upper = up != 0;
+    return diff ? 0xFFu : id;
+}
 
 struct FieldSrc { uint8_t node; const char *name; uint8_t ty, sub, tgt; };
 
-// Returns 0 on success. `fields` is the schema (node, name, ty, sub, tgt); `fin` maps finish values.
+// Returns 0 on success. `fields` is the schema (node, name, ty, sub, tgt); `fin` maps finish values. Every name is [a-z_]
+// and at most NAME_LEN_MAX bytes long.
 inline int build_tables(DfaTables &T, const FieldSrc *fields, int n_fields, const char *const *fin_names,
                         const uint8_t *fin_vals, int n_fin) {
     memset(&T, 0, sizeof T);
@@ -85,11 +124,7 @@ inline int build_tables(DfaTables &T, const FieldSrc *fields, int n_fields, cons
         else if (c == 0xE0) k = C_HE0; else if (c == 0xED) k = C_HED; else if (c >= 0xE1 && c <= 0xEF) k = C_HE1;
         else if (c == 0xF0) k = C_HF0; else if (c >= 0xF1 && c <= 0xF3) k = C_HF1; else if (c == 0xF4) k = C_HF4;
         else if (c >= 0x80) k = C_HINV;
-        uint16_t sym = SYM_OTHER, up = 0;
-        if (c >= 'a' && c <= 'z') sym = (uint16_t)(c - 'a');
-        else if (c >= 'A' && c <= 'Z') { sym = (uint16_t)(c - 'A'); up = CLS_UPPER; }
-        else if (c == '_') sym = 26;
-        T.clssym[c] = (uint16_t)(k | (sym << 8) | up | (k == C_BSLASH ? CLS_ESC : 0) | (k >= C_H80 ? CLS_HI : 0));
+        T.clssym[c] = (uint16_t)(k | (k == C_BSLASH ? CLS_ESC : 0) | (k >= C_H80 ? CLS_HI : 0));
     }
     // ---------------- automaton
     auto set = [&](int s, int c, uint8_t v) { T.tr[s * NCLS + c] = v; };
@@ -149,41 +184,42 @@ inline int build_tables(DfaTables &T, const FieldSrc *fields, int n_fields, cons
     set(S_T1, C_r, S_T2); set(S_T2, C_u, S_T3); set(S_T3, C_e, A_LIT_TRUE);
     set(S_F1, C_a, S_F2); set(S_F2, C_l, S_F3); set(S_F3, C_s, S_F4); set(S_F4, C_e, A_LIT_FALSE);
     set(S_N1, C_u, S_N2); set(S_N2, C_l, S_N3); set(S_N3, C_l, A_LIT_NULL);
-    // ---------------- names: trie + field table
+    // ---------------- names: hash + field table
     const char *names[NNAMES]; int n_names = 0;
     auto name_id = [&](const char *s) {
         for (int i = 0; i < n_names; i++) if (!strcmp(names[i], s)) return i;
-        if (n_names >= NNAMES) return -1;
+        const size_t n = strlen(s);
+        if (n_names >= NNAMES || n == 0 || n > (size_t)NAME_LEN_MAX) return -1;
+        for (const char *p = s; *p; p++) if (!((*p >= 'a' && *p <= 'z') || *p == '_')) return -1;
         names[n_names] = s;
+        memcpy(T.nword[n_names], s, n);        // little-endian words, as the device loads them
+        T.nlen[n_names] = (uint8_t)n;
         return n_names++;
     };
-    memset(T.accept, 0xFF, sizeof T.accept);
     memset(T.finmap, 0xFF, sizeof T.finmap);
-    int n_nodes = 2;   // 0 dead, 1 root
-    auto insert = [&](const char *s, int id) {
-        int cur = TRIE_ROOT;
-        for (const char *p = s; *p; p++) {
-            int sym = (*p == '_') ? 26 : (*p >= 'a' && *p <= 'z') ? *p - 'a' : -1;
-            if (sym < 0) return -1;
-            uint16_t &nx = T.kt[cur * NSYM + sym];
-            if (nx == TRIE_DEAD) { if (n_nodes >= NTRIE) return -1; nx = (uint16_t)n_nodes++; }
-            cur = nx;
-        }
-        T.accept[cur] = (uint8_t)id;
-        return 0;
-    };
     for (int i = 0; i < n_fields; i++) {
         int id = name_id(fields[i].name);
-        if (id < 0 || insert(fields[i].name, id) != 0) return -1;
+        if (id < 0) return -1;
         T.field[fields[i].node * NNAMES + id] =
             (uint16_t)(fields[i].ty | (fields[i].sub << 4) | (fields[i].tgt << 9) | FIELD_VALID);
     }
     for (int i = 0; i < n_fin; i++) {
         int id = name_id(fin_names[i]);
-        if (id < 0 || insert(fin_names[i], id) != 0) return -1;
+        if (id < 0) return -1;
         T.finmap[id] = fin_vals[i];
     }
-    return 0;
+    // perfect hash: the first odd multiplier under which the names fall into distinct slots
+    uint32_t mul = 0x9E3779B1u;
+    for (int tries = 0; tries < 100000 && !T.nhash_mul; tries++, mul += 0x632BE5ABu * 2u) {
+        memset(T.nhash, 0xFF, sizeof T.nhash);
+        bool ok = true;
+        for (int i = 0; i < n_names && ok; i++) {
+            const uint32_t h = name_hash(mul, T.nword[i][0], T.nlen[i]);
+            if (T.nhash[h] != 0xFF) ok = false; else T.nhash[h] = (uint8_t)i;
+        }
+        if (ok) T.nhash_mul = mul;
+    }
+    return T.nhash_mul ? 0 : -1;
 }
 
 } // namespace ssetab
