@@ -8,6 +8,7 @@
  *   ssegw_recv                      `line, ok := <-streamCh` (api/routes.go:602-606, mcp/agent.go:171)
  *   ssegw_agent_recv and friends    mcp.Agent.RunWithStream for one iteration (mcp/agent.go:126-290, final [DONE] :140-143)
  *   ssegw_proxy_stream / _step    handleStreamingRequest, the raw /proxy/:provider/... stream loop (api/routes.go:129-232)
+ *   ssegw_counters                  what the device did for the collected batches (SSE_FLAG_COUNTERS), for export as metrics
  *   ssegw_mcp_writer_step           one turn of handleMCPStreamingRequest's writer (api/middlewares/mcp.go:253-299): the
  *                                   terminal-frame rule (:261-268) and the upstream-error sniff that may set 503 (:272-280)
  */
@@ -43,6 +44,10 @@ sse_bytes ssegw_agent_content(ssegw *g, int stream);
 int    ssegw_agent_has_tool_calls(ssegw *g, int stream);
 int    ssegw_agent_terminated(ssegw *g, int stream, int *finish);
 size_t ssegw_agent_tool_calls(ssegw *g, int stream, sse_tool_call *calls, size_t cap);
+/* SSE_FLAG_COUNTERS: the sse_counters of every batch this gateway has collected, added up (d_items_per_pull: the last batch's),
+ * e.g. for export as monotonic counters. SSE_ERR_ARG unless the gateway was made by ssegw_new_cfg with a config that has the
+ * flag, or when out->struct_size != sizeof(sse_counters). */
+int    ssegw_counters(ssegw *g, sse_counters *out);
 
 /* The raw proxy stream handler (api/routes.go:129-232, taken when Accept is exactly text/event-stream, :118): reader and
  * writer in one loop, no channel in between. ssegw_proxy_stream opens the upstream body as a mode P stream (fed through

@@ -85,6 +85,9 @@ typedef struct {
                                     submits the rest (in[consumed:]) for that connection in a later batch, before any newer bytes.
                                   - tool calls / usages / decoded text: sse_collect grows the slot's arenas and decodes the batch again.
                                   sse_result.overflow reports the SSE_OVF_* bits of what was deferred or grown. Not with SSE_FLAG_KERNEL_FUSED. */
+#define SSE_FLAG_COUNTERS 256u /* run counting instantiations of the produce, decode and finalize kernels and keep a block of counters per
+                                  slot (sse_counters_read): what the kernels did for the batch. Results are identical; the counting
+                                  kernels are slower (DESIGN.md 4.3). Not with SSE_FLAG_KERNEL_FUSED. */
 
 /* One segment = the bytes read from ONE connection since the previous batch. in_off is 16-byte aligned. */
 typedef struct {
@@ -263,6 +266,63 @@ int sse_upload(sse_ctx *ctx, int slot, uint32_t n_segs, uint32_t in_bytes, void 
 int sse_launch(sse_ctx *ctx, int slot, uint32_t n_segs, void *cuda_stream);   /* kernels only */
 int sse_download(sse_ctx *ctx, int slot, sse_result *res, void *cuda_stream); /* D2H + sync */
 int sse_launch_count(sse_ctx *ctx, uint64_t *kernel_launches);                /* kernels launched so far */
+
+/* ---- SSE_FLAG_COUNTERS: what the kernels did for one batch ----
+ * Sums over the batch, in this order. Lines, frames and items count what the batch's results hold; bytes are payload or
+ * frame bytes. The c_* fields are clock64() cycles of the counting decode kernel summed over its warps: they show how its time
+ * divides, not the time of the default kernels, which run without the counting statements. */
+typedef struct {
+    uint32_t struct_size;          /* sizeof(sse_counters) */
+    uint32_t decode_passes;        /* decode launches behind the records (SSE_FLAG_DEFER: 1 + passes after the arenas grew) */
+    /* produce stage (and the finalize stage's page returns) */
+    uint64_t p_segments;           /* segments the produce kernel took a ticket for */
+    uint64_t p_segments_skipped;   /* segments of finished or dead connections (bytes not read) */
+    uint64_t p_windows;            /* windows staged into shared memory */
+    uint64_t p_window_bytes;       /* their bytes: carried tail plus segment bytes */
+    uint64_t p_rounds;             /* line rounds (each round's allocation) */
+    uint64_t p_lines;              /* complete lines ('\n' found) */
+    uint64_t p_frames_zero_copy;   /* frames returned as spans of the input arena */
+    uint64_t p_frames_materialised;/* frames written to the out arena */
+    uint64_t p_bytes_materialised; /* their lengths (without alignment padding) */
+    uint64_t p_items;              /* decode work items written */
+    uint64_t p_long_lines;         /* lines completed outside the window (carry slot or line pool) */
+    uint64_t p_pool_pages_taken;   /* line-pool pages taken */
+    uint64_t p_pool_pages_returned;/* line-pool pages returned (completed, failed or finished lines) */
+    uint64_t p_deferred_rounds;    /* SSE_FLAG_DEFER: rounds that did not fit and were left for a later batch */
+    /* decode stage: the pass whose records the batch returns */
+    uint64_t d_items;              /* work items decoded */
+    uint64_t d_pulls;              /* pulls of work items by a warp */
+    uint64_t d_items_per_pull;     /* items per pull the launch chose (8, 16 or 32; not a sum: ssegw_counters keeps the last) */
+    uint64_t d_warp_rounds;        /* automaton rounds executed per warp */
+    uint64_t d_busy_lane_rounds;   /* sum of the lanes busy with a line over those rounds (<= 32 * d_warp_rounds) */
+    uint64_t d_skip_windows;       /* 16-byte windows a lane examined while skipping the plain bytes of strings and digit runs */
+    uint64_t d_skip_bytes;         /* payload bytes those skips took */
+    uint64_t d_coop_strings;       /* long strings the whole warp finished for a lane */
+    uint64_t d_coop_steps;         /* 512-byte steps of the warp over them */
+    uint64_t d_coop_bytes;         /* payload bytes they took */
+    uint64_t d_plain_steps;        /* automaton steps without an action (one byte each) */
+    uint64_t d_actions;            /* actions run (one byte each) */
+    uint64_t d_action_redos;       /* extra action calls for a byte looked up again in a new state */
+    uint64_t d_abandoned_bytes;    /* bytes jumped over after a syntax or depth error */
+    uint64_t d_template_lines;     /* SSE_FLAG_TEMPLATES: lines retired by a template */
+    uint64_t d_template_bytes;     /* their payload bytes */
+    uint64_t d_template_misses;    /* lines that tried a template and went to the automaton */
+    uint64_t d_unquote_jobs;       /* strings unquoted by the whole warp */
+    uint64_t d_unquote_bytes;      /* their source bytes */
+    uint64_t d_lines_finished;     /* records written by the decode kernel */
+    uint64_t c_total;              /* cycles from a warp's first pull to its exit */
+    uint64_t c_pull;               /* taking work items: ticket, item loads, template lookup */
+    uint64_t c_skip;               /* skipping plain bytes lane by lane */
+    uint64_t c_coop;               /* the warp finishing long strings */
+    uint64_t c_steps;              /* automaton steps and actions */
+    uint64_t c_finish;             /* writing records */
+    uint64_t c_unquote;            /* unquoting strings with the whole warp */
+} sse_counters;
+/* Byte identity of a batch without SSE_F_DONE_EXACT lines (those get no work item):
+ *   d_skip_bytes + d_coop_bytes + d_plain_steps + d_actions + d_abandoned_bytes + d_template_bytes == sum of sse_rec.payload_len.
+ * Valid after a successful sse_collect or sse_download of the slot and before sse_release. SSE_ERR_ARG: the context has no
+ * SSE_FLAG_COUNTERS, or out->struct_size != sizeof(sse_counters); SSE_ERR_BUSY: the slot holds no collected batch. */
+int sse_counters_read(sse_ctx *ctx, int slot, sse_counters *out);
 
 /* ---- host-side folds of the records (the reference's consumers, fed from the side-band) ---- */
 typedef struct { const uint8_t *p; size_t n; } sse_bytes;

@@ -8,7 +8,7 @@ from . import build as _build
 
 SSE_OK, SSE_ERR_NO_DEVICE, SSE_ERR_CUDA, SSE_ERR_ARG, SSE_ERR_BUSY, SSE_ERR_OVERFLOW, SSE_ERR_NOMEM, SSE_ERR_UNDECODED = 0, -1, -2, -3, -4, -5, -6, -7
 MODE_P, MODE_R, MODE_PARSE = 0, 1, 2
-FLAG_KERNEL_FUSED, FLAG_COPY_OUT, FLAG_TEMPLATES, FLAG_DEFER = 4, 8, 16, 64
+FLAG_KERNEL_FUSED, FLAG_COPY_OUT, FLAG_TEMPLATES, FLAG_DEFER, FLAG_COUNTERS = 4, 8, 16, 64, 256
 NONE = 0xFFFFFFFF
 MAX_LINE_BYTES = 16777215   # SSE_MAX_LINE_BYTES: decode work items carry a 24-bit payload length
 
@@ -89,12 +89,33 @@ class ToolCall(C.Structure):
     _fields_ = [("id", Bytes), ("type", Bytes), ("name", Bytes), ("arguments", Bytes)]
 
 
+# sse_counters (SSE_FLAG_COUNTERS): the uint64_t fields in header order
+COUNTER_FIELDS = (
+    "p_segments", "p_segments_skipped", "p_windows", "p_window_bytes", "p_rounds", "p_lines", "p_frames_zero_copy",
+    "p_frames_materialised", "p_bytes_materialised", "p_items", "p_long_lines", "p_pool_pages_taken", "p_pool_pages_returned",
+    "p_deferred_rounds",
+    "d_items", "d_pulls", "d_items_per_pull", "d_warp_rounds", "d_busy_lane_rounds", "d_skip_windows", "d_skip_bytes",
+    "d_coop_strings", "d_coop_steps", "d_coop_bytes", "d_plain_steps", "d_actions", "d_action_redos", "d_abandoned_bytes",
+    "d_template_lines", "d_template_bytes", "d_template_misses", "d_unquote_jobs", "d_unquote_bytes", "d_lines_finished",
+    "c_total", "c_pull", "c_skip", "c_coop", "c_steps", "c_finish", "c_unquote")
+
+
+class Counters(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("decode_passes", C.c_uint32)] + [(n, C.c_uint64) for n in COUNTER_FIELDS]
+
+
+def counters_dict(k: Counters) -> dict:
+    d = {n: int(getattr(k, n)) for n in COUNTER_FIELDS}
+    d["decode_passes"] = int(k.decode_passes)
+    return d
+
+
 assert C.sizeof(Seg) == 16 and C.sizeof(Rec) == 32 and C.sizeof(Tc) == 48 and C.sizeof(SegResult) == 32
 
 EXPORTS = [
     "sse_init", "sse_init_ex", "sse_line_pool_config", "sse_line_pool_stats", "sse_destroy", "sse_strerror", "sse_last_cuda_error", "sse_abi_version", "sse_default_config", "sse_worst_case_config",
     "sse_acquire", "sse_submit", "sse_collect", "sse_release", "sse_reset_conn", "sse_reset_all",
-    "sse_upload", "sse_launch", "sse_download", "sse_launch_count", "sse_at",
+    "sse_upload", "sse_launch", "sse_download", "sse_launch_count", "sse_at", "sse_counters_read",
     "sse_agent_new", "sse_agent_free", "sse_agent_reset", "sse_agent_feed", "sse_agent_content",
     "sse_agent_has_tool_calls", "sse_agent_terminated", "sse_agent_tool_calls",
     "sse_telemetry_new", "sse_telemetry_free", "sse_telemetry_reset", "sse_telemetry_feed", "sse_telemetry_feed_bytes", "sse_telemetry_finish",
@@ -143,6 +164,7 @@ def load(build_if_missing: bool = True):
     L.sse_launch.argtypes = [vp, i32, u32, vp]
     L.sse_download.argtypes = [vp, i32, C.POINTER(Result), vp]
     L.sse_launch_count.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.sse_counters_read.argtypes = [vp, i32, C.POINTER(Counters)]
     L.sse_at.argtypes = [C.POINTER(Result), u32]
     L.sse_at.restype = C.POINTER(C.c_uint8)
     if hasattr(L, "ssegw_mcp_writer_step"):

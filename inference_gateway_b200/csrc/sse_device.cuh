@@ -101,13 +101,41 @@ struct KParams {
     uint32_t *pool_stack;    uint32_t *pool_next;
     PoolChain *pool_chain;
     uint32_t page_bytes, pool_pages, max_line;
+    // SSE_FLAG_COUNTERS: the slot's counter block (CN_*), which selects the counting kernels; nullptr: the default kernels
+    unsigned long long *cnt;
 };
+
+// SSE_FLAG_COUNTERS: the counter block of a slot, one 64-bit counter per index, in the order of the uint64_t fields of
+// sse_counters (include/sse_gpu.h). The produce part is written by the produce and finalize kernels, the rest by the decode kernel.
+enum : uint32_t {
+    CN_P_SEGMENTS, CN_P_SEGMENTS_SKIPPED, CN_P_WINDOWS, CN_P_WINDOW_BYTES, CN_P_ROUNDS, CN_P_LINES, CN_P_FRAMES_ZERO_COPY,
+    CN_P_FRAMES_MATERIALISED, CN_P_BYTES_MATERIALISED, CN_P_ITEMS, CN_P_LONG_LINES, CN_P_POOL_PAGES_TAKEN, CN_P_POOL_PAGES_RETURNED,
+    CN_P_DEFERRED_ROUNDS,
+    CN_D_ITEMS, CN_D_PULLS, CN_D_ITEMS_PER_PULL, CN_D_WARP_ROUNDS, CN_D_BUSY_LANE_ROUNDS, CN_D_SKIP_WINDOWS, CN_D_SKIP_BYTES,
+    CN_D_COOP_STRINGS, CN_D_COOP_STEPS, CN_D_COOP_BYTES, CN_D_PLAIN_STEPS, CN_D_ACTIONS, CN_D_ACTION_REDOS, CN_D_ABANDONED_BYTES,
+    CN_D_TEMPLATE_LINES, CN_D_TEMPLATE_BYTES, CN_D_TEMPLATE_MISSES, CN_D_UNQUOTE_JOBS, CN_D_UNQUOTE_BYTES, CN_D_LINES_FINISHED,
+    CN_C_TOTAL, CN_C_PULL, CN_C_SKIP, CN_C_COOP, CN_C_STEPS, CN_C_FINISH, CN_C_UNQUOTE,
+    CN_COUNT
+};
+constexpr uint32_t CN_DECODE_FIRST = CN_D_ITEMS;   // the decode part: [CN_DECODE_FIRST, CN_COUNT)
+static_assert(CN_DECODE_FIRST <= 32 && CN_COUNT - CN_DECODE_FIRST <= 32, "a warp keeps one counter per lane");
 
 #ifdef __CUDACC__
 __device__ __forceinline__ void sse_overflow(Counters *c, uint32_t which) {
     atomicOr(&c->overflow, which);
     atomicExch(&c->status, (int)SSE_ERR_OVERFLOW);
 }
+
+// SSE_FLAG_COUNTERS: a warp's counters, one per lane (lane k holds counter first + k, 64-bit). add() takes a warp-uniform value
+// and is called by all lanes of the warp; flush() adds them to the counter block with one atomicAdd per counter.
+struct WarpTally {
+    unsigned long long v;
+    __device__ __forceinline__ void add(uint32_t k, unsigned long long x) { if ((threadIdx.x & 31u) == k) v += x; }
+    __device__ __forceinline__ void flush(unsigned long long *first, uint32_t n) {
+        const uint32_t k = threadIdx.x & 31u;
+        if (k < n && v) atomicAdd(first + k, v);
+    }
+};
 #endif
 
 // launch wrappers (sse_kernel.cu)

@@ -16,6 +16,7 @@
 //
 // Channel capacity is 100 as in provider.go:307: a stream with 100 undelivered elements stops accepting upstream bytes
 // (ssegw_upstream_write returns 0 bytes accepted), which is the back-pressure the reader goroutine would feel.
+#include <stddef.h>
 #include <stdint.h>
 #include <string.h>
 #include <deque>
@@ -49,7 +50,26 @@ struct ssegw {
     std::vector<Stream> streams;
     std::string last_error;
     size_t rr = 0;              // the batcher starts its scan one stream further every tick (no slot is favoured)
+    sse_counters sum{};         // SSE_FLAG_COUNTERS: every collected batch's counters added up (ssegw_counters)
 };
+
+namespace {
+
+// SSE_FLAG_COUNTERS: adds the counters of the batch just collected in `slot` to the gateway's sums (d_items_per_pull is the
+// launch's choice, not an amount: the last batch's is kept)
+void add_counters(ssegw *g, int slot) {
+    sse_counters k{};
+    k.struct_size = sizeof k;
+    if (sse_counters_read(g->ctx, slot, &k) != SSE_OK) return;
+    uint64_t *dst = &g->sum.p_segments;
+    const uint64_t *src = &k.p_segments;
+    const size_t n = (sizeof k - offsetof(sse_counters, p_segments)) / sizeof(uint64_t);
+    for (size_t i = 0; i < n; i++) dst[i] += src[i];
+    g->sum.d_items_per_pull = k.d_items_per_pull;
+    g->sum.decode_passes += k.decode_passes;
+}
+
+} // namespace
 
 extern "C" {
 
@@ -150,6 +170,7 @@ int ssegw_pump(ssegw *g) {
             sse_release(g->ctx, slot);
             return rc;
         }
+        if (g->cfg.flags & SSE_FLAG_COUNTERS) add_counters(g, slot);
         for (uint32_t k = 0; k < n; k++) {
             Stream &s = g->streams[who[k]];
             // only the bytes the batch took leave the queue: a deferred rest is submitted again, before anything newer
@@ -191,6 +212,13 @@ int ssegw_recv(ssegw *g, int id, uint8_t *buf, size_t cap, size_t *n) {
 }
 
 void ssegw_release_stream(ssegw *g, int id) { g->streams[(size_t)id].open = false; }
+
+int ssegw_counters(ssegw *g, sse_counters *out) {
+    if (!g || !out || out->struct_size != sizeof(sse_counters) || !(g->cfg.flags & SSE_FLAG_COUNTERS)) return SSE_ERR_ARG;
+    *out = g->sum;
+    out->struct_size = sizeof(sse_counters);
+    return SSE_OK;
+}
 
 // ---- handleStreamingRequest (api/routes.go:129-232): the raw proxy loop reads and writes in one goroutine
 int ssegw_proxy_stream(ssegw *g) { return ssegw_stream_chat_completions(g, SSE_MODE_P); }

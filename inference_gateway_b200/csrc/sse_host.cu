@@ -15,6 +15,10 @@
 #include <vector>
 #include "sse_device.cuh"
 
+static_assert(sizeof(sse_counters) == 8 + CN_COUNT * sizeof(uint64_t) && offsetof(sse_counters, p_segments) == 8 &&
+              offsetof(sse_counters, d_items) == 8 + 8 * CN_D_ITEMS && offsetof(sse_counters, c_unquote) == 8 + 8 * CN_C_UNQUOTE,
+              "sse_counters holds the counter block in CN_* order");
+
 namespace {
 
 thread_local char g_cuda_err[256] = "";
@@ -47,6 +51,11 @@ struct Slot {
     uint2 *d_tiles = nullptr;                                  // fused pipeline: tile list of the plan kernel
     uint32_t n_segs = 0, in_bytes = 0;
     uint32_t cap_tcs = 0, cap_usages = 0, cap_text = 0;        // decode-stage capacities (SSE_FLAG_DEFER grows them per slot)
+    // SSE_FLAG_COUNTERS: the batch's counter block (CN_*), device and pinned; kept apart from Counters, which the default path
+    // clears and downloads every batch
+    unsigned long long *d_cnt = nullptr, *h_cnt = nullptr;
+    uint32_t decode_passes = 0;
+    bool cnt_ready = false;                                    // h_cnt holds the counters of the batch last downloaded
 };
 
 } // namespace
@@ -83,7 +92,7 @@ void free_slot(Slot &s) {
     if (s.kernel_done) cudaEventDestroy(s.kernel_done);
     cudaFreeHost(s.h_in); cudaFreeHost(s.h_segs); cudaFreeHost(s.h_out); cudaFreeHost(s.h_frames); cudaFreeHost(s.h_recs);
     cudaFreeHost(s.h_tcs); cudaFreeHost(s.h_usages); cudaFreeHost(s.h_text); cudaFreeHost(s.h_runs); cudaFreeHost(s.h_segres);
-    cudaFreeHost(s.h_ctr);
+    cudaFreeHost(s.h_ctr); cudaFreeHost(s.h_cnt); cudaFree(s.d_cnt);
     cudaFree(s.d_segs); cudaFree(s.d_out);   // d_in lives inside d_out's allocation
     cudaFree(s.d_frames); cudaFree(s.d_recs); cudaFree(s.d_tcs);
     cudaFree(s.d_usages); cudaFree(s.d_text); cudaFree(s.d_runs); cudaFree(s.d_segres); cudaFree(s.d_ctr); cudaFree(s.d_items); cudaFree(s.d_segterm); cudaFree(s.d_items2); cudaFree(s.d_tiles);
@@ -109,6 +118,7 @@ KParams make_params(sse_ctx *c, Slot &s, uint32_t n_segs) {
     p.pool_chain = c->d_pool_chain;
     p.page_bytes = c->pool.page_bytes; p.pool_pages = c->pool.pool_pages;
     p.max_line = c->pool.pool_pages ? c->pool.max_line_bytes : c->cfg.carry_slot_bytes;
+    p.cnt = s.d_cnt;
     return p;
 }
 
@@ -140,6 +150,8 @@ int do_upload(sse_ctx *c, Slot &s, uint32_t n_segs, uint32_t in_bytes, cudaStrea
 
 int do_launch(sse_ctx *c, Slot &s, uint32_t n_segs, cudaStream_t st) {
     CU(cudaMemsetAsync(s.d_ctr, 0, sizeof(Counters), st));
+    s.cnt_ready = false;
+    if (s.d_cnt) CU(cudaMemsetAsync(s.d_cnt, 0, CN_COUNT * sizeof(unsigned long long), st));
     if (n_segs) {
         KParams p = make_params(c, s, n_segs);
         int e;
@@ -214,6 +226,10 @@ int redecode(sse_ctx *c, Slot &s, Counters &k, cudaStream_t st, uint32_t &grown)
         k.n_tcs = k.n_usages = k.text_bytes = 0; k.item_ticket = 0; k.status = SSE_OK; k.overflow = 0;
         *s.h_ctr = k;
         CU(cudaMemcpyAsync(s.d_ctr, s.h_ctr, offsetof(Counters, class_count), cudaMemcpyHostToDevice, st));
+        if (s.d_cnt) {   // the decode counters describe the pass whose records the batch returns
+            CU(cudaMemsetAsync(s.d_cnt + CN_DECODE_FIRST, 0, (CN_COUNT - CN_DECODE_FIRST) * sizeof(unsigned long long), st));
+            s.decode_passes++;
+        }
         if (c->have_last) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
         const int e = sse_launch_decode(make_params(c, s, s.n_segs), (void *)st, c->sm_count, c->device);
         if (e != 0) { cu_ok((cudaError_t)e, "decode kernel launch"); return SSE_ERR_CUDA; }
@@ -233,6 +249,7 @@ int do_download(sse_ctx *c, Slot &s, sse_result *res, cudaStream_t st) {
     Counters k = *s.h_ctr;
     memset(res, 0, sizeof *res);
     res->n_segs = s.n_segs;
+    s.decode_passes = s.n_segs ? 1u : 0u;
     uint32_t bits = 0;
     if (c->cfg.flags & SSE_FLAG_DEFER) {
         // the produce stage reports what it deferred in k.overflow without failing the batch; only the decode stage sets status
@@ -262,7 +279,9 @@ int do_download(sse_ctx *c, Slot &s, sse_result *res, cudaStream_t st) {
     if (k.text_bytes) CU(cudaMemcpyAsync(s.h_text, s.d_text, k.text_bytes, cudaMemcpyDeviceToHost, st));
     if (k.n_runs) CU(cudaMemcpyAsync(s.h_runs, s.d_runs, (size_t)k.n_runs * sizeof(sse_run), cudaMemcpyDeviceToHost, st));
     if (s.n_segs) CU(cudaMemcpyAsync(s.h_segres, s.d_segres, (size_t)s.n_segs * sizeof(sse_seg_result), cudaMemcpyDeviceToHost, st));
+    if (s.d_cnt) CU(cudaMemcpyAsync(s.h_cnt, s.d_cnt, CN_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
+    s.cnt_ready = s.d_cnt != nullptr;
     res->out = s.h_out; res->frames = s.h_frames; res->recs = s.h_recs; res->tcs = s.h_tcs; res->usages = s.h_usages;
     res->text = s.h_text; res->runs = s.h_runs; res->segs = s.h_segres;
     res->in = s.h_in; res->in_base = in_base_of(c->cfg);
@@ -358,8 +377,9 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
     if (cfg->n_slots < 1 || cfg->n_slots > 8 || cfg->max_conns == 0 || cfg->max_segs == 0 ||
         (cfg->in_arena_bytes & 15u) || cfg->carry_slot_bytes < 8192 + 16 || (cfg->carry_slot_bytes & 15u)) return SSE_ERR_ARG;
     if ((uint64_t)in_base_of(*cfg) + cfg->in_arena_bytes + 16 >= (1ull << 31)) return SSE_ERR_ARG;   // arena offsets are 31-bit
-    if (cfg->flags & ~(SSE_FLAG_KERNEL_FUSED | SSE_FLAG_COPY_OUT | SSE_FLAG_TEMPLATES | SSE_FLAG_DEFER)) return SSE_ERR_ARG;   // unknown engine flag
+    if (cfg->flags & ~(SSE_FLAG_KERNEL_FUSED | SSE_FLAG_COPY_OUT | SSE_FLAG_TEMPLATES | SSE_FLAG_DEFER | SSE_FLAG_COUNTERS)) return SSE_ERR_ARG;   // unknown engine flag
     if ((cfg->flags & SSE_FLAG_DEFER) && (cfg->flags & SSE_FLAG_KERNEL_FUSED)) return SSE_ERR_ARG;   // the tile kernel does not defer
+    if ((cfg->flags & SSE_FLAG_COUNTERS) && (cfg->flags & SSE_FLAG_KERNEL_FUSED)) return SSE_ERR_ARG;   // ... and has no counting instantiation
     // with SSE_FLAG_DEFER a segment alone in a batch must always get somewhere: one round of up to 64 lines (at most a window of
     // bytes plus a '\n' per line), and the longest line a connection may hold, must fit an empty batch
     if ((cfg->flags & SSE_FLAG_DEFER) &&
@@ -421,6 +441,8 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
         ok = ok && dalloc(s.d_items, cfg->max_recs) && dalloc(s.d_segterm, cfg->max_segs);
         ok = ok && dalloc(s.d_items2, cfg->max_recs);
         ok = ok && dalloc(s.d_tiles, (size_t)cfg->max_segs + 64);
+        if (ok && (cfg->flags & SSE_FLAG_COUNTERS))
+            ok = dalloc(s.d_cnt, CN_COUNT) && halloc(s.h_cnt, CN_COUNT) && cu_ok(cudaMemset(s.d_cnt, 0, CN_COUNT * sizeof(unsigned long long)), "cudaMemset");
     }
     if (!ok) { sse_destroy(c); return SSE_ERR_CUDA; }
     *out = c;
@@ -488,6 +510,7 @@ int sse_release(sse_ctx *c, int slot) {
     Slot &s = c->slots[slot];
     if (s.state == SLOT_SUBMITTED) { CU(cudaSetDevice(c->device)); CU(cudaStreamSynchronize(s.stream)); }
     s.state = SLOT_FREE;
+    s.cnt_ready = false;
     return SSE_OK;
 }
 
@@ -561,6 +584,16 @@ int sse_debug_tcache(sse_ctx *c, uint32_t *out, uint32_t words) {
     const uint32_t n = words < sse_fused_tcache_words() ? words : sse_fused_tcache_words();
     CU(cudaMemcpy(out, c->d_tcache, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     return (int)n;
+}
+
+int sse_counters_read(sse_ctx *c, int slot, sse_counters *out) {
+    if (!c || !out || out->struct_size != sizeof(sse_counters) || !(c->cfg.flags & SSE_FLAG_COUNTERS) || slot < 0 ||
+        slot >= (int)c->slots.size()) return SSE_ERR_ARG;
+    const Slot &s = c->slots[slot];
+    if ((s.state != SLOT_COLLECTED && s.state != SLOT_ACQUIRED) || !s.cnt_ready) return SSE_ERR_BUSY;
+    out->decode_passes = s.decode_passes;
+    memcpy(&out->p_segments, s.h_cnt, CN_COUNT * sizeof(uint64_t));
+    return SSE_OK;
 }
 
 int sse_launch_count(sse_ctx *c, uint64_t *kernel_launches) {

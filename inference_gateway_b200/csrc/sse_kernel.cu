@@ -24,8 +24,37 @@ namespace {
 #ifndef SSE_V1_MINB
 #define SSE_V1_MINB 2
 #endif
+
+// ---- SSE_FLAG_COUNTERS (the counting instantiation only)
+// Pages held by conn's line-pool chain. Only the warp that has the connection's segment moves its pages during the produce
+// launch, so the difference across a call is the pages that call took or returned.
+__device__ __forceinline__ uint32_t pool_held(const KParams &P, uint32_t conn) {
+    uint32_t n = 0;
+    if (P.pool_pages && lane_id() == 0) n = ((volatile PoolChain *)P.pool_chain)[conn].n_pages;
+    return __shfl_sync(FULL, n, 0);
+}
+__device__ __forceinline__ void tally_pages(WarpTally &T, uint32_t before, uint32_t after) {
+    T.add(CN_P_POOL_PAGES_TAKEN, after > before ? after - before : 0u);
+    T.add(CN_P_POOL_PAGES_RETURNED, before > after ? before - after : 0u);
+}
+// A line assembled outside the window was completed: its frame (always materialised) and work item, read back from the run
+// complete_long_line appended (had_first / last_before: rc before the call).
+__device__ __forceinline__ void tally_long_line(const KParams &P, WarpTally &T, const RunChain &rc, bool had_first, uint32_t last_before) {
+    uint32_t nf = 0, fl = 0, ni = 0;
+    if (lane_id() == 0 && rc.have_first && (!had_first || rc.last_idx != last_before)) {
+        const sse_run r = rc.last_idx == SSE_NONE ? rc.first : P.runs[rc.last_idx];   // lane 0 wrote it
+        nf = r.frame_count;
+        if (nf) fl = P.frames[r.frame_first].len;
+        if (r.rec_count && !(P.recs[r.rec_first].flags & SSE_F_DONE_EXACT)) ni = 1;
+    }
+    nf = __shfl_sync(FULL, nf, 0); fl = __shfl_sync(FULL, fl, 0); ni = __shfl_sync(FULL, ni, 0);
+    T.add(CN_P_LINES, 1); T.add(CN_P_LONG_LINES, 1);
+    T.add(CN_P_FRAMES_MATERIALISED, nf); T.add(CN_P_BYTES_MATERIALISED, fl); T.add(CN_P_ITEMS, ni);
+}
+
 // DEFER: SSE_FLAG_DEFER (its own instantiation: the cold deferral paths do not weigh on the default kernel's registers)
-template <bool SPLIT, bool DEFER>
+// CNT: SSE_FLAG_COUNTERS (its own instantiation: with CNT = false every counting statement is compiled out)
+template <bool SPLIT, bool DEFER, bool CNT>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, SSE_V1_MINB)
 sse_stream_kernel(const __grid_constant__ KParams P) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -39,6 +68,8 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
     WarpSmem &W = cs.w[threadIdx.x >> 5];
     uint8_t *buf = W.buf;
     const uint32_t lane = lane_id();
+    WarpTally T;
+    if constexpr (CNT) T.v = 0;
 
     // tickets are taken one segment ahead: while a segment is processed, the next one's first window is on its way to L2
     uint32_t s_next = 0;
@@ -47,6 +78,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
     for (;;) {
         const uint32_t s = s_next;
         if (s >= P.n_segs) break;
+        if constexpr (CNT) T.add(CN_P_SEGMENTS, 1);
         if (lane == 0) s_next = atomicAdd(&P.ctr->ticket, 1u);
         s_next = __shfl_sync(FULL, s_next, 0);
         if (s_next < P.n_segs) {
@@ -72,6 +104,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                 r.flags = (cst.flags & CONN_DEAD) ? SSE_SEG_DEAD : SSE_SEG_FINISHED; r.consumed = seg.in_len;
                 P.seg_results[s] = r;
             }
+            if constexpr (CNT) T.add(CN_P_SEGMENTS_SKIPPED, 1);
             continue;
         }
 
@@ -112,6 +145,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
             carry_front = false;
             __syncwarp();
             int pos = base;
+            if constexpr (CNT) { T.add(CN_P_WINDOWS, 1); T.add(CN_P_WINDOW_BYTES, (uint32_t)(fill - base)); }
 
             if (in_long) {
                 // still inside a line longer than the window: look for its end only
@@ -122,7 +156,11 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     if (m) q = i0 + __ffs(m) - 1;
                 }
                 int take = (q < 0) ? (fill - base) : (q - base + 1);
-                if (!hold_back(P, conn, slot, clen, buf + base, take)) { dead = true; break; }
+                uint32_t pages = 0;
+                if constexpr (CNT) pages = pool_held(P, conn);
+                const bool held = hold_back(P, conn, slot, clen, buf + base, take);
+                if constexpr (CNT) tally_pages(T, pages, pool_held(P, conn));
+                if (!held) { dead = true; break; }
                 clen += take;
                 __syncwarp();
                 if (q < 0) {
@@ -130,7 +168,15 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     if (consumed >= in_len) break;
                     continue;
                 }
-                if (!complete_long_line<DEFER>(P, rc, conn, slot, clen, mode, SPLIT ? (int)s : -1)) {
+                const bool had_first = rc.have_first;
+                const uint32_t last_before = rc.last_idx;
+                if constexpr (CNT) pages = pool_held(P, conn);
+                const bool completed = complete_long_line<DEFER>(P, rc, conn, slot, clen, mode, SPLIT ? (int)s : -1);
+                if constexpr (CNT) {
+                    tally_pages(T, pages, pool_held(P, conn));
+                    if (completed) tally_long_line(P, T, rc, had_first, last_before);
+                }
+                if (!completed) {
                     consumed = q + in_delta; clen--;   // (SSE_FLAG_DEFER) the segment stops at the line's '\n'
                     overflow = true; break;
                 }
@@ -269,6 +315,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     ob = (uint32_t)r0; qb = (uint32_t)(r0 >> 32); fb = (uint32_t)r1; rb = (uint32_t)(r1 >> 32);
                 }
                 ob = __shfl_sync(FULL, ob, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0); qb = __shfl_sync(FULL, qb, 0);
+                if constexpr (CNT) T.add(CN_P_ROUNDS, 1);
                 if (!DEFER) {
                     if (ob + tot_b + 16 > P.cap_out || fb + tot_f > P.cap_frames || rb + tot_r > P.cap_recs ||
                         (SPLIT && qb + tot_q > P.cap_items)) {
@@ -281,8 +328,19 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     const bool need_run = rc.have_first && (tot_f | tot_r) != 0u;
                     if ((!fits || need_run) && !admit_round(P, rc, fits, qb, tot_q, need_run)) {
                         consumed = pos + in_delta;   // the segment stops before this round
+                        if constexpr (CNT) T.add(CN_P_DEFERRED_ROUNDS, 1);
                         overflow = true; break;
                     }
+                }
+                if constexpr (CNT) {
+                    uint32_t nzc = 0, nmat = 0, bmat = 0;
+                    #pragma unroll
+                    for (int h = 0; h < 2; h++)
+                        if (my_flen[h]) { if (my_zc[h]) nzc++; else { nmat++; bmat += my_flen[h]; } }
+                    T.add(CN_P_LINES, (uint32_t)n_lines); T.add(CN_P_ITEMS, tot_q);
+                    T.add(CN_P_FRAMES_ZERO_COPY, __reduce_add_sync(FULL, nzc));
+                    T.add(CN_P_FRAMES_MATERIALISED, __reduce_add_sync(FULL, nmat));
+                    T.add(CN_P_BYTES_MATERIALISED, __reduce_add_sync(FULL, bmat));
                 }
                 // frame table
                 #pragma unroll
@@ -444,20 +502,21 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
         }
         __syncwarp();
     }
+    if constexpr (CNT) T.flush(P.cnt, CN_DECODE_FIRST);
 }
 
 } // namespace
 
-template <bool SPLIT, bool DEFER>
+template <bool SPLIT, bool DEFER, bool CNT>
 static int launch_v1(const KParams &p, void *stream, int sm_count) {
     static bool attr_set = false;
     static int ctas_per_sm = 0;
     const size_t smem = sizeof(CtaSmem);
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(sse_stream_kernel<SPLIT, DEFER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(sse_stream_kernel<SPLIT, DEFER, CNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return (int)e;
         int n = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sse_stream_kernel<SPLIT, DEFER>, WARPS_PER_CTA * 32, smem);
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sse_stream_kernel<SPLIT, DEFER, CNT>, WARPS_PER_CTA * 32, smem);
         if (e != cudaSuccess) return (int)e;
         ctas_per_sm = n > 0 ? n : 1;
         attr_set = true;
@@ -465,10 +524,11 @@ static int launch_v1(const KParams &p, void *stream, int sm_count) {
     int grid = sm_count * ctas_per_sm;   // persistent: one resident wave, warps pull segments by ticket
     int need = (int)((p.n_segs + WARPS_PER_CTA - 1) / WARPS_PER_CTA);
     if (need < grid) grid = need > 0 ? need : 1;
-    sse_stream_kernel<SPLIT, DEFER><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(p);
+    sse_stream_kernel<SPLIT, DEFER, CNT><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(p);
     return (int)cudaGetLastError();
 }
 
 int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count) {
-    return (p.flags & SSE_FLAG_DEFER) ? launch_v1<true, true>(p, stream, sm_count) : launch_v1<true, false>(p, stream, sm_count);
+    if (p.cnt) return (p.flags & SSE_FLAG_DEFER) ? launch_v1<true, true, true>(p, stream, sm_count) : launch_v1<true, false, true>(p, stream, sm_count);
+    return (p.flags & SSE_FLAG_DEFER) ? launch_v1<true, true, false>(p, stream, sm_count) : launch_v1<true, false, false>(p, stream, sm_count);
 }

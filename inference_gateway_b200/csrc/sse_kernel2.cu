@@ -12,6 +12,7 @@
 //   sse_finalize_kernel                    early termination (agent.go:235-242): cut a segment's runs after its terminating chunk
 //   sse_decode_kernel<TPL=true>            the same with skeleton-template replay in front of the automaton (SSE_FLAG_TEMPLATES;
 //                                          opt-in: measured slower, DESIGN.md 4.2)
+//   sse_decode_kernel<TPL, CNT=true>       SSE_FLAG_COUNTERS: the same with per-warp counters and cycle marks (DTally)
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "sse_common.cuh"
@@ -397,6 +398,23 @@ __device__ bool v2_finish_line(const KParams &P, Lane &L, LaneScratch &S, LaneJo
     return terminates;
 }
 
+// ---- SSE_FLAG_COUNTERS (the counting instantiation only): a warp's decode counters, one per lane (WarpTally from CN_DECODE_FIRST),
+// and the clock of its last mark. mark(k) charges the cycles since the previous mark to bucket k: the warp is converged there and
+// lane 0's clock is the warp's.
+struct DTally {
+    WarpTally t;
+    long long last;
+    __device__ __forceinline__ void add(uint32_t k, unsigned long long x) { t.add(k - CN_DECODE_FIRST, x); }
+    __device__ __forceinline__ void lanes(uint32_t k, uint32_t x) { add(k, __reduce_add_sync(FULL, x)); }   // sum over the lanes
+    __device__ __forceinline__ void ballot(uint32_t k, bool x) { add(k, (uint32_t)__popc(__ballot_sync(FULL, x))); }
+    __device__ __forceinline__ void mark(uint32_t k) {
+        __syncwarp();
+        const long long now = __shfl_sync(FULL, (long long)clock64(), 0);
+        add(k, (unsigned long long)(now - last));
+        last = now;
+    }
+};
+
 // ---- stragglers inside a long string value. A lane skips at most SKIPW windows of a string per round, so a 4 KB value costs it
 // 64 rounds while the lanes with shorter lines have retired and the warp runs almost empty; the length of a nearly empty launch (a
 // steady-state tick) is exactly that walk. When at most SSE_COOP lanes of the warp (any number of them when the launch has fewer
@@ -412,8 +430,8 @@ __device__ __forceinline__ uint32_t first_special16_from0(const uint4 &v) {     
     const unsigned long long lo = ((unsigned long long)s1 << 32) | s0, hi = ((unsigned long long)s3 << 32) | s2;
     return lo ? (uint32_t)(__ffsll((long long)lo) - 1) >> 3 : (hi ? 8u + ((uint32_t)(__ffsll((long long)hi) - 1) >> 3) : 16u);
 }
-template <bool RO>
-__device__ __forceinline__ void coop_string_skip(const KParams &P, Lane &L, unsigned mm) {
+template <bool RO, bool CNT>
+__device__ __forceinline__ void coop_string_skip(const KParams &P, Lane &L, unsigned mm, DTally &C) {
     const uint32_t lane = lane_id();
     #pragma unroll 1
     while (mm) {
@@ -421,9 +439,11 @@ __device__ __forceinline__ void coop_string_skip(const KParams &P, Lane &L, unsi
         mm &= mm - 1;
         uint32_t q = __shfl_sync(FULL, L.p, src);                 // 16-byte aligned: the lane's own skip stopped at a window border
         const uint32_t qe = __shfl_sync(FULL, L.pe, src);
+        const uint32_t q0 = q;
         uint32_t pos;
         #pragma unroll 1
         for (;;) {
+            if constexpr (CNT) C.add(CN_D_COOP_STEPS, 1);
             const uint32_t off = q + lane * 16u;
             uint32_t stop = 0xFFFFFFFFu;                         // where this lane's 16 bytes end the run (none: they are all plain)
             if (off >= qe) stop = qe;
@@ -435,6 +455,7 @@ __device__ __forceinline__ void coop_string_skip(const KParams &P, Lane &L, unsi
             if (hm) { pos = __shfl_sync(FULL, stop, __ffs(hm) - 1); break; }
             q += 512u;
         }
+        if constexpr (CNT) { C.add(CN_D_COOP_STRINGS, 1); C.add(CN_D_COOP_BYTES, pos - q0); }
         if ((int)lane == src) {
             L.slen += pos - L.p; L.p = pos;
             if (L.p < L.pe) L.win = ldwin16<RO>(P.out, L.p);
@@ -443,9 +464,12 @@ __device__ __forceinline__ void coop_string_skip(const KParams &P, Lane &L, unsi
 }
 
 // One round of the per-lane automaton: KSTEPS plain steps, then the pending action (if any) of every lane.
-template <bool RO, bool REC>
-__device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, Lane &L, LaneScratch &S, LaneJobs *J, const uint32_t coop_max) {
+template <bool RO, bool REC, bool CNT>
+__device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, Lane &L, LaneScratch &S, LaneJobs *J, const uint32_t coop_max,
+                                         DTally &C) {
     uint32_t pend = 0;                       // action | cls << 8 | in_str << 16 | in_tok << 17
+    uint32_t n_win = 0, n_plain = 0, n_act = 0, p0 = 0;      // (CNT) this lane's windows of phase A, steps, v2_action calls
+    if constexpr (CNT) { C.add(CN_D_WARP_ROUNDS, 1); C.ballot(CN_D_BUSY_LANE_ROUNDS, L.busy); p0 = L.p; }
     // phase A (once per round, only the lanes inside a string or a digit run): jump over the plain bytes -- to the next '"',
     // '\\', control or non-ASCII byte of a key or value string, or to the next non-digit of an integer, fraction or exponent --
     // up to SKIPW windows. The automaton would walk those bytes without changing its state or flags; the key's or value's
@@ -457,6 +481,7 @@ __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, L
         int w = 0;
         #pragma unroll 1
         for (; w < SKIPW; w++) {
+            if constexpr (CNT) n_win++;
             const uint32_t i = L.p & 15u;
             uint32_t s0, s1, s2, s3;
             if (str_run) { s0 = special_mask4(L.win.x); s1 = special_mask4(L.win.y); s2 = special_mask4(L.win.z); s3 = special_mask4(L.win.w); }
@@ -479,10 +504,12 @@ __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, L
         }
         more = str_run && w == SKIPW;
     }
+    if constexpr (CNT) { C.lanes(CN_D_SKIP_WINDOWS, n_win); C.lanes(CN_D_SKIP_BYTES, L.p - p0); C.mark(CN_C_SKIP); }
     if (SSE_COOP) {
         const unsigned mm = __ballot_sync(FULL, more);
-        if (mm && (uint32_t)__popc(mm) <= coop_max) coop_string_skip<RO>(P, L, mm);
+        if (mm && (uint32_t)__popc(mm) <= coop_max) coop_string_skip<RO, CNT>(P, L, mm, C);
     }
+    if constexpr (CNT) C.mark(CN_C_COOP);
     // phase B: plain automaton steps
     #pragma unroll
     for (int k = 0; k < KSTEPS; k++) {
@@ -496,6 +523,7 @@ __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, L
             const bool in_str = L.st >= S_KSTR, in_tok = L.st >= S_NMINUS;
             const uint32_t t = T.tr[L.st * NCLS + cls];
             if (t < A_FIRST) {
+                if constexpr (CNT) n_plain++;
                 L.sf = in_str ? (L.sf | (e >> 13)) : (L.sf & ~SF_STRMASK);
                 L.slen = in_tok ? L.slen + 1 : 0;
                 L.st = t;
@@ -507,7 +535,9 @@ __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, L
     if (pend) {
         uint32_t t = pend & 0xFFu;
         const uint32_t cls = (pend >> 8) & 0xFFu;
+        if constexpr (CNT) p0 = L.p;
         for (;;) {
+            if constexpr (CNT) n_act++;
             if (!v2_action<REC>(P, T, L, S, J, t)) break;         // the action chose the next state
             t = T.tr[L.st * NCLS + cls];                     // redo: same byte, new state
             if (t < A_FIRST) { L.st = t; break; }
@@ -515,9 +545,15 @@ __device__ __forceinline__ void v2_round(const KParams &P, const DfaTables &T, L
         const bool in_str = (pend & 0x10000u) != 0;
         const uint32_t nf = (cls == C_BSLASH ? SF_ESC : 0u) | (cls >= C_H80 ? SF_HI : 0u);
         L.sf = in_str ? (L.sf | nf) : (L.sf & ~SF_STRMASK);
+        if constexpr (CNT) p0 = L.p - p0;            // bytes a syntax or depth error jumped over (L.p = L.pe - 1)
         L.slen = (pend & 0x20000u) ? L.slen + 1 : 0;
         L.p++;
         if ((L.p & 15u) == 0 && L.p < L.pe) L.win = ldwin16<RO>(P.out, L.p);
+    }
+    if constexpr (CNT) {
+        C.lanes(CN_D_PLAIN_STEPS, n_plain); C.lanes(CN_D_ACTIONS, pend ? 1u : 0u);
+        C.lanes(CN_D_ACTION_REDOS, n_act ? n_act - 1u : 0u); C.lanes(CN_D_ABANDONED_BYTES, pend ? p0 : 0u);
+        C.mark(CN_C_STEPS);
     }
 }
 
@@ -805,7 +841,8 @@ struct CtaSmem3 {
 };
 static_assert(sizeof(CtaSmem3) <= 227 * 1024, "shared memory budget");
 
-template <bool TPL>
+// CNT: SSE_FLAG_COUNTERS (its own instantiation: with CNT = false every counting statement is compiled out)
+template <bool TPL, bool CNT>
 __global__ void __launch_bounds__(V3_WARPS * 32, 1)
 sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict__ gT) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -849,6 +886,14 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
     L.finish = 0; L.ct = L.ct1 = L.sstk = 0; L.content_off = L.content_len = 0; L.tc_count = 0; L.tc_first = SSE_NONE;
     S.rec = S.frame = S.slot = S.plen = 0;
 
+    DTally C;
+    long long t_start = 0;
+    if constexpr (CNT) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) P.cnt[CN_D_ITEMS_PER_PULL] = batch;
+        C.t.v = 0;
+        __syncwarp();
+        t_start = C.last = __shfl_sync(FULL, (long long)clock64(), 0);
+    }
     for (;;) {
         uint32_t base = 0;
         if (lane == 0) base = atomicAdd(&P.ctr->item_ticket, batch);
@@ -856,6 +901,7 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
         if (base >= n_items) break;
         const uint32_t idx = base + lane;
         const bool has = lane < batch && idx < n_items;
+        if constexpr (CNT) { C.add(CN_D_PULLS, 1); C.ballot(CN_D_ITEMS, has); }
         if (has) {
             const uint4 it = P.items_sorted[idx];
             L.p = it.x; S.plen = it.y & 0x00FFFFFFu; L.pe = it.x + S.plen; S.rec = it.z; S.slot = it.w;   // slot: segment index
@@ -893,6 +939,10 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
                 uint32_t d = 0;
                 t_walk<true, true>(P, Tm, L, S, J, L.p, L.pe, d, full);
             }
+            if constexpr (CNT) {
+                C.ballot(CN_D_TEMPLATE_LINES, toff != 0u); C.ballot(CN_D_LINES_FINISHED, toff != 0u);
+                C.lanes(CN_D_TEMPLATE_BYTES, toff ? S.plen : 0u); C.ballot(CN_D_TEMPLATE_MISSES, cand && !toff);
+            }
             if (toff) {                                  // the record is written, the lane retires
                 L.n_choices = Tm[3] & 0xFFFFu;
                 if (Tm[2] & SSE_F_TC_NONNIL) L.sf |= SF_TCNONNIL;
@@ -913,12 +963,14 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
             }
         }
         if (L.busy && L.p < L.pe) L.win = ldwin16<true>(P.out, L.p);      // the automaton reads the payload through a 16-byte window
+        if constexpr (CNT) C.mark(CN_C_PULL);
         for (;;) {
             const bool any_busy = __any_sync(FULL, L.busy);
             if (any_busy) {
                 #pragma unroll 1
                 for (int round = 0; round < ROUNDS; round++) {
-                    v2_round<true, TPL>(P, T, L, S, J, coop_max);
+                    v2_round<true, TPL, CNT>(P, T, L, S, J, coop_max, C);
+                    if constexpr (CNT) C.ballot(CN_D_LINES_FINISHED, L.busy && L.p >= L.pe);
                     if (L.busy && L.p >= L.pe) {
                         const uint32_t ps = L.pe - S.plen, pe = L.pe;
                         if (v2_finish_line<TPL>(P, L, S, J)) atomicMin(&P.seg_term[S.slot], S.rec);   // agent.go:235-242, resolved in stage 3
@@ -935,6 +987,7 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
                         }
                         L.p = L.pe = 0;
                     }
+                    if constexpr (CNT) C.mark(CN_C_FINISH);
                 }
             }
             // strings that need unquoting were queued by the lanes: decode them with the whole warp
@@ -947,14 +1000,22 @@ sse_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__restrict
                 const uint32_t nj = LJ.n;
                 for (uint32_t k = 0; k < nj; k++) {
                     const UnquoteJob jb = LJ.j[k];
+                    if constexpr (CNT) { C.add(CN_D_UNQUOTE_JOBS, 1); C.add(CN_D_UNQUOTE_BYTES, jb.e - jb.s); }
                     warp_unquote(P.out, jb.s, jb.e, P.text + jb.dst, jb.patch);
                 }
                 __syncwarp();
                 if ((int)lane == leader) LJ.n = 0;
             }
             __syncwarp();
+            if constexpr (CNT) C.mark(CN_C_UNQUOTE);
             if (!any_busy) break;
         }
+    }
+    if constexpr (CNT) {
+        __syncwarp();
+        const long long t_end = __shfl_sync(FULL, (long long)clock64(), 0);
+        C.add(CN_C_TOTAL, (unsigned long long)(t_end - t_start));
+        C.t.flush(P.cnt + CN_DECODE_FIRST, CN_COUNT - CN_DECODE_FIRST);
     }
     // one CTA hands what it has learnt to the next launch (all CTAs see the same kinds of lines)
     if (templates && blockIdx.x == 0) {
@@ -1049,6 +1110,7 @@ __global__ void __launch_bounds__(SCATTER_TPB) sse_bucket_scatter_kernel(const K
 // resubmit: bytes its batch deferred (SSE_FLAG_DEFER) would be ignored, so the whole segment counts as consumed. Where the
 // segment terminates does not depend on the tool-call, usage and text arenas, so this stage is complete even when the decode
 // stage ran out of them (and is decoded again by sse_launch_decode).
+template <bool CNT>
 __global__ void sse_finalize_kernel(const __grid_constant__ KParams P) {
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= P.n_segs) return;
@@ -1074,7 +1136,9 @@ __global__ void sse_finalize_kernel(const __grid_constant__ KParams P) {
     const uint32_t conn = P.segs[s].conn;
     // the produce stage kept reading after the terminating chunk and may have pooled a line that is never completed
     if (P.pool_pages && ((volatile PoolChain *)P.pool_chain)[conn].n_pages) {
-        pool_lock(P.pool_hdr); pool_release_locked(P, conn); pool_unlock(P.pool_hdr);
+        pool_lock(P.pool_hdr);
+        if constexpr (CNT) atomicAdd(P.cnt + CN_P_POOL_PAGES_RETURNED, (unsigned long long)((volatile PoolChain *)P.pool_chain)[conn].n_pages);
+        pool_release_locked(P, conn); pool_unlock(P.pool_hdr);
     }
     ConnState ns; ns.carry_len = 0; ns.flags = CONN_FINISHED;
     P.conns[conn] = ns;
@@ -1124,24 +1188,40 @@ int sse_v2_prepare(int device) {
     if (e != cudaSuccess) return (int)e;
     e = cudaMemcpy(d, &T, sizeof T, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(sse_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
+    e = cudaFuncSetAttribute(sse_decode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(sse_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
+    e = cudaFuncSetAttribute(sse_decode_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
+    if (e != cudaSuccess) return (int)e;
+    e = cudaFuncSetAttribute(sse_decode_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
+    if (e != cudaSuccess) return (int)e;
+    e = cudaFuncSetAttribute(sse_decode_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
     if (e != cudaSuccess) return (int)e;
     g_tables_dev[device] = d;
     return 0;
+}
+
+// the decode kernel the context's flags select: templates (KParams.tcache) and counters (KParams.cnt)
+static void launch_decode_kernel(const KParams &p, cudaStream_t st, int sm_count, int device) {
+    const DfaTables *t = g_tables_dev[device];
+    if (p.cnt) {
+        if (p.tcache) sse_decode_kernel<true, true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
+        else sse_decode_kernel<false, true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
+    } else {
+        if (p.tcache) sse_decode_kernel<true, false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
+        else sse_decode_kernel<false, false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
+    }
 }
 
 int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device) {
     sse_bucket_hist_kernel<<<sm_count * 2, 512, 0, (cudaStream_t)stream>>>(p);
     sse_bucket_scan_kernel<<<1, SCAN_TPB, 0, (cudaStream_t)stream>>>(p);
     sse_bucket_scatter_kernel<<<sm_count * 2, SCATTER_TPB, 0, (cudaStream_t)stream>>>(p);
-    if (p.tcache) sse_decode_kernel<true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), (cudaStream_t)stream>>>(p, g_tables_dev[device]);
-    else sse_decode_kernel<false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), (cudaStream_t)stream>>>(p, g_tables_dev[device]);
+    launch_decode_kernel(p, (cudaStream_t)stream, sm_count, device);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return (int)e;
     const int tpb = 256;
-    sse_finalize_kernel<<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
+    if (p.cnt) sse_finalize_kernel<true><<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
+    else sse_finalize_kernel<false><<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
     return (int)cudaGetLastError();
 }
 
@@ -1149,8 +1229,7 @@ int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int
 // in items_sorted (the caller has reset the decode counters). Records are rewritten whole, so a second pass gives the records a
 // single pass with large enough arenas gives.
 int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device) {
-    if (p.tcache) sse_decode_kernel<true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), (cudaStream_t)stream>>>(p, g_tables_dev[device]);
-    else sse_decode_kernel<false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), (cudaStream_t)stream>>>(p, g_tables_dev[device]);
+    launch_decode_kernel(p, (cudaStream_t)stream, sm_count, device);
     return (int)cudaGetLastError();
 }
 

@@ -211,6 +211,14 @@ class SseEngine:
         A.check(rc, "sse_download")
         return self._wrap(res)
 
+    def counters(self, slot) -> dict:
+        """sse_counters_read (engine made with flags=FLAG_COUNTERS): what the kernels did for the batch collected or downloaded in
+        slot, as {field: int} with the field names of sse_counters, plus decode_passes. Valid until the slot is released."""
+        k = A.Counters()
+        k.struct_size = C.sizeof(A.Counters)
+        A.check(self.L.sse_counters_read(self._ctx, slot, C.byref(k)), "sse_counters_read")
+        return A.counters_dict(k)
+
     def launch_count(self) -> int:
         n = C.c_uint64()
         A.check(self.L.sse_launch_count(self._ctx, C.byref(n)), "sse_launch_count")

@@ -43,6 +43,7 @@ class Gateway:
         L.ssegw_agent_terminated.argtypes = [vp, i32, C.POINTER(i32)]
         L.ssegw_agent_tool_calls.argtypes = [vp, i32, C.POINTER(A.ToolCall), C.c_size_t]
         L.ssegw_agent_tool_calls.restype = C.c_size_t
+        L.ssegw_counters.argtypes = [vp, C.POINTER(A.Counters)]
         st = i32()
         self._pool = make_line_pool(**line_pool) if line_pool is not None else None
         if config is not None:
@@ -120,6 +121,14 @@ class Gateway:
         g = lambda x: C.string_at(x.p, x.n) if x.n else b""
         calls = [dict(id=g(arr[i].id), type=g(arr[i].type), name=g(arr[i].name), args=g(arr[i].arguments)) for i in range(min(n, 64))]
         return content, bool(self.L.ssegw_agent_has_tool_calls(self.g, sid)), term, fin.value, calls
+
+    def counters(self) -> dict:
+        """ssegw_counters: the sse_counters of every batch collected so far, added up (the gateway's config must have
+        FLAG_COUNTERS), as {field: int} plus decode_passes."""
+        k = A.Counters()
+        k.struct_size = C.sizeof(A.Counters)
+        A.check(self.L.ssegw_counters(self.g, C.byref(k)), "ssegw_counters")
+        return A.counters_dict(k)
 
     def release(self, sid: int):
         self.L.ssegw_release_stream(self.g, sid)

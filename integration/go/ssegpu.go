@@ -55,6 +55,9 @@ func envUint32(name string) uint32 {
 // shared by all connections: a line longer than the carry slot continues there instead of failing its stream, up to
 // GPU_LINE_POOL_MAX_LINE bytes per connection (default and ceiling SSE_MAX_LINE_BYTES, 16 MiB - 1).
 //
+// GPU_COUNTERS=1 sets SSE_FLAG_COUNTERS: the counting kernels run and Counters(slot) reports what they did for each batch
+// (INTEGRATION.md section 2 maps the fields to metric names).
+//
 // GPU_DEFER=1 sets SSE_FLAG_DEFER: a batch whose results do not fit the default capacities no longer fails (which would close
 // every stream in it); what does not fit waits for the next batch. The batcher must then keep the unconsumed tail of a
 // deferred segment (data[res.Consumed(i):], see Result.Deferred) at the head of that connection's queue and submit it before
@@ -65,6 +68,9 @@ func NewContext(device int, maxConns, bytesPerBatch uint32) (*Context, error) {
 	C.sse_default_config(&cfg, C.uint32_t(maxConns), C.uint32_t(bytesPerBatch))
 	if os.Getenv("GPU_DEFER") == "1" {
 		cfg.flags |= C.SSE_FLAG_DEFER
+	}
+	if os.Getenv("GPU_COUNTERS") == "1" {
+		cfg.flags |= C.SSE_FLAG_COUNTERS
 	}
 	var ctx *C.sse_ctx
 	if pages := envUint32("GPU_LINE_POOL_PAGES"); pages > 0 {
@@ -83,6 +89,15 @@ func NewContext(device int, maxConns, bytesPerBatch uint32) (*Context, error) {
 		return nil, err
 	}
 	return &Context{c: ctx}, nil
+}
+
+// Counters returns what the kernels did for the batch collected in slot (SSE_FLAG_COUNTERS, GPU_COUNTERS=1): valid after
+// Collect and before Release. The batcher adds them up and exports them as monotonic counters.
+func (x *Context) Counters(slot C.int) (C.sse_counters, error) {
+	var k C.sse_counters
+	k.struct_size = C.uint32_t(unsafe.Sizeof(k))
+	err := statusErr("sse_counters_read", C.sse_counters_read(x.c, slot, &k))
+	return k, err
 }
 
 // LinePoolStats returns the pages of the line pool held now and the most ever held at once.
