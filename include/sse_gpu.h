@@ -84,7 +84,10 @@ typedef struct {
                                     SSE_SEG_DEFERRED and sse_seg_result.consumed tells how many of its bytes the batch took. The caller
                                     submits the rest (in[consumed:]) for that connection in a later batch, before any newer bytes.
                                   - tool calls / usages / decoded text: sse_collect grows the slot's arenas and decodes the batch again.
-                                  sse_result.overflow reports the SSE_OVF_* bits of what was deferred or grown. Not with SSE_FLAG_KERNEL_FUSED. */
+                                  sse_result.overflow reports the SSE_OVF_* bits of what was deferred or grown. Not with SSE_FLAG_KERNEL_FUSED.
+                                  With batches in flight (n_slots > 1): a deferred rest must reach the connection before its newer bytes,
+                                  so produce-side deferral is only safe while each connection is in at most one uncollected batch. Growing
+                                  the decode arenas has no such limit: the batch is decoded again behind whatever was submitted since. */
 #define SSE_FLAG_COUNTERS 256u /* run counting instantiations of the produce, decode and finalize kernels and keep a block of counters per
                                   slot (sse_counters_read): what the kernels did for the batch. Results are identical; the counting
                                   kernels are slower (DESIGN.md 4.3). Not with SSE_FLAG_KERNEL_FUSED. */
@@ -259,9 +262,12 @@ int sse_release(sse_ctx *ctx, int slot);
 
 /* connection state */
 int sse_reset_conn(sse_ctx *ctx, uint32_t conn);                 /* ordered after already submitted batches */
-int sse_reset_all(sse_ctx *ctx, void *cuda_stream);              /* all connections; async on the stream */
+int sse_reset_all(sse_ctx *ctx, void *cuda_stream);              /* all connections; async on the stream (NULL: ordered
+                                                                    after already submitted batches, like sse_reset_conn) */
 
-/* device-resident replay (bench / roofline measurement): the three stages of sse_submit/sse_collect */
+/* device-resident replay (bench / roofline measurement): the three stages of sse_submit/sse_collect.
+ * sse_upload, sse_launch, sse_download and sse_reset_all with a non-NULL stream are ordered only by the stream passed to them,
+ * not with sse_submit, sse_reset_conn or sse_reset_all(NULL). A caller that mixes the two paths synchronises in between. */
 int sse_upload(sse_ctx *ctx, int slot, uint32_t n_segs, uint32_t in_bytes, void *cuda_stream);
 int sse_launch(sse_ctx *ctx, int slot, uint32_t n_segs, void *cuda_stream);   /* kernels only */
 int sse_download(sse_ctx *ctx, int slot, sse_result *res, void *cuda_stream); /* D2H + sync */

@@ -186,6 +186,26 @@ def cut_bounds(bodies, n_batches: int, seed: int) -> np.ndarray:
     return np.concatenate([np.zeros((n, 1), np.int64), np.minimum(cuts, lens[:, None]), lens[:, None]], axis=1)
 
 
+def fill_pieces(arena, segs, bodies, modes, bounds, b, providers=None) -> int:
+    """Writes piece b of every body (bounds[i, b]:bounds[i, b + 1]) as segment i for connection i into an acquired slot.
+    Returns the batch's input bytes."""
+    n = len(bodies)
+    plen = bounds[:, b + 1] - bounds[:, b]
+    aligned = (plen + 15) & ~15
+    offs = np.zeros(n, dtype=np.int64)
+    offs[1:] = np.cumsum(aligned)[:-1]
+    for i in range(n):
+        if plen[i]:
+            arena[offs[i]:offs[i] + plen[i]] = np.frombuffer(bodies[i], dtype=np.uint8, count=int(plen[i]), offset=int(bounds[i, b]))
+    segs["conn"][:n] = np.arange(n, dtype=np.uint32)
+    segs["in_off"][:n] = offs
+    segs["in_len"][:n] = plen
+    segs["mode"][:n] = modes
+    segs["provider"][:n] = 0 if providers is None else providers
+    segs["reserved"][:n] = 0
+    return int(offs[-1] + aligned[-1])
+
+
 def digest_run(eng, bodies, modes, bounds, providers=None, on_batch=None):
     """Feeds body i in the pieces bounds[i] gives (one micro-batch per piece index, every connection in every batch, empty
     pieces included) and folds every batch result into per-connection digests. modes: one mode for all connections or one per
@@ -199,21 +219,8 @@ def digest_run(eng, bodies, modes, bounds, providers=None, on_batch=None):
     conn = np.arange(n, dtype=np.uint32)
     eng.reset_all()
     for b in range(n_batches):
-        plen = bounds[:, b + 1] - bounds[:, b]
-        aligned = (plen + 15) & ~15
-        offs = np.zeros(n, dtype=np.int64)
-        offs[1:] = np.cumsum(aligned)[:-1]
         slot, arena, segs = eng.acquire()
-        for i in range(n):
-            if plen[i]:
-                arena[offs[i]:offs[i] + plen[i]] = np.frombuffer(bodies[i], dtype=np.uint8, count=int(plen[i]), offset=int(bounds[i, b]))
-        segs["conn"][:n] = conn
-        segs["in_off"][:n] = offs
-        segs["in_len"][:n] = plen
-        segs["mode"][:n] = modes
-        segs["provider"][:n] = 0 if providers is None else providers
-        segs["reserved"][:n] = 0
-        eng.submit(slot, n, int(offs[-1] + aligned[-1]))
+        eng.submit(slot, n, fill_pieces(arena, segs, bodies, modes, bounds, b, providers))
         res = eng.collect(slot)
         try:
             check_result(eng, res, segs[:n])
@@ -223,6 +230,113 @@ def digest_run(eng, bodies, modes, bounds, providers=None, on_batch=None):
         finally:
             eng.release(slot)
     return d, carry, flags
+
+
+class PipelinedDigests:
+    """digest_run with up to `depth` batches in flight: batch b is filled and submitted while up to depth - 1 earlier batches
+    are still uncollected. collect_order "fifo" collects the oldest batch once depth are in flight; "lifo" fills every slot and
+    then collects the newest first. Whatever order they are collected in, results are folded into the digests in fold_order
+    (default: submission order); a collected slot stays unreleased until its turn comes, so fold_order may only move a batch
+    by less than depth places. Every collected batch passes check_result.
+    between(b) runs after submit b and before the next acquire; on_batch(b, result, slot) sees every result, in fold order,
+    before its slot is released. step() submits one batch, so two runs (on two contexts) can be interleaved."""
+
+    def __init__(self, eng, bodies, modes, bounds, depth, collect_order="fifo", providers=None, between=None, on_batch=None,
+                 fold_order=None):
+        assert collect_order in ("fifo", "lifo") and 1 <= depth <= eng.cfg.n_slots
+        self.eng, self.bodies, self.modes, self.bounds, self.providers = eng, bodies, modes, bounds, providers
+        self.depth, self.lifo, self.between, self.on_batch = depth, collect_order == "lifo", between, on_batch
+        self.n = n = len(bodies)
+        self.n_batches = bounds.shape[1] - 1
+        self.order = list(range(self.n_batches)) if fold_order is None else list(fold_order)
+        assert sorted(self.order) == list(range(self.n_batches))
+        self.d = orc.new_digests(n)
+        self.carry = np.zeros(n, dtype=np.uint32)
+        self.flags = np.zeros(n, dtype=np.uint32)
+        self.conn = np.arange(n, dtype=np.uint32)
+        self.inflight = []      # (batch, slot, segs) submitted, not collected, oldest first
+        self.collected = {}     # batch -> (slot, result) collected, not yet folded
+        self.next_batch = 0
+        self.folded = 0
+        eng.reset_all()
+
+    def _collect(self, k):
+        b, slot, segs = self.inflight.pop(k)
+        try:
+            res = self.eng.collect(slot)
+            check_result(self.eng, res, segs)
+        except BaseException:
+            self.eng.release(slot)
+            raise
+        self.collected[b] = (slot, res)
+
+    def _fold_ready(self):
+        while self.folded < self.n_batches and self.order[self.folded] in self.collected:
+            b = self.order[self.folded]
+            slot, res = self.collected.pop(b)
+            try:
+                assert orc.digest_result(res.raw, self.conn, self.d, self.carry, self.flags) == self.n
+                if self.on_batch is not None:
+                    self.on_batch(b, res, slot)
+            finally:
+                self.eng.release(slot)
+            self.folded += 1
+
+    def _drain(self):
+        while self.inflight:
+            self._collect(-1 if self.lifo else 0)
+        self._fold_ready()
+
+    def step(self) -> bool:
+        """Submits the next batch (collecting first where depth batches are held). False once every batch was submitted."""
+        if self.next_batch == self.n_batches:
+            return False
+        while len(self.inflight) + len(self.collected) >= self.depth:
+            assert self.inflight, f"fold order {self.order} holds {self.depth} collected batches: it cannot advance"
+            if self.lifo:
+                self._drain()
+            else:
+                self._collect(0)
+                self._fold_ready()
+        b = self.next_batch
+        slot, arena, segs = self.eng.acquire()
+        try:
+            self.eng.submit(slot, self.n, fill_pieces(arena, segs, self.bodies, self.modes, self.bounds, b, self.providers))
+        except BaseException:
+            self.eng.release(slot)
+            raise
+        self.inflight.append((b, slot, segs[:self.n].copy()))
+        self.next_batch += 1
+        if self.between is not None:
+            self.between(b)
+        return True
+
+    def finish(self):
+        """Submits what is left, collects and folds everything. Returns (digests, carry_len, seg_flags) as digest_run does."""
+        while self.step():
+            pass
+        self._drain()
+        assert self.folded == self.n_batches and not self.collected
+        return self.d, self.carry, self.flags
+
+    def abort(self):
+        """Releases every slot the run still holds (after a failure), so that the context stays usable."""
+        for _, slot, _ in self.inflight:
+            self.eng.release(slot)
+        for slot, _ in self.collected.values():
+            self.eng.release(slot)
+        self.inflight, self.collected = [], {}
+
+
+def digest_run_pipelined(eng, bodies, modes, bounds, depth, collect_order="fifo", providers=None, between=None, on_batch=None,
+                         fold_order=None):
+    """digest_run with depth batches in flight (PipelinedDigests). Returns (digests, carry_len, seg_flags)."""
+    run = PipelinedDigests(eng, bodies, modes, bounds, depth, collect_order, providers, between, on_batch, fold_order)
+    try:
+        return run.finish()
+    except BaseException:
+        run.abort()
+        raise
 
 
 def oracle_digests(bodies, modes):
