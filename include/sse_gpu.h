@@ -236,7 +236,9 @@ void sse_worst_case_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_p
  * continues in pool pages instead of failing the stream; its pages return to the pool when the line completes, when the
  * connection dies or finishes, and on sse_reset_conn / sse_reset_all. A connection fails (SSE_SEG_LINE_TOO_LONG |
  * SSE_SEG_DEAD) only when its line would exceed max_line_bytes or no page is free. A completed pooled line is always
- * materialised in the out arena (never a zero-copy span). Not available with SSE_FLAG_KERNEL_FUSED. */
+ * materialised in the out arena (never a zero-copy span). A payload of 32 KiB or more is decoded by a whole warp (a context
+ * whose longest line, max_line_bytes here or carry_slot_bytes without a pool, is at least that long runs one more kernel per
+ * batch, which sse_launch_count counts). Not available with SSE_FLAG_KERNEL_FUSED. */
 #define SSE_MAX_LINE_BYTES 16777215u   /* decode work items carry a 24-bit payload length */
 typedef struct {
     uint32_t struct_size;      /* sizeof(sse_line_pool) */
@@ -326,6 +328,11 @@ typedef struct {
 } sse_counters;
 /* Byte identity of a batch without SSE_F_DONE_EXACT lines (those get no work item):
  *   d_skip_bytes + d_coop_bytes + d_plain_steps + d_actions + d_abandoned_bytes + d_template_bytes == sum of sse_rec.payload_len.
+ * A long line (a payload of 32 KiB or more, in a context that can hold one) is decoded by a whole warp and counted into the same
+ * fields: one d_pulls and one d_items; its automaton rounds are d_warp_rounds with one busy lane; each jump of the warp over a
+ * string body or digit run is one d_coop_strings, with its 512-byte d_coop_steps and d_coop_bytes (value bodies with their
+ * escapes and UTF-8 sequences); every string it unquotes is one d_unquote_jobs; its cycles are in c_total and the c_* parts
+ * (the jumps in c_coop).
  * Valid after a successful sse_collect or sse_download of the slot and before sse_release. SSE_ERR_ARG: the context has no
  * SSE_FLAG_COUNTERS, or out->struct_size != sizeof(sse_counters); SSE_ERR_BUSY: the slot holds no collected batch. */
 int sse_counters_read(sse_ctx *ctx, int slot, sse_counters *out);

@@ -10,8 +10,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # SSE_LIB: load this prebuilt library instead (A/B runs of build-time knobs on the GPU box, tools/build_variants.sh); never rebuilt
 LIB = os.environ.get("SSE_LIB") or os.path.join(HERE, "libssegpu.so")
-SOURCES = ["sse_fused.cu", "sse_kernel.cu", "sse_kernel2.cu", "sse_host.cu", "sse_fold.cpp", "sse_gateway.cpp"]
-HEADERS = ["sse_device.cuh", "sse_common.cuh", "sse_tables.h", os.path.join("..", "..", "include", "sse_gpu.h"),
+SOURCES = ["sse_fused.cu", "sse_kernel.cu", "sse_kernel2.cu", "sse_long.cu", "sse_host.cu", "sse_fold.cpp", "sse_gateway.cpp"]
+HEADERS = ["sse_device.cuh", "sse_common.cuh", "sse_v2.cuh", "sse_tables.h", os.path.join("..", "..", "include", "sse_gpu.h"),
            os.path.join("..", "..", "include", "sse_gateway.h")]
 
 

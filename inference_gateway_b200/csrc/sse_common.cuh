@@ -476,6 +476,85 @@ __device__ __noinline__ void warp_unquote(const uint8_t *__restrict__ src, uint3
     __syncwarp();
 }
 
+// Warp-parallel unquote of a string body [s, e) the automaton accepted (escapes are well formed; the UTF-8 need not be): the
+// same bytes as json_unquote_write, 32 source bytes per step, one per lane. What a byte is follows from facts local to it: a
+// backslash starts an escape unless the run of backslashes before it has odd length (its parity is carried from step to step),
+// and a byte is inside an earlier unit when an escape or a valid UTF-8 sequence that starts at most 11 bytes before it reaches
+// over it (a max-scan of where the units end, carried from step to step). A byte nothing covers starts a unit: a plain byte, an
+// escape (with its low surrogate when a high one is followed by one, else U+FFFD for a surrogate), a valid sequence (copied), or
+// an invalid byte (U+FFFD). Output positions are a warp prefix sum of the units' lengths. The long-line kernel's (the decode kernel keeps
+// warp_unquote above: its strings are short and mostly plain, and it is compiled as it was before the long-line stage).
+__device__ __noinline__ void warp_unquote_parallel(const uint8_t *__restrict__ src, uint32_t s, uint32_t e, uint8_t *__restrict__ dst, uint32_t *patch) {
+    const uint32_t lane = lane_id();
+    uint32_t n = 0, cover = s, esc_in = 0;       // cover: no earlier unit reaches a byte at or after it; esc_in: a backslash escapes the step's first byte
+    for (uint32_t b = s; b < e; b += 32u) {
+        const uint32_t i = b + lane;
+        const bool in = i < e;
+        const uint32_t c = in ? (uint32_t)src[i] : 0u;
+        const unsigned bsm = __ballot_sync(FULL, in && c == '\\');
+        const unsigned him = __ballot_sync(FULL, in && c >= 0x80u);
+        if (!(bsm | him | esc_in) && cover <= b) {       // plain ASCII: copied as it is
+            if (in) dst[n + lane] = (uint8_t)c;
+            n += min(32u, e - b);
+            continue;
+        }
+        // backslashes right before this byte, and whether they leave it escaped
+        const unsigned nz = ~bsm & ((1u << lane) - 1u);
+        const bool escaped = nz ? (((lane - 1u - (31u - __clz(nz))) & 1u) != 0u) : (((lane + esc_in) & 1u) != 0u);
+        const bool start_esc = in && c == '\\' && !escaped;
+        uint32_t unit_end = 0, r = 0, k = 0;            // (candidate) unit [i, unit_end); r: rune of an escape; k: valid sequence length
+        if (start_esc) {
+            const uint32_t c1 = src[i + 1];
+            unit_end = i + 2u;
+            switch (c1) {
+            case 'b': r = 8; break;
+            case 'f': r = 12; break;
+            case 'n': r = 10; break;
+            case 'r': r = 13; break;
+            case 't': r = 9; break;
+            case 'u': {
+                r = (uint32_t)hex4(src + i + 2u);
+                unit_end = i + 6u;
+                if (r >= 0xD800u && r < 0xE000u) {
+                    int r1 = -1;
+                    if (i + 12u <= e && src[i + 6u] == '\\' && src[i + 7u] == 'u') r1 = hex4(src + i + 8u);
+                    if (r < 0xDC00u && r1 >= 0xDC00 && r1 < 0xE000) { r = 0x10000u + ((r - 0xD800u) << 10) + ((uint32_t)r1 - 0xDC00u); unit_end = i + 12u; }
+                    else r = 0xFFFDu;
+                }
+                break;
+            }
+            default: r = c1; break;     // '"', '\\', '/'
+            }
+        } else if (in && c >= 0x80u) {
+            k = (uint32_t)utf8_valid_len(src + i, (int)(e - i));
+            if (k) unit_end = i + k;
+        }
+        uint32_t reach = unit_end;                       // inclusive max-scan: how far the units starting up to this lane reach
+        #pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(FULL, reach, d); if ((int)lane >= d) reach = max(reach, v); }
+        uint32_t before = __shfl_up_sync(FULL, reach, 1);
+        before = max(lane ? before : 0u, cover);
+        const bool unit = in && before <= i;
+        uint32_t len = 0;
+        if (unit) len = start_esc ? (r < 0x80u ? 1u : r < 0x800u ? 2u : r < 0x10000u ? 3u : 4u) : c < 0x80u ? 1u : (k ? k : 3u);
+        uint32_t incl = len;
+        #pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, d); if ((int)lane >= d) incl += v; }
+        const uint32_t o = n + incl - len;
+        if (unit) {
+            if (start_esc) put_rune(dst, o, r);
+            else if (c < 0x80u) dst[o] = (uint8_t)c;
+            else if (k) { for (uint32_t q = 0; q < k; q++) dst[o + q] = src[i + q]; }
+            else put_rune(dst, o, 0xFFFDu);
+        }
+        n += __shfl_sync(FULL, incl, 31);
+        cover = max(cover, __shfl_sync(FULL, reach, 31));
+        if (~bsm) esc_in = (uint32_t)__clz(~bsm) & 1u;      // the run of backslashes that ends the step (all 32: unchanged)
+    }
+    if (lane == 0) *patch = n;
+    __syncwarp();
+}
+
 struct ParseOut {
     uint32_t flags;
     uint32_t content_off, content_len;

@@ -59,11 +59,20 @@ struct alignas(8) Counters {
     uint32_t n_tiles;      // fused pipeline: tiles written by the plan kernel
     uint32_t reserved1;
     uint32_t overflow;     // SSE_OVF_* bits: which arena was too small (SSE_FLAG_DEFER: also what the produce stage deferred)
-    uint32_t pad[2];
+    uint32_t n_long;       // split pipeline: work items of at least KParams.long_line payload bytes (items_sorted[0, n_long))
+    uint32_t long_ticket;  // split pipeline: next long item for the long-line decode kernel
     // device-only tail (the host reads the struct up to here)
     uint32_t class_count[SSE_N_BUCKETS];  // split pipeline: items per bucket (see item_bucket)
     uint32_t class_cursor[SSE_N_BUCKETS];
+    uint32_t long_cursor;                 // split pipeline: next free place of a long item in items_sorted
 };
+
+// Work items whose payload is at least SSE_LONG_LINE bytes are decoded by a whole warp each (sse_long_decode_kernel) instead of
+// one decode lane, in contexts that can hold a line that long (KParams.long_line). 0: no long-line stage (A/B builds only).
+#ifndef SSE_LONG_LINE
+#define SSE_LONG_LINE 32768
+#endif
+static_assert(SSE_LONG_LINE == 0 || SSE_LONG_LINE > 8192, "the long-line threshold lies above every line a produce window holds");
 
 static_assert(offsetof(Counters, out_bytes) % 8 == 0 && offsetof(Counters, n_items) == offsetof(Counters, out_bytes) + 4 &&
               offsetof(Counters, n_frames) % 8 == 0 && offsetof(Counters, n_recs) == offsetof(Counters, n_frames) + 4,
@@ -101,6 +110,9 @@ struct KParams {
     uint32_t *pool_stack;    uint32_t *pool_next;
     PoolChain *pool_chain;
     uint32_t page_bytes, pool_pages, max_line;
+    // split pipeline: payload length from which a work item goes to the long-line decode kernel (0: the context cannot hold such
+    // a line, and neither the sort nor the launch has a long-line stage)
+    uint32_t long_line;
     // SSE_FLAG_COUNTERS: the slot's counter block (CN_*), which selects the counting kernels; nullptr: the default kernels
     unsigned long long *cnt;
 };
@@ -144,6 +156,9 @@ int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int
 int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device);           // SSE_FLAG_DEFER: stage 2 again (grown arenas)
 int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream);              // line pool: reset one connection (SSE_NONE: all)
 int sse_v2_prepare(int device);                                                        // builds + uploads the automaton tables
+int sse_long_prepare(int device);                                                      // long-line decode kernel: occupancy (sse_long.cu)
+namespace ssetab { struct DfaTables; }
+void sse_launch_long_decode(const KParams &p, const ssetab::DfaTables *tables, void *stream, int sm_count, int device);   // stage 2a
 int sse_fused_prepare(int device);                                                     // fused pipeline: tables + kernel attributes
 int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device);        // plan kernel + fused tile kernel
 uint32_t sse_fused_max_line(void);

@@ -118,6 +118,7 @@ KParams make_params(sse_ctx *c, Slot &s, uint32_t n_segs) {
     p.pool_chain = c->d_pool_chain;
     p.page_bytes = c->pool.page_bytes; p.pool_pages = c->pool.pool_pages;
     p.max_line = c->pool.pool_pages ? c->pool.max_line_bytes : c->cfg.carry_slot_bytes;
+    p.long_line = (SSE_LONG_LINE && !(c->cfg.flags & SSE_FLAG_KERNEL_FUSED) && p.max_line >= SSE_LONG_LINE) ? SSE_LONG_LINE : 0u;
     p.cnt = s.d_cnt;
     return p;
 }
@@ -162,7 +163,7 @@ int do_launch(sse_ctx *c, Slot &s, uint32_t n_segs, cudaStream_t st) {
         else {   // default: produce -> sort -> decode (templates / automaton) -> finalize
             e = sse_launch_produce_kernel(p, (void *)st, c->sm_count);
             if (e == 0) e = sse_launch_decode_finalize(p, (void *)st, c->sm_count, c->device);
-            c->launches += 6;   // produce, bucket hist/scan/scatter, decode, finalize
+            c->launches += p.long_line ? 7 : 6;   // produce, bucket hist/scan/scatter, [long-line decode,] decode, finalize
         }
         if (e != 0) { cu_ok((cudaError_t)e, "stream kernel launch"); return SSE_ERR_CUDA; }
     }
@@ -223,7 +224,8 @@ int redecode(sse_ctx *c, Slot &s, Counters &k, cudaStream_t st, uint32_t &grown)
         if (rc == SSE_OK && (ovf & SSE_OVF_TEXT)) rc = grow(s.d_text, s.h_text, s.cap_text, k.text_bytes, w.text_arena_bytes);
         if (rc != SSE_OK) return rc;
         grown |= ovf;
-        k.n_tcs = k.n_usages = k.text_bytes = 0; k.item_ticket = 0; k.status = SSE_OK; k.overflow = 0;
+        // the lane decoder's items start after the long ones (items_sorted[0, n_long)), which the long-line kernel takes again
+        k.n_tcs = k.n_usages = k.text_bytes = 0; k.item_ticket = k.n_long; k.long_ticket = 0; k.status = SSE_OK; k.overflow = 0;
         *s.h_ctr = k;
         CU(cudaMemcpyAsync(s.d_ctr, s.h_ctr, offsetof(Counters, class_count), cudaMemcpyHostToDevice, st));
         if (s.d_cnt) {   // the decode counters describe the pass whose records the batch returns
@@ -231,9 +233,10 @@ int redecode(sse_ctx *c, Slot &s, Counters &k, cudaStream_t st, uint32_t &grown)
             s.decode_passes++;
         }
         if (c->have_last) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
-        const int e = sse_launch_decode(make_params(c, s, s.n_segs), (void *)st, c->sm_count, c->device);
+        const KParams p = make_params(c, s, s.n_segs);
+        const int e = sse_launch_decode(p, (void *)st, c->sm_count, c->device);
         if (e != 0) { cu_ok((cudaError_t)e, "decode kernel launch"); return SSE_ERR_CUDA; }
-        c->launches += 1;
+        c->launches += p.long_line ? 2 : 1;
         CU(cudaEventRecord(c->last_kernel, st));
         c->have_last = true;
         CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, st));

@@ -8,7 +8,7 @@ mkdir -p variants
 while [ $# -ge 2 ]; do
   name=$1; defs=$2; shift 2
   ( cd inference_gateway_b200/csrc && nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2 -shared -cudart static \
-      $defs -o ../../variants/$name.so sse_fused.cu sse_kernel.cu sse_kernel2.cu sse_host.cu sse_fold.cpp sse_gateway.cpp ) &
+      $defs -o ../../variants/$name.so sse_fused.cu sse_kernel.cu sse_kernel2.cu sse_long.cu sse_host.cu sse_fold.cpp sse_gateway.cpp ) &
 done
 wait
 ls -la variants/
