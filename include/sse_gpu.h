@@ -73,7 +73,8 @@ typedef struct {
 #define SSE_FLAG_KERNEL_FUSED 4u /* single-pass tile kernel (1-D TMA staging, stop bitmap, warp-per-line template replay): reads the payload from HBM
                                     once; slower than the default pipeline on H100 (DESIGN.md 4.3) */
 #define SSE_FLAG_TEMPLATES 16u /* skeleton-template replay: lines whose JSON skeleton was seen before skip the automaton (results identical;
-                                  measured slower than the automaton alone on H100, DESIGN.md 4.3, so off by default) */
+                                  on H100 slower than the automaton alone in most measured shapes, faster in two, DESIGN.md 4.3,
+                                  so off by default) */
 #define SSE_FLAG_COPY_OUT 8u   /* materialise every frame in the out arena. Default: a frame whose bytes already stand in the
                                   caller's input arena exactly as the reference would send them (every mode P line, and a mode R
                                   "data: ...\n" line followed by a blank line) is returned as a span of the input arena and is
