@@ -1,6 +1,6 @@
 // sse_common.cuh -- device helpers shared by the stream kernels: schema of the decoded document, strings.TrimSpace,
-// encoding/json pieces (string / number scanners, unquote, key folding), the sequential per-line decoder (v1 and
-// slow path of v2), run bookkeeping and the long-line path. Included by sse_kernel.cu and sse_kernel2.cu.
+// encoding/json pieces (number checks, unquote, key folding, the lane's unquote queue), run bookkeeping, the long-line
+// path and the line pool. Included by every kernel source.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -30,10 +30,11 @@ enum : uint8_t { TG_NONE, TG_CHOICES, TG_USAGE, TG_PROMPT, TG_COMPLETION, TG_TOT
 struct FieldDef { uint8_t len, ty, sub, tgt; char name[20]; };
 constexpr int N_FIELDS = 39;
 struct alignas(16) Schema { FieldDef f[N_FIELDS]; uint8_t first[N_COUNT]; uint8_t cnt[N_COUNT]; uint8_t pad[2]; };
-static_assert(sizeof(Schema) % 4 == 0, "schema is copied as 32-bit words");
 
+// The one declaration of the schema: in constant memory for the slow key path (escaped, non-ASCII or case-folded keys:
+// match_field), and constexpr, so that the host builds the decode tables from a compile-time copy of it (sse_build_tables).
 #define FD(nm, ty, sub, tgt) { (uint8_t)(sizeof(nm) - 1), ty, sub, tgt, nm }
-__constant__ Schema c_schema = {
+constexpr __constant__ Schema c_schema = {
     {
         /* N_ROOT (0..7) */
         FD("choices", TY_SLICE, A_CHOICES, TG_CHOICES), FD("created", TY_INT, 0, 0), FD("id", TY_STR, 0, 0),
@@ -69,6 +70,7 @@ __constant__ Schema c_schema = {
     /* cnt   */ { 0, 8, 4, 6, 5, 2, 1, 3, 2, 4, 3, 1, 0, 0, 0, 0, 0 },
     { 0, 0 },
 };
+#undef FD
 
 struct LineEnt {
     uint16_t nl;        // window position of the terminating '\n'
@@ -77,8 +79,7 @@ struct LineEnt {
     uint16_t pay_e;
     uint16_t flen;      // emitted frame length (0: nothing emitted)
     uint8_t  kind;      // K_*
-    uint8_t  parse;     // 1: decode payload
-    uint16_t rel;       // split pipeline: index among this round's work items
+    uint16_t rel;       // index among this round's work items
     uint16_t zc;        // 1: the frame's bytes stand in the input arena as they are (no copy; offsets are input offsets)
     uint16_t clen;      // bytes this line occupies in the out arena (frame, or the payload of a swallowed line that is decoded)
 };
@@ -93,7 +94,6 @@ struct WarpSmem {
 };
 
 struct CtaSmem {
-    Schema schema;
     WarpSmem w[WARPS_PER_CTA];
 };
 
@@ -380,7 +380,7 @@ __device__ __noinline__ uint32_t classify_finish(const uint8_t *s, int n) {
     return SSE_FIN_OTHER;
 }
 
-// ---------------------------------------------------------------- the decoder (one lane per line)
+// ---------------------------------------------------------------- unquote queues
 // Deferred unquote jobs of one lane: drained warp-cooperatively (warp_unquote) instead of byte-by-byte on one lane.
 struct UnquoteJob { uint32_t s, e, dst, pad; uint32_t *patch; };
 #ifndef SSE_MAX_JOBS
@@ -388,40 +388,7 @@ struct UnquoteJob { uint32_t s, e, dst, pad; uint32_t *patch; };
 #endif
 constexpr int MAX_JOBS = SSE_MAX_JOBS;   // queue full: the lane unquotes the string itself (slow, exact)
 struct LaneJobs { uint32_t n; uint32_t pad; UnquoteJob j[MAX_JOBS]; };
-
-struct ParseCtx {
-    LaneJobs *jobs = nullptr;   // optional: where to queue unquote work
-    const uint8_t *sm;     // warp window
-    const KParams *P;
-    const Schema *S;
-    bool emitted;          // string spans may point into the out arena
-    int64_t out_delta;     // out_off = out_delta + window position
-};
 struct Span { uint32_t off, len; bool text; };
-
-// dec: 0 = the raw bytes are the decoded string; 1 = has escapes; 2 (or 3) = may also hold invalid UTF-8, which
-// Go replaces by U+FFFD (1 byte -> 3). Decoding is single pass into a bound-sized text-arena allocation.
-__device__ __noinline__ Span capture(const ParseCtx &cx, int s, int e, int dec, uint32_t *patch = nullptr) {
-    Span r;
-    if (!dec && cx.emitted) { r.off = (uint32_t)(cx.out_delta + s); r.len = (uint32_t)(e - s); r.text = false; return r; }
-    const uint32_t raw = (uint32_t)(e - s);
-    r.text = true; r.len = 0; r.off = 0;
-    if (raw == 0) return r;
-    const uint32_t bound = (((dec & 2) ? 3u * raw : raw) + 3u) & ~3u;   // 4-byte aligned allocations
-    uint32_t o = atomicAdd(&cx.P->ctr->text_bytes, bound);
-    if (o + bound > cx.P->cap_text) { sse_overflow(cx.P->ctr, SSE_OVF_TEXT); return r; }
-    r.off = o;
-    if (dec && patch && cx.jobs && cx.jobs->n < (uint32_t)MAX_JOBS) {
-        // the decoded length is patched into *patch when the warp drains the queue; raw > 0 implies decoded > 0
-        UnquoteJob &j = cx.jobs->j[cx.jobs->n++];
-        j.s = (uint32_t)s; j.e = (uint32_t)e; j.dst = o; j.patch = patch;
-        r.len = raw;
-        return r;
-    }
-    if (dec) r.len = json_unquote_write(cx.sm, s, e, cx.P->text + o);
-    else { for (int i = s; i < e; i++) cx.P->text[o + (i - s)] = cx.sm[i]; r.len = raw; }
-    return r;
-}
 
 // Warp-cooperative unquote (same result as json_unquote_write): runs of plain bytes are copied 32 at a time, the byte that
 // stops a run (escape or non-ASCII sequence) is handled by lane 0 with the exact decode.go rules.
@@ -555,12 +522,6 @@ __device__ __noinline__ void warp_unquote_parallel(const uint8_t *__restrict__ s
     __syncwarp();
 }
 
-struct ParseOut {
-    uint32_t flags;
-    uint32_t content_off, content_len;
-    uint32_t tc_first, tc_count, n_choices, usage;
-};
-
 // ---------------------------------------------------------------- warp-cooperative helpers
 // copy n bytes global -> shared so that they END at smem offset `end_off` (byte granularity)
 __device__ void copy_g2s_bytes(uint8_t *sm_dst, const uint8_t *g_src, int n) {
@@ -690,14 +651,13 @@ __device__ __noinline__ bool reserve_long(const KParams &P, RunChain &rc, uint32
 }
 
 // A line that never fit the window, assembled in the connection's carry slot (HBM): classified and emitted straight from
-// global memory. seg >= 0 (split pipeline): its payload becomes a work item like any other line's -- the decode kernel
-// reads payloads from the arenas, so a line of any length up to carry_slot_bytes is decoded. seg < 0 (first-generation
-// kernel): the payload is not decoded (SSE_F_TOO_LONG). at != SSE_NONE: the line already stands in the out arena at offset
-// `at` (a pooled line gathered there, one spare byte after it) and is emitted in place: frame, payload and the swallowed
-// line's materialised payload are spans of it, nothing is copied. resv (SSE_FLAG_DEFER): the line's results go where reserve_long
-// put them (rc.rv), and what the line does not use of that reservation is left as a hole.
+// global memory. Its payload becomes a work item of segment seg like any other line's -- the decode kernel reads payloads
+// from the arenas, so a line of any length up to carry_slot_bytes is decoded. at != SSE_NONE: the line already stands in the
+// out arena at offset `at` (a pooled line gathered there, one spare byte after it) and is emitted in place: frame, payload
+// and the swallowed line's materialised payload are spans of it, nothing is copied. resv (SSE_FLAG_DEFER): the line's results
+// go where reserve_long put them (rc.rv), and what the line does not use of that reservation is left as a hole.
 template <bool RESV>
-__device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, const uint8_t *line, int L, uint32_t mode, int seg = -1,
+__device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, const uint8_t *line, int L, uint32_t mode, uint32_t seg,
                                                uint32_t at = SSE_NONE) {
     const uint32_t lane = lane_id();
     int a = 0, b = L;           // frame source [a, b) ; R: trimmed
@@ -718,9 +678,10 @@ __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, c
     }
     // payload handed to the decoder: [ps, pe) of the line
     const int ps = (mode & SSE_MODE_R) ? (pref ? a + 6 : a) : 6, pe = (mode & SSE_MODE_R) ? b : L - 1;
-    const bool item = seg >= 0 && parse;
-    const bool exact = item && done && pref && pe - ps == 6;          // `data: [DONE]` cannot be this long; kept for symmetry
-    const uint32_t extra = (item && !emit) ? (uint32_t)(pe - ps) : 0u;   // a swallowed line's payload is materialised for the decoder
+    // `data: [DONE]` once its white space is trimmed: nothing to decode, the record is final and there is no work item
+    const bool exact = done && pref && pe - ps == 6;
+    const bool item = parse && !exact;
+    const uint32_t extra = (parse && !emit) ? (uint32_t)(pe - ps) : 0u;   // a swallowed line's payload is materialised for the decoder
     uint32_t nf = emit ? 1u : 0u, nr = parse ? 1u : 0u;
     const bool in_place = at != SSE_NONE;
     uint32_t ob = 0, fb = 0, rb = 0, qb = 0;
@@ -731,11 +692,11 @@ __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, c
             if ((nf || extra) && !in_place) ob = atomicAdd(&P.ctr->out_bytes, ((uint32_t)flen + extra + 15u) & ~15u);
             if (nf) fb = atomicAdd(&P.ctr->n_frames, 1u);
             if (nr) rb = atomicAdd(&P.ctr->n_recs, 1u);
-            if (item && !exact) qb = atomicAdd(&P.ctr->n_items, 1u);
+            if (item) qb = atomicAdd(&P.ctr->n_items, 1u);
         }
         ob = __shfl_sync(FULL, ob, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0); qb = __shfl_sync(FULL, qb, 0);
         bool ovf = (!in_place && (nf || extra) && (ob + (uint32_t)flen + extra + 16u > P.cap_out)) || (nf && fb >= P.cap_frames) ||
-                   (nr && rb >= P.cap_recs) || (item && !exact && qb >= P.cap_items);
+                   (nr && rb >= P.cap_recs) || (item && qb >= P.cap_items);
         if (ovf) { if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT); return false; }
     }
     // frame and payload offsets in the out arena
@@ -752,15 +713,15 @@ __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, c
     if (parse && lane == 0) {
         sse_rec r;
         r.frame = emit ? fb : SSE_NONE;
-        r.flags = item ? (exact ? (SSE_F_DONE_LINE | SSE_F_DONE_EXACT) : 0u) : (SSE_F_TOO_LONG | (done ? SSE_F_DONE_LINE : 0u));
+        r.flags = exact ? (SSE_F_DONE_LINE | SSE_F_DONE_EXACT) : 0u;
         r.content_off = r.content_len = 0; r.tc_first = SSE_NONE; r.tc_count = 0; r.n_choices = 0; r.usage = SSE_NONE;
         r.payload_len = (uint32_t)(pe - ps);
         P.recs[rb] = r;
-        if (item && !exact) {
+        if (item) {
             uint4 it;
             it.x = po;
             it.y = (uint32_t)(pe - ps) | (done ? 0x40000000u : ((mode & SSE_MODE_R) ? 0x80000000u : 0u));
-            it.z = rb; it.w = (uint32_t)seg;
+            it.z = rb; it.w = seg;
             P.items[qb] = it;
         }
     }
@@ -869,7 +830,7 @@ __device__ __noinline__ bool pool_append(const KParams &P, uint32_t conn, const 
 // A pooled line is complete (its last byte, the '\n', was appended): gathered from its pages into the out arena with 16-byte
 // copies, classified and emitted in place by process_long_line, then its pages are returned to the pool.
 template <bool RESV>
-__device__ __noinline__ bool pool_long_line(const KParams &P, RunChain &rc, uint32_t conn, int L, uint32_t mode, int seg) {
+__device__ __noinline__ bool pool_long_line(const KParams &P, RunChain &rc, uint32_t conn, int L, uint32_t mode, uint32_t seg) {
     const uint32_t lane = lane_id(), PB = P.page_bytes;
     const uint32_t bytes = ((uint32_t)L + 1u + 15u) & ~15u;    // + 1: mode R's frame ends in a second '\n'
     uint32_t ob = 0, pg = 0;
@@ -943,7 +904,7 @@ __device__ __noinline__ void drop_newline(const KParams &P, uint32_t conn, uint8
 // is reserved before anything is written, and when that does not fit the line gives its '\n' back: the connection keeps the
 // line's other bytes (clen - 1) and the '\n' is the first byte the caller resubmits.
 template <bool DEFER>
-__device__ __noinline__ bool complete_long_line(const KParams &P, RunChain &rc, uint32_t conn, uint8_t *slot, int clen, uint32_t mode, int seg) {
+__device__ __noinline__ bool complete_long_line(const KParams &P, RunChain &rc, uint32_t conn, uint8_t *slot, int clen, uint32_t mode, uint32_t seg) {
     if (DEFER && !reserve_long(P, rc, (uint32_t)clen)) { drop_newline(P, conn, slot, clen); return false; }
     return clen > (int)P.carry_slot ? pool_long_line<DEFER>(P, rc, conn, clen, mode, seg)
                                     : process_long_line<DEFER>(P, rc, slot, clen, mode, seg);

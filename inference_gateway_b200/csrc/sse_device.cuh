@@ -155,9 +155,10 @@ int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count);    
 int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device);  // split pipeline, stages 2+3
 int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device);           // SSE_FLAG_DEFER: stage 2 again (grown arenas)
 int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream);              // line pool: reset one connection (SSE_NONE: all)
+namespace ssetab { struct DfaTables; }
+int sse_build_tables(ssetab::DfaTables &T);                                            // the decode tables of the schema (host)
 int sse_v2_prepare(int device);                                                        // builds + uploads the automaton tables
 int sse_long_prepare(int device);                                                      // long-line decode kernel: occupancy (sse_long.cu)
-namespace ssetab { struct DfaTables; }
 void sse_launch_long_decode(const KParams &p, const ssetab::DfaTables *tables, void *stream, int sm_count, int device);   // stage 2a
 int sse_fused_prepare(int device);                                                     // fused pipeline: tables + kernel attributes
 int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device);        // plan kernel + fused tile kernel

@@ -1,6 +1,7 @@
-// sse_fused.cu -- the default pipeline: ONE pass over the input arena (plan kernel + fused tile kernel).
+// sse_fused.cu -- the single-pass tile kernel (SSE_FLAG_KERNEL_FUSED): ONE pass over the input arena (plan kernel + fused
+// tile kernel).
 //
-// A CTA owns a tile: up to 64 KB of consecutive connection segments (carry tail of the previous batch + new bytes),
+// A CTA owns a tile: up to 48 KiB (TILE) of consecutive connection segments (carry tail of the previous batch + new bytes),
 // staged from HBM into shared memory by 1-D bulk copies (cp.async.bulk, one per segment, completion on an mbarrier).
 // Everything the reference does per line happens on that tile, so the payload crosses HBM exactly once:
 //
@@ -18,12 +19,12 @@
 //             do not stand in the input as they must be sent go through the warp-cooperative serializer; unterminated
 //             tails go back to the connection's carry slot (what bufio.Reader would hold)
 //
-// A segment that does not fit a tile (carry + bytes > 64 KB) is walked window by window by one CTA (restart at the
-// unterminated line); a line longer than carry_slot_bytes (<= 65,504) fails the connection loudly, as before.
+// A segment that does not fit a tile (carry + bytes > TILE) is walked window by window by one CTA (restart at the
+// unterminated line); a line longer than carry_slot_bytes (<= TILE - 32 = 49,120, sse_fused_max_line) fails the connection
+// loudly.
 // Pure integer/byte work, no tensor cores.
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 #include "sse_common.cuh"
 #include "sse_tables.h"
 
@@ -33,6 +34,7 @@ using namespace ssetab;
 
 constexpr int F_THREADS = 512;
 constexpr int F_WARPS = F_THREADS / 32;
+constexpr int F_CTAS_PER_SM = 2;           // persistent: the grid is this many CTAs per SM, all resident
 constexpr uint32_t TILE = 49152;
 constexpr uint32_t TILE_PAD = 64;
 constexpr uint32_t BM_WORDS = TILE / 32;
@@ -53,6 +55,7 @@ struct FRec { uint16_t n, nonsimple, n_str, n_arr; FRecEv ev[REC_MAX]; };       
 constexpr int HASH_BITS = 7;
 struct FName { uint32_t w[5]; uint32_t len; };           // struct-tag name, zero padded
 struct FFin { uint32_t w[4]; uint8_t len, val, pad[2]; };
+constexpr int N_FIN = SSE_FIN_FUNCTION_CALL;             // finish_reason values with a code of their own: codes 1..N_FIN
 struct FTables {
     uint16_t clssym[256];
     uint8_t tr[(NST * NCLS + 3) & ~3];
@@ -60,7 +63,7 @@ struct FTables {
     uint8_t hash[1 << HASH_BITS];                         // perfect hash of (first 4 bytes | 0x20202020, length) -> name id
     FName name[NNAMES];
     uint16_t field[N_NODES * NNAMES];                     // (struct, name id) -> ty | sub << 4 | tgt << 9 | FIELD_VALID
-    FFin fin[5];
+    FFin fin[N_FIN];                                      // fin[v - 1]: the finish_reason value whose code is v
 };
 static_assert(sizeof(FTables) % 4 == 0, "tables are copied as 32-bit words");
 
@@ -105,7 +108,7 @@ struct FSmem {
     uint32_t bc[16];
     long long prof_t;
 };
-static_assert(sizeof(FSmem) <= 113 * 1024, "two CTAs per SM");
+static_assert(F_CTAS_PER_SM == 2 && sizeof(FSmem) <= 113 * 1024, "two CTAs per SM");
 
 #ifdef SSE_PROF
 __device__ unsigned long long g_prof[160];
@@ -552,7 +555,7 @@ __device__ __noinline__ uint32_t f_match_finish(const FSmem &S, uint32_t s, uint
     uint32_t k[5];
     load_words(S, s, len, k);
     #pragma unroll
-    for (int i = 0; i < 5; i++) {
+    for (int i = 0; i < N_FIN; i++) {
         const FFin &F = S.T.fin[i];
         if (F.len == len && k[0] == F.w[0] && k[1] == F.w[1] && k[2] == F.w[2] && k[3] == F.w[3]) return F.val;
     }
@@ -1706,7 +1709,7 @@ __device__ __noinline__ uint32_t big_segment(const KParams &P, FSmem &S, uint32_
     return phase;
 }
 
-__global__ void __launch_bounds__(F_THREADS, 2)
+__global__ void __launch_bounds__(F_THREADS, F_CTAS_PER_SM)
 sse_fused_kernel(const __grid_constant__ KParams P, const FTables *__restrict__ gT) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     FSmem &S = *reinterpret_cast<FSmem *>(smem_raw);
@@ -1880,28 +1883,26 @@ FTables *g_ftables_dev[16] = { nullptr };
 int sse_fused_prepare(int device) {
     if (device < 0 || device >= 16) return (int)cudaErrorInvalidValue;
     if (g_ftables_dev[device]) return 0;
-    static Schema keep;
-    cudaError_t e = cudaMemcpyFromSymbol(&keep, c_schema, sizeof keep);
-    if (e != cudaSuccess) return (int)e;
-    static ssetab::FieldSrc fs[N_FIELDS];
+    static DfaTables D;
+    if (sse_build_tables(D) != 0) return (int)cudaErrorInvalidValue;
     static FTables T;
     memset(&T, 0, sizeof T);
-    memset(T.hash, 0xFF, sizeof T.hash);
-    int n = 0, n_names = 0;
-    for (int node = 0; node < N_COUNT; node++)
-        for (int k = 0; k < keep.cnt[node]; k++) {
-            const FieldDef &f = keep.f[keep.first[node] + k];
-            fs[n].node = (uint8_t)node; fs[n].name = f.name; fs[n].ty = f.ty; fs[n].sub = f.sub; fs[n].tgt = f.tgt;
-            n++;
-            int id = -1;
-            for (int i = 0; i < n_names; i++) if (T.name[i].len == f.len && !memcmp(T.name[i].w, f.name, f.len)) id = i;
-            if (id < 0) {
-                if (n_names >= NNAMES) return (int)cudaErrorInvalidValue;
-                id = n_names++;
-                memcpy(T.name[id].w, f.name, f.len); T.name[id].len = f.len;
-            }
-            T.field[node * NNAMES + id] = (uint16_t)(f.ty | (f.sub << 4) | (f.tgt << 9) | FIELD_VALID);
-        }
+    memcpy(T.clssym, D.clssym, sizeof T.clssym);
+    memcpy(T.tr, D.tr, NST * NCLS);
+    memcpy(T.field, D.field, sizeof T.field);
+    // the struct-tag names only: build_tables gives them the first ids, and every one of them names a field
+    int n_names = 0;
+    for (int id = 0; id < NNAMES; id++)
+        for (int node = 0; node < N_NODES; node++)
+            if (D.field[node * NNAMES + id] & FIELD_VALID) n_names = id + 1;
+    for (int i = 0; i < n_names; i++) { memcpy(T.name[i].w, D.nword[i], sizeof T.name[i].w); T.name[i].len = D.nlen[i]; }
+    for (int id = 0; id < NNAMES; id++) {
+        const uint32_t v = D.finmap[id];
+        if (v == 0xFFu) continue;
+        if (v < 1u || v > (uint32_t)N_FIN || D.nlen[id] > sizeof T.fin[0].w) return (int)cudaErrorInvalidValue;
+        FFin &F = T.fin[v - 1];
+        memcpy(F.w, D.nword[id], sizeof F.w); F.len = D.nlen[id]; F.val = (uint8_t)v;
+    }
     // perfect hash: the first odd multiplier under which the names fall into distinct slots
     uint32_t mul = 0x9E3779B1u;
     for (int tries = 0; tries < 100000; tries++, mul += 0x632BE5ABu * 2u) {
@@ -1915,15 +1916,8 @@ int sse_fused_prepare(int device) {
         if (ok) { memcpy(T.hash, used, sizeof used); T.hash_mul = mul; break; }
     }
     if (!T.hash_mul) return (int)cudaErrorInvalidValue;
-    static const char *fin_names[] = { "stop", "tool_calls", "length", "content_filter", "function_call" };
-    static const uint8_t fin_vals[] = { SSE_FIN_STOP, SSE_FIN_TOOL_CALLS, SSE_FIN_LENGTH, SSE_FIN_CONTENT_FILTER, SSE_FIN_FUNCTION_CALL };
-    for (int i = 0; i < 5; i++) { memcpy(T.fin[i].w, fin_names[i], strlen(fin_names[i])); T.fin[i].len = (uint8_t)strlen(fin_names[i]); T.fin[i].val = fin_vals[i]; }
-    static ssetab::DfaTables D;
-    if (ssetab::build_tables(D, fs, n, fin_names, fin_vals, 5) != 0) return (int)cudaErrorInvalidValue;
-    memcpy(T.clssym, D.clssym, sizeof T.clssym);
-    memcpy(T.tr, D.tr, NST * NCLS);
     FTables *d = nullptr;
-    e = cudaMalloc((void **)&d, sizeof T);
+    cudaError_t e = cudaMalloc((void **)&d, sizeof T);
     if (e != cudaSuccess) return (int)e;
     e = cudaMemcpy(d, &T, sizeof T, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) return (int)e;
@@ -1952,9 +1946,7 @@ int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device) {
     sse_plan_kernel<<<(groups + 3) / 4, 128, 0, (cudaStream_t)stream>>>(p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return (int)e;
-    static int per_sm = 0;
-    if (!per_sm) { const char *e = getenv("SSE_CTAS_PER_SM"); per_sm = e ? atoi(e) : 2; if (per_sm < 1 || per_sm > 2) per_sm = 2; }
-    int grid = sm_count * per_sm;  // persistent: two resident CTAs per SM pull tiles by ticket
-    sse_fused_kernel<<<grid, F_THREADS, sizeof(FSmem), (cudaStream_t)stream>>>(p, g_ftables_dev[device]);
+    // persistent: the resident CTAs pull tiles by ticket
+    sse_fused_kernel<<<sm_count * F_CTAS_PER_SM, F_THREADS, sizeof(FSmem), (cudaStream_t)stream>>>(p, g_ftables_dev[device]);
     return (int)cudaGetLastError();
 }

@@ -7,9 +7,9 @@
 //   emit     frame table; a frame that stands in the input arena as it must be sent is a span of it (zero-copy), the others
 //            go through the warp-cooperative serializer into the out arena      (agent.go:195 / routes.go:613)
 //   items    a stub record + a 16-byte work item per line to decode (lines longer than the window are assembled in the carry
-//            slot, past it in line-pool pages, and become work items too); sse_kernel2.cu sorts the items, decodes them (sse_decode_kernel) and resolves
-//            early termination (sse_finalize_kernel). The template parameter SPLIT is always true: the first-generation
-//            kernel that decoded in place (SPLIT = false) was removed in round 2.
+//            slot, past it in line-pool pages, and become work items too); sse_kernel2.cu sorts the items, decodes them
+//            (sse_decode_kernel) and resolves early termination (sse_finalize_kernel). An exact `data: [DONE]` line has nothing
+//            to decode: its record is written here, final, and it gets no work item.
 //   finish   carry update, per-segment result
 //
 // Pure integer/byte work, no tensor cores.
@@ -54,17 +54,11 @@ __device__ __forceinline__ void tally_long_line(const KParams &P, WarpTally &T, 
 
 // DEFER: SSE_FLAG_DEFER (its own instantiation: the cold deferral paths do not weigh on the default kernel's registers)
 // CNT: SSE_FLAG_COUNTERS (its own instantiation: with CNT = false every counting statement is compiled out)
-template <bool SPLIT, bool DEFER, bool CNT>
+template <bool DEFER, bool CNT>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, SSE_V1_MINB)
 sse_stream_kernel(const __grid_constant__ KParams P) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     CtaSmem &cs = *reinterpret_cast<CtaSmem *>(smem_raw);
-    {   // schema table: constant -> shared (lanes index it divergently)
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(&c_schema);
-        uint32_t *dst = reinterpret_cast<uint32_t *>(&cs.schema);
-        for (int i = threadIdx.x; i < (int)(sizeof(Schema) / 4); i += blockDim.x) dst[i] = src[i];
-    }
-    __syncthreads();
     WarpSmem &W = cs.w[threadIdx.x >> 5];
     uint8_t *buf = W.buf;
     const uint32_t lane = lane_id();
@@ -96,7 +90,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
         RunChain rc; rc.have_first = false; rc.last_idx = SSE_NONE; rc.pre = SSE_NONE;
         rc.first.frame_first = rc.first.frame_count = rc.first.rec_first = rc.first.rec_count = 0; rc.first.next = SSE_NONE;
         uint32_t seg_flags = 0;
-        if (SPLIT && lane == 0) P.seg_term[s] = SSE_NONE;
+        if (lane == 0) P.seg_term[s] = SSE_NONE;
 
         if (cst.flags & (CONN_FINISHED | CONN_DEAD)) {
             if (lane == 0) {
@@ -124,7 +118,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
         // overflow: the segment stops. Without SSE_FLAG_DEFER the batch has failed; with it the rest of the segment is deferred
         // and `consumed` becomes the input-arena offset of the first byte not taken (before seg.in_off: that line starts in the
         // carried tail)
-        bool terminated = false, dead = false, overflow = false;
+        bool dead = false, overflow = false;
 
         for (;;) {   // windows
             const int A = (pend + 15) & ~15;
@@ -171,7 +165,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                 const bool had_first = rc.have_first;
                 const uint32_t last_before = rc.last_idx;
                 if constexpr (CNT) pages = pool_held(P, conn);
-                const bool completed = complete_long_line<DEFER>(P, rc, conn, slot, clen, mode, SPLIT ? (int)s : -1);
+                const bool completed = complete_long_line<DEFER>(P, rc, conn, slot, clen, mode, s);
                 if constexpr (CNT) {
                     tally_pages(T, pages, pool_held(P, conn));
                     if (completed) tally_long_line(P, T, rc, had_first, last_before);
@@ -265,10 +259,10 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                         }
                         LineEnt &e = W.lt[i];
                         e.src_s = (uint16_t)src_s; e.pay_s = (uint16_t)pay_s; e.pay_e = (uint16_t)pay_e;
-                        // bytes to materialise: a frame that is not a span of the input; in the split pipeline also the payload of a
-                        // swallowed "[DONE]"-containing line (agent.go:182: still parsed), which the decode kernel reads from an arena
-                        const int clen = zc ? 0 : (flen ? flen : ((SPLIT && kind == K_DONE) ? pay_e - pay_s : 0));
-                        e.flen = (uint16_t)flen; e.kind = (uint8_t)kind; e.parse = (uint8_t)parse; e.zc = (uint16_t)zc; e.clen = (uint16_t)clen;
+                        // bytes to materialise: a frame that is not a span of the input; also the payload of a swallowed
+                        // "[DONE]"-containing line (agent.go:182: still parsed), which the decode kernel reads from an arena
+                        const int clen = zc ? 0 : (flen ? flen : (kind == K_DONE ? pay_e - pay_s : 0));
+                        e.flen = (uint16_t)flen; e.kind = (uint8_t)kind; e.zc = (uint16_t)zc; e.clen = (uint16_t)clen;
                         my_flen[h] = (uint32_t)flen; my_kind[h] = kind; my_parse[h] = parse; my_zc[h] = zc; my_clen[h] = (uint32_t)clen;
                     }
                 }
@@ -286,26 +280,23 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                     pre_b[h] = tot_b + sb - vb; pre_f[h] = tot_f + sf - vf; pre_r[h] = tot_r + sr - vr;
                     tot_b += __shfl_sync(FULL, sb, 31); tot_f += __shfl_sync(FULL, sf, 31); tot_r += __shfl_sync(FULL, sr, 31);
                 }
-                // split pipeline: every line to decode is a work item; index = rank among this round's items
-                uint32_t tot_q = 0, qb = 0;
-                if (SPLIT) {
-                    uint32_t my_q = 0;
-                    #pragma unroll
-                    for (int h = 0; h < 2; h++) my_q += (my_parse[h] && (my_kind[h] == K_EMIT || my_kind[h] == K_DONE)) ? 1u : 0u;
-                    uint32_t pre_q = my_q;
-                    #pragma unroll
-                    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(FULL, pre_q, d); if ((int)lane >= d) pre_q += t; }
-                    tot_q = __shfl_sync(FULL, pre_q, 31);
-                    pre_q -= my_q;
-                    #pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        int i = (int)lane + 32 * h;
-                        if (i < n_lines && my_parse[h] && (my_kind[h] == K_EMIT || my_kind[h] == K_DONE))
-                            W.lt[i].rel = (uint16_t)(pre_q + ((h == 1 && my_parse[0] && (my_kind[0] == K_EMIT || my_kind[0] == K_DONE)) ? 1u : 0u));
-                    }
-                    __syncwarp();
+                // every line to decode is a work item; index = rank among this round's items
+                uint32_t my_q = 0;
+                #pragma unroll
+                for (int h = 0; h < 2; h++) my_q += (my_parse[h] && (my_kind[h] == K_EMIT || my_kind[h] == K_DONE)) ? 1u : 0u;
+                uint32_t pre_q = my_q;
+                #pragma unroll
+                for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(FULL, pre_q, d); if ((int)lane >= d) pre_q += t; }
+                const uint32_t tot_q = __shfl_sync(FULL, pre_q, 31);
+                pre_q -= my_q;
+                #pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    int i = (int)lane + 32 * h;
+                    if (i < n_lines && my_parse[h] && (my_kind[h] == K_EMIT || my_kind[h] == K_DONE))
+                        W.lt[i].rel = (uint16_t)(pre_q + ((h == 1 && my_parse[0] && (my_kind[0] == K_EMIT || my_kind[0] == K_DONE)) ? 1u : 0u));
                 }
-                uint32_t ob = 0, fb = 0, rb = 0;
+                __syncwarp();
+                uint32_t ob = 0, qb = 0, fb = 0, rb = 0;
                 if (lane == 0) {     // the round's allocation: two 64-bit atomics (Counters: out_bytes | n_items, n_frames | n_recs)
                     const unsigned long long a0 = (unsigned long long)((tot_b + 15u) & ~15u) | ((unsigned long long)tot_q << 32);
                     const unsigned long long a1 = (unsigned long long)tot_f | ((unsigned long long)tot_r << 32);
@@ -317,14 +308,13 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                 ob = __shfl_sync(FULL, ob, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0); qb = __shfl_sync(FULL, qb, 0);
                 if constexpr (CNT) T.add(CN_P_ROUNDS, 1);
                 if (!DEFER) {
-                    if (ob + tot_b + 16 > P.cap_out || fb + tot_f > P.cap_frames || rb + tot_r > P.cap_recs ||
-                        (SPLIT && qb + tot_q > P.cap_items)) {
+                    if (ob + tot_b + 16 > P.cap_out || fb + tot_f > P.cap_frames || rb + tot_r > P.cap_recs || qb + tot_q > P.cap_items) {
                         if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT);
                         overflow = true; break;
                     }
                 } else {
                     const bool fits = !(ob + tot_b + 16 > P.cap_out || fb + tot_f > P.cap_frames || rb + tot_r > P.cap_recs ||
-                                        (SPLIT && qb + tot_q > P.cap_items));
+                                        qb + tot_q > P.cap_items);
                     const bool need_run = rc.have_first && (tot_f | tot_r) != 0u;
                     if ((!fits || need_run) && !admit_round(P, rc, fits, qb, tot_q, need_run)) {
                         consumed = pos + in_delta;   // the segment stops before this round
@@ -368,80 +358,39 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                         o += e.clen;
                     }
                 }
-                // decode: one lane per line
-                uint32_t term_line = 0xFFFFu;
-                constexpr int UNROLL_DEC = SPLIT ? 2 : 1;   // the produce stage only writes a stub and a work item here
-                #pragma unroll UNROLL_DEC
+                // records, one lane per line: a line to decode gets a stub record and a work item; an exact `data: [DONE]` line
+                // (only A6's loop end, agent.go:385-396) gets its final record
+                #pragma unroll
                 for (int h = 0; h < 2; h++) {
                     int i = (int)lane + 32 * h;
                     if (i < n_lines && my_parse[h]) {
                         const LineEnt e = W.lt[i];
-                        ParseCtx cx; cx.sm = buf; cx.P = &P; cx.S = &cs.schema;
-                        cx.emitted = my_kind[h] == K_EMIT;
-                        cx.out_delta = e.zc ? (int64_t)P.in_base + in_delta
-                                            : (int64_t)(ob + pre_b[h]) - (int64_t)(e.flen ? e.src_s : e.pay_s);
-                        if (SPLIT && (my_kind[h] == K_EMIT || my_kind[h] == K_DONE)) {
-                            const bool swallowed = my_kind[h] == K_DONE;
-                            sse_rec stub;
-                            stub.frame = swallowed ? SSE_NONE : fb + pre_f[h]; stub.flags = 0; stub.content_off = stub.content_len = 0; stub.tc_first = SSE_NONE;
-                            stub.tc_count = 0; stub.n_choices = 0; stub.usage = SSE_NONE; stub.payload_len = (uint32_t)(e.pay_e - e.pay_s);
-                            P.recs[rb + pre_r[h]] = stub;
-                            uint4 it;
-                            it.x = (uint32_t)(cx.out_delta + (int64_t)e.pay_s);
-                            it.z = rb + pre_r[h];
-                            // scheduling key of the decode kernel's item sort: provider hint x position of the line in its round; the
-                            // second decoded line of a round (first content delta, the longest) sorts first: long work early
-                            const uint32_t ord = min((uint32_t)e.rel, 7u);
-                            const uint32_t cls = ((ord == 1u ? 0u : (ord == 0u ? 1u : ord)) << 2) | (seg.provider & 3u);
-                            // bit 31: the line can terminate the stream (emitted, mode R); bit 30: swallowed line (SSE_F_DONE_LINE)
-                            it.y = (uint32_t)(e.pay_e - e.pay_s) | (cls << 24) | (swallowed ? 0x40000000u : ((mode & SSE_MODE_R) ? 0x80000000u : 0u));
-                            it.w = s;
-                            P.items[qb + e.rel] = it;
-                            continue;
-                        }
-                        ParseOut po;
-                        // (split pipeline: only exact "[DONE]" payloads get here, the sequential decoder is not part of that kernel)
-                        po.flags = 0; po.content_off = po.content_len = 0; po.tc_first = SSE_NONE; po.tc_count = po.n_choices = 0; po.usage = SSE_NONE;
+                        const bool exact = my_kind[h] == K_DONE_EXACT, swallowed = my_kind[h] == K_DONE;
                         sse_rec r;
-                        r.frame = cx.emitted ? fb + pre_f[h] : SSE_NONE;
-                        r.flags = po.flags;
-                        if (my_kind[h] == K_DONE) r.flags |= SSE_F_DONE_LINE;
-                        if (my_kind[h] == K_DONE_EXACT) r.flags = SSE_F_DONE_LINE | SSE_F_DONE_EXACT;
-                        uint32_t fin = (po.flags & SSE_F_FINISH_MASK) >> SSE_F_FINISH_SHIFT;
-                        if ((mode & SSE_MODE_R) && my_kind[h] == K_EMIT && (po.flags & SSE_F_JSON_OK) && po.n_choices > 0 &&
-                            (fin == SSE_FIN_STOP || fin == SSE_FIN_TOOL_CALLS)) {            // agent.go:235-242
-                            r.flags |= SSE_F_TERMINATES;
-                            term_line = min(term_line, (uint32_t)i);
-                        }
-                        r.content_off = po.content_off; r.content_len = po.content_len;
-                        r.tc_first = po.tc_first; r.tc_count = (uint16_t)min(po.tc_count, 0xFFFFu);
-                        r.n_choices = (uint16_t)min(po.n_choices, 0xFFFFu);
-                        r.usage = po.usage; r.payload_len = (uint32_t)(e.pay_e - e.pay_s);
-                        if (my_kind[h] == K_DONE_EXACT) { r.content_off = r.content_len = 0; r.tc_first = SSE_NONE; r.tc_count = 0; r.n_choices = 0; r.usage = SSE_NONE; }
+                        r.frame = my_kind[h] == K_EMIT ? fb + pre_f[h] : SSE_NONE; r.flags = exact ? SSE_F_DONE_LINE | SSE_F_DONE_EXACT : 0u;
+                        r.content_off = r.content_len = 0; r.tc_first = SSE_NONE; r.tc_count = 0; r.n_choices = 0; r.usage = SSE_NONE;
+                        r.payload_len = (uint32_t)(e.pay_e - e.pay_s);
                         P.recs[rb + pre_r[h]] = r;
+                        if (exact) continue;
+                        uint4 it;
+                        // the payload's arena offset: in the input (zero-copy) or where the line was materialised
+                        it.x = e.zc ? P.in_base + (uint32_t)(in_delta + (int)e.pay_s) : ob + pre_b[h] + (uint32_t)(e.pay_s - (e.flen ? e.src_s : e.pay_s));
+                        it.z = rb + pre_r[h];
+                        // scheduling key of the decode kernel's item sort: provider hint x position of the line in its round; the
+                        // second decoded line of a round (first content delta, the longest) sorts first: long work early
+                        const uint32_t ord = min((uint32_t)e.rel, 7u);
+                        const uint32_t cls = ((ord == 1u ? 0u : (ord == 0u ? 1u : ord)) << 2) | (seg.provider & 3u);
+                        // bit 31: the line can terminate the stream (emitted, mode R); bit 30: swallowed line (SSE_F_DONE_LINE)
+                        it.y = (uint32_t)(e.pay_e - e.pay_s) | (cls << 24) | (swallowed ? 0x40000000u : ((mode & SSE_MODE_R) ? 0x80000000u : 0u));
+                        it.w = s;
+                        P.items[qb + e.rel] = it;
                     }
                 }
-                #pragma unroll
-                for (int d = 16; d >= 1; d >>= 1) term_line = min(term_line, __shfl_xor_sync(FULL, term_line, d));
-                uint32_t run_f = tot_f, run_r = tot_r;
-                if (term_line != 0xFFFFu) {
-                    // lines after the terminating chunk are never read by the reference: cut the run there
-                    uint32_t cf = 0, cr = 0;
-                    #pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        int i = (int)lane + 32 * h;
-                        if (i < n_lines && (uint32_t)i <= term_line) { cf += my_flen[h] ? 1u : 0u; cr += my_parse[h]; }
-                    }
-                    #pragma unroll
-                    for (int d = 16; d >= 1; d >>= 1) { cf += __shfl_xor_sync(FULL, cf, d); cr += __shfl_xor_sync(FULL, cr, d); }
-                    run_f = cf; run_r = cr; terminated = true;
-                }
-                append_run(P, rc, fb, run_f, rb, run_r);
+                append_run(P, rc, fb, tot_f, rb, tot_r);
                 pos = (int)W.lt[n_lines - 1].nl + 1;
                 __syncwarp();
-                if (terminated) break;
             }
-            if (terminated || overflow) break;
+            if (overflow) break;
 
             const int tail = fill - pos;
             // A tail is at most one window (BUF bytes) and sse_init refuses a carry slot shorter than BUF + 16, so the two slot
@@ -481,7 +430,6 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
             }
         }
 
-        if (terminated) seg_flags |= SSE_SEG_TERMINATED;
         if (dead) seg_flags |= SSE_SEG_LINE_TOO_LONG | SSE_SEG_DEAD;
         const bool deferred = DEFER && overflow;
         if (deferred) seg_flags |= SSE_SEG_DEFERRED;
@@ -492,8 +440,8 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                 // deferred at the first line, which starts in the carried tail: the connection is left exactly as it was
                 ns = P.conns[conn]; consumed = 0;
             } else {
-                ns.carry_len = (terminated || dead) ? 0u : (uint32_t)clen;
-                ns.flags = (terminated ? CONN_FINISHED : 0u) | (dead ? CONN_DEAD : 0u) | ((in_long && !terminated && !dead) ? CONN_LONG : 0u);
+                ns.carry_len = dead ? 0u : (uint32_t)clen;
+                ns.flags = dead ? CONN_DEAD : (in_long ? CONN_LONG : 0u);
                 P.conns[conn] = ns;
             }
             sse_seg_result r; r.run = rc.first; r.carry_len = ns.carry_len; r.flags = seg_flags;
@@ -507,16 +455,16 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
 
 } // namespace
 
-template <bool SPLIT, bool DEFER, bool CNT>
-static int launch_v1(const KParams &p, void *stream, int sm_count) {
+template <bool DEFER, bool CNT>
+static int launch_stream_kernel(const KParams &p, void *stream, int sm_count) {
     static bool attr_set = false;
     static int ctas_per_sm = 0;
     const size_t smem = sizeof(CtaSmem);
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(sse_stream_kernel<SPLIT, DEFER, CNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(sse_stream_kernel<DEFER, CNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return (int)e;
         int n = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sse_stream_kernel<SPLIT, DEFER, CNT>, WARPS_PER_CTA * 32, smem);
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sse_stream_kernel<DEFER, CNT>, WARPS_PER_CTA * 32, smem);
         if (e != cudaSuccess) return (int)e;
         ctas_per_sm = n > 0 ? n : 1;
         attr_set = true;
@@ -524,11 +472,11 @@ static int launch_v1(const KParams &p, void *stream, int sm_count) {
     int grid = sm_count * ctas_per_sm;   // persistent: one resident wave, warps pull segments by ticket
     int need = (int)((p.n_segs + WARPS_PER_CTA - 1) / WARPS_PER_CTA);
     if (need < grid) grid = need > 0 ? need : 1;
-    sse_stream_kernel<SPLIT, DEFER, CNT><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(p);
+    sse_stream_kernel<DEFER, CNT><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(p);
     return (int)cudaGetLastError();
 }
 
 int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count) {
-    if (p.cnt) return (p.flags & SSE_FLAG_DEFER) ? launch_v1<true, true, true>(p, stream, sm_count) : launch_v1<true, false, true>(p, stream, sm_count);
-    return (p.flags & SSE_FLAG_DEFER) ? launch_v1<true, true, false>(p, stream, sm_count) : launch_v1<true, false, false>(p, stream, sm_count);
+    if (p.cnt) return (p.flags & SSE_FLAG_DEFER) ? launch_stream_kernel<true, true>(p, stream, sm_count) : launch_stream_kernel<false, true>(p, stream, sm_count);
+    return (p.flags & SSE_FLAG_DEFER) ? launch_stream_kernel<true, false>(p, stream, sm_count) : launch_stream_kernel<false, false>(p, stream, sm_count);
 }

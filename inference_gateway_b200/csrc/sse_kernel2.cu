@@ -642,26 +642,30 @@ DfaTables *g_tables_dev[16] = { nullptr };
 
 } // namespace
 
-int sse_v2_prepare(int device) {
-    if (device < 0 || device >= 16) return (int)cudaErrorInvalidValue;
-    if (g_tables_dev[device]) return 0;
-    static Schema keep;   // field names must outlive build_tables
-    cudaError_t e = cudaMemcpyFromSymbol(&keep, c_schema, sizeof keep);
-    if (e != cudaSuccess) return (int)e;
-    static ssetab::FieldSrc fs[N_FIELDS];
+int sse_build_tables(ssetab::DfaTables &T) {
+    static_assert(ssetab::N_NODES == N_COUNT, "the field table has a row per schema node");
+    static constexpr Schema S = c_schema;     // the host's copy, made at compile time (host code does not read constant memory)
+    ssetab::FieldSrc fs[N_FIELDS];
     int n = 0;
     for (int node = 0; node < N_COUNT; node++)
-        for (int k = 0; k < keep.cnt[node]; k++) {
-            const FieldDef &f = keep.f[keep.first[node] + k];
+        for (int k = 0; k < S.cnt[node]; k++) {
+            const FieldDef &f = S.f[S.first[node] + k];
             fs[n].node = (uint8_t)node; fs[n].name = f.name; fs[n].ty = f.ty; fs[n].sub = f.sub; fs[n].tgt = f.tgt;
             n++;
         }
-    static const char *fin_names[] = { "stop", "tool_calls", "length", "content_filter", "function_call" };
+    // finish_reason values with a code of their own (common_types.go:33-39); any other non-empty value is SSE_FIN_OTHER
+    static const char *const fin_names[] = { "stop", "tool_calls", "length", "content_filter", "function_call" };
     static const uint8_t fin_vals[] = { SSE_FIN_STOP, SSE_FIN_TOOL_CALLS, SSE_FIN_LENGTH, SSE_FIN_CONTENT_FILTER, SSE_FIN_FUNCTION_CALL };
+    return ssetab::build_tables(T, fs, n, fin_names, fin_vals, 5);
+}
+
+int sse_v2_prepare(int device) {
+    if (device < 0 || device >= 16) return (int)cudaErrorInvalidValue;
+    if (g_tables_dev[device]) return 0;
     static ssetab::DfaTables T;
-    if (ssetab::build_tables(T, fs, n, fin_names, fin_vals, 5) != 0) return (int)cudaErrorInvalidValue;
+    if (sse_build_tables(T) != 0) return (int)cudaErrorInvalidValue;
     DfaTables *d = nullptr;
-    e = cudaMalloc((void **)&d, sizeof T);
+    cudaError_t e = cudaMalloc((void **)&d, sizeof T);
     if (e != cudaSuccess) return (int)e;
     e = cudaMemcpy(d, &T, sizeof T, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) return (int)e;

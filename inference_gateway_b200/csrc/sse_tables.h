@@ -38,11 +38,7 @@ enum : uint8_t {
 constexpr uint16_t CLS_ESC = 0x2000, CLS_HI = 0x4000;   // clssym flags: backslash, byte >= 0x80 (>> 13 gives the per-string flag bits)
 constexpr int NAME_WORDS = 5, NAME_LEN_MAX = 4 * NAME_WORDS;   // longest name: 20 bytes
 constexpr int NHASH_BITS = 7;
-
-// schema enums (same values as sse_common.cuh)
-enum : uint8_t { TTY_SKIP, TTY_STR, TTY_PSTR, TTY_INT, TTY_F32, TTY_STRUCT, TTY_PSTRUCT, TTY_SLICE, TTY_PSLICE,
-                 TTY_GOOGLE, TTY_ROOT, TTY_TS };
-constexpr int N_NODES = 17;
+constexpr int N_NODES = 17;                // the schema's node count (N_COUNT, sse_common.cuh)
 constexpr int NNAMES = 40;
 constexpr uint16_t FIELD_VALID = 0x8000;   // field entry: ty | sub << 4 | tgt << 9 | FIELD_VALID
 

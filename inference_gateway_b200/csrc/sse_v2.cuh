@@ -105,19 +105,37 @@ __device__ __noinline__ uint32_t body_name(const uint8_t *base, const DfaTables 
     return id | (upper ? 0x100u : 0u);
 }
 
-// Span of a captured string: without escapes it is the payload's own bytes (no call, nothing through local memory); the
-// rare decoded case goes through capture() (text-arena allocation + queued warp-cooperative unquote).
+// A captured string the decoder has to unquote [s, e) of the payload arena. dec: 1 = has escapes; 2 (or 3) = may also hold
+// invalid UTF-8, which Go replaces by U+FFFD (1 byte -> 3). It gets a text-arena allocation of that bound (4-byte aligned) and
+// goes on the lane's queue, whose decoded length the warp patches into *patch; when the queue is full the lane decodes it.
+__device__ __noinline__ Span capture_text(const KParams &P, LaneJobs *J, uint32_t s, uint32_t e, int dec, uint32_t *patch) {
+    Span r;
+    const uint32_t raw = e - s;
+    r.text = true; r.len = 0; r.off = 0;
+    if (raw == 0) return r;
+    const uint32_t bound = (((dec & 2) ? 3u * raw : raw) + 3u) & ~3u;
+    const uint32_t o = atomicAdd(&P.ctr->text_bytes, bound);
+    if (o + bound > P.cap_text) { sse_overflow(P.ctr, SSE_OVF_TEXT); return r; }
+    r.off = o;
+    if (J->n < (uint32_t)MAX_JOBS) {      // raw > 0 implies decoded > 0
+        UnquoteJob &j = J->j[J->n++];
+        j.s = s; j.e = e; j.dst = o; j.patch = patch;
+        r.len = raw;
+        return r;
+    }
+    r.len = json_unquote_write(P.out, (int)s, (int)e, P.text + o);
+    return r;
+}
+// Span of a captured string: without escapes it is the payload's own bytes (no call, nothing through local memory)
 __device__ __forceinline__ Span capture_v2(const KParams &P, LaneJobs *J, uint32_t s, uint32_t e, int dec, uint32_t *patch) {
     if (!dec) { Span r; r.off = s; r.len = e - s; r.text = false; return r; }
-    ParseCtx cx; cx.jobs = J; cx.sm = P.out; cx.P = &P; cx.S = nullptr; cx.emitted = true; cx.out_delta = 0;
-    return capture(cx, (int)s, (int)e, dec, patch);
+    return capture_text(P, J, s, e, dec, patch);
 }
 // The long-line kernel's unquote queue: long enough that every string to decode goes on it (it is drained every ROUNDS rounds,
 // and a round captures at most one tool-call element, 4 strings; a line adds its content once).
 constexpr int LONG_JOBS = 4 * ROUNDS + 1;
 struct LongJobs { uint32_t n; uint32_t pad; UnquoteJob j[LONG_JOBS]; };
-// capture() for the long-line kernel: the same text-arena allocation (raw length, 3x with invalid UTF-8, 4-byte aligned), and the
-// decode always queued for the warp
+// capture_v2 for the long-line kernel: the same text-arena allocation, and the decode always queued for the warp
 __device__ __noinline__ Span capture_v2(const KParams &P, LongJobs *J, uint32_t s, uint32_t e, int dec, uint32_t *patch) {
     Span r;
     if (!dec) { r.off = s; r.len = e - s; r.text = false; return r; }

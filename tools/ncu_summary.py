@@ -23,7 +23,7 @@ WANT = ["gpu__time_duration.sum", "dram__bytes_read.sum", "dram__bytes_write.sum
         "smsp__average_warps_issue_stalled_short_scoreboard_per_issue_active.ratio",
         "smsp__average_warps_issue_stalled_branch_resolving_per_issue_active.ratio",
         "lts__t_sector_hit_rate.pct", "launch__grid_size", "launch__block_size"]
-HEAD = {"produce": "stage 1 of the split pipeline: sse_stream_kernel<SPLIT=true> (stage, split, classify, frame table, work items; "
+HEAD = {"produce": "stage 1 of the split pipeline: sse_stream_kernel (stage, split, classify, frame table, work items; "
                    "zero-copy frames are not serialized)",
         "decode": "stage 3 of the split pipeline: sse_decode_kernel (table-driven automaton, one lane per line, items sorted by "
                   "(length, shape))"}
