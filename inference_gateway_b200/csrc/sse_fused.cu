@@ -1445,7 +1445,7 @@ __device__ __noinline__ void process_window(const KParams &P, FSmem &S, uint32_t
             if (mode & SSE_MODE_R) mode |= SSE_MODE_PARSE;
             int a = (int)start, b = (int)nl + 1;
             if (sg.state & (FS_SKIP | FS_TERM | FS_DEAD)) kind = K_DROP;
-            else if (nl - start > P.carry_slot) { atomicMin(&S.seg[lo].dead, k); kind = K_DROP; }
+            else if (nl + 1u - start > P.carry_slot) { atomicMin(&S.seg[lo].dead, k); kind = K_DROP; }   // the line with its '\n', as the produce kernel counts it
             else if (mode & SSE_MODE_R) {
                 lflags |= LF_RMODE;
                 { const uint32_t ab = trim_space_ab(S.tile, (uint32_t)a, (uint32_t)b); a = (int)(ab & 0xFFFFu); b = (int)(ab >> 16); }   // agent.go:178-179
