@@ -4,7 +4,8 @@
  *
  *   ssegw_stream_chat_completions   core.IProvider.StreamChatCompletions (providers/core/interfaces.go:22; provider.go:277-344)
  *   ssegw_upstream_write / _close   response.Body bytes / EOF-or-error (provider.go:322-330)
- *   ssegw_pump                      one tick of the per-GPU batcher (INTEGRATION.md section 2)
+ *   ssegw_pump                      one tick of the per-GPU batchers (INTEGRATION.md section 2), batches in flight per context
+ *   ssegw_flush                     collects every batch still in flight
  *   ssegw_recv                      `line, ok := <-streamCh` (api/routes.go:602-606, mcp/agent.go:171)
  *   ssegw_agent_recv and friends    mcp.Agent.RunWithStream for one iteration (mcp/agent.go:126-290, final [DONE] :140-143)
  *   ssegw_proxy_stream / _step    handleStreamingRequest, the raw /proxy/:provider/... stream loop (api/routes.go:129-232)
@@ -32,6 +33,28 @@ ssegw *ssegw_new_ex(int device, uint32_t max_conns, uint32_t bytes_per_batch, co
  * next tick (streams with deferred bytes are offered first) instead of failing every stream of the batch. ssegw_new and
  * ssegw_new_ex use sse_worst_case_config. pool may be NULL. A bad config is refused (SSE_ERR_ARG) before a device is touched. */
 ssegw *ssegw_new_cfg(int device, const sse_config *cfg, const sse_line_pool *pool, int *status);
+/* One gateway over several contexts, each with up to `depth` batches in flight: the per-GPU batchers of INTEGRATION.md
+ * section 2 behind one set of streams. One context is opened per entry of devices (cfg and pool for each; a device may appear
+ * more than once, which gives independent contexts on one GPU), and the gateway holds n_devices * cfg->max_conns streams:
+ * stream id = context index * cfg->max_conns + connection. A new stream (ssegw_stream_chat_completions, ssegw_proxy_stream)
+ * goes to a free connection of the context with the fewest open streams, the lowest index on a tie, and stays there for its
+ * whole life (carry state and line-pool pages are per context).
+ * depth (1 .. cfg->n_slots) is how many batches a context may have uncollected. ssegw_pump then runs, per context: fill and
+ * submit a batch if any stream has bytes that may go in; collect every batch sse_poll reports done, oldest first; collect the
+ * oldest, blocking, while depth batches are uncollected. Frames reach the channels, the agent folds and the counters at
+ * collect time, in submission order per context. At depth 1 this is ssegw_new_cfg's tick: a pump delivers what it submitted.
+ * Bytes leave a stream's queue when they are submitted. Without SSE_FLAG_DEFER a stream may have bytes in several uncollected
+ * batches (the device keeps their order); with it, a stream is not offered again while it is in an uncollected batch, and its
+ * deferred rest goes back to the front of its queue when that batch is collected. A failed batch closes its streams, and
+ * later batches deliver nothing more to them; what a batch returns for a stream released since goes to nobody. An upstream
+ * EOF closes the channel once no byte of the stream is queued or in an uncollected batch.
+ * Bad arguments are refused with SSE_ERR_ARG before a device is touched: n_devices 0 or above 64, depth outside 1 ..
+ * cfg->n_slots, and what ssegw_new_cfg refuses. */
+ssegw *ssegw_new_multi(const int *devices, uint32_t n_devices, const sse_config *cfg, const sse_line_pool *pool, uint32_t depth,
+                       int *status);
+/* Collects every uncollected batch of every context. Returns the frames delivered, or the first negative sse_status (the
+ * batches after a failed one are still collected). ssegw_free flushes before it destroys the contexts. */
+int    ssegw_flush(ssegw *g);
 void   ssegw_free(ssegw *g);
 int    ssegw_stream_chat_completions(ssegw *g, uint8_t mode);
 size_t ssegw_upstream_write(ssegw *g, int stream, const uint8_t *data, size_t n);
@@ -44,9 +67,9 @@ sse_bytes ssegw_agent_content(ssegw *g, int stream);
 int    ssegw_agent_has_tool_calls(ssegw *g, int stream);
 int    ssegw_agent_terminated(ssegw *g, int stream, int *finish);
 size_t ssegw_agent_tool_calls(ssegw *g, int stream, sse_tool_call *calls, size_t cap);
-/* SSE_FLAG_COUNTERS: the sse_counters of every batch this gateway has collected, added up (d_items_per_pull: the last batch's),
- * e.g. for export as monotonic counters. SSE_ERR_ARG unless the gateway was made by ssegw_new_cfg with a config that has the
- * flag, or when out->struct_size != sizeof(sse_counters). */
+/* SSE_FLAG_COUNTERS: the sse_counters of every batch this gateway has collected, on every context, added up (d_items_per_pull:
+ * the last batch's), e.g. for export as monotonic counters. SSE_ERR_ARG unless the gateway was made by ssegw_new_cfg or
+ * ssegw_new_multi with a config that has the flag, or when out->struct_size != sizeof(sse_counters). */
 int    ssegw_counters(ssegw *g, sse_counters *out);
 
 /* The raw proxy stream handler (api/routes.go:129-232, taken when Accept is exactly text/event-stream, :118): reader and

@@ -262,6 +262,12 @@ int sse_acquire(sse_ctx *ctx, int *slot, sse_batch *batch);
 int sse_submit(sse_ctx *ctx, int slot, uint32_t n_segs, uint32_t in_bytes);
 int sse_collect(sse_ctx *ctx, int slot, sse_result *res);
 int sse_release(sse_ctx *ctx, int slot);
+/* Whether a submitted batch is done, without blocking: 1 when the work sse_submit queued for the slot (its kernels and the copy
+ * of its counters to the host) has completed, so that sse_collect waits only for its own result copies; 0 while it is still
+ * running; SSE_ERR_BUSY when the slot is not in the submitted state; SSE_ERR_ARG for a bad context or slot; SSE_ERR_CUDA (text
+ * in sse_last_cuda_error) when the device reports an error. Under SSE_FLAG_DEFER, sse_collect on a slot polled ready may still
+ * run the decode stage again, when its decode arenas grow. */
+int sse_poll(sse_ctx *ctx, int slot);
 
 /* connection state */
 int sse_reset_conn(sse_ctx *ctx, uint32_t conn);                 /* ordered after already submitted batches */

@@ -114,7 +114,7 @@ assert C.sizeof(Seg) == 16 and C.sizeof(Rec) == 32 and C.sizeof(Tc) == 48 and C.
 
 EXPORTS = [
     "sse_init", "sse_init_ex", "sse_line_pool_config", "sse_line_pool_stats", "sse_destroy", "sse_strerror", "sse_last_cuda_error", "sse_abi_version", "sse_default_config", "sse_worst_case_config",
-    "sse_acquire", "sse_submit", "sse_collect", "sse_release", "sse_reset_conn", "sse_reset_all",
+    "sse_acquire", "sse_submit", "sse_poll", "sse_collect", "sse_release", "sse_reset_conn", "sse_reset_all",
     "sse_upload", "sse_launch", "sse_download", "sse_launch_count", "sse_at", "sse_counters_read",
     "sse_agent_new", "sse_agent_free", "sse_agent_reset", "sse_agent_feed", "sse_agent_content",
     "sse_agent_has_tool_calls", "sse_agent_terminated", "sse_agent_tool_calls",
@@ -156,6 +156,7 @@ def load(build_if_missing: bool = True):
     L.sse_worst_case_config.restype = None
     L.sse_acquire.argtypes = [vp, C.POINTER(i32), C.POINTER(Batch)]
     L.sse_submit.argtypes = [vp, i32, u32, u32]
+    L.sse_poll.argtypes = [vp, i32]
     L.sse_collect.argtypes = [vp, i32, C.POINTER(Result)]
     L.sse_release.argtypes = [vp, i32]
     L.sse_reset_conn.argtypes = [vp, u32]

@@ -8,7 +8,8 @@
 //   ssegw_upstream_write/close     ~ bytes arriving on response.Body / EOF-or-error (provider.go:322-330: the
 //                                    unterminated tail is dropped, then the channel is closed)
 //   ssegw_pump                     ~ one tick of the per-GPU batcher goroutine (INTEGRATION.md): micro-batch every
-//                                    stream's pending bytes, sse_submit, sse_collect, deliver frames to the channels
+//                                    stream's pending bytes, sse_submit, sse_collect what is done (up to `depth` batches
+//                                    stay in flight per context), deliver frames to the channels
 //   ssegw_recv                     ~ `line, ok := <-streamCh` (api/routes.go:602-606, mcp/agent.go:171)
 //   ssegw_agent_*                  ~ mcp.Agent.RunWithStream for one iteration (mcp/agent.go:126-290): forwards frames to
 //                                    the middleware channel, exposes accumulated content / tool calls / finish, appends the
@@ -16,6 +17,7 @@
 //
 // Channel capacity is 100 as in provider.go:307: a stream with 100 undelivered elements stops accepting upstream bytes
 // (ssegw_upstream_write returns 0 bytes accepted), which is the back-pressure the reader goroutine would feel.
+#include <limits.h>
 #include <stddef.h>
 #include <stdint.h>
 #include <string.h>
@@ -28,6 +30,7 @@ namespace {
 
 constexpr size_t CHAN_CAP = 100;
 constexpr size_t PENDING_CAP = 4u << 20;   // per-stream bytes waiting for a batch
+constexpr uint32_t MAX_DEVICES = 64;       // contexts of one gateway (ssegw_new_multi)
 
 struct Stream {
     bool open = false;          // slot in use
@@ -40,16 +43,31 @@ struct Stream {
     sse_agent_fold *agent = nullptr;
     bool done_sent = false;
     bool deferred = false;      // SSE_FLAG_DEFER: the last batch left bytes of this stream in `pending`; offered first next tick
+    uint64_t gen = 0;           // bumped at every open: a batch that holds bytes of an earlier stream on the slot delivers nothing here
+    uint32_t in_flight = 0;     // uncollected batches that hold bytes of this stream (this generation)
+};
+
+// One stream's bytes in a submitted batch: where they stand in the batch's input arena, and which stream they were taken from.
+struct Member { uint32_t stream; uint64_t gen; uint32_t off, len; };
+struct InFlight { int slot; std::vector<Member> who; };
+
+// One context (one device, or one of several contexts on a device): its connections are streams
+// [index * max_conns, (index + 1) * max_conns) of the gateway, and its uncollected batches, oldest first.
+struct Ctx {
+    sse_ctx *ctx = nullptr;
+    std::deque<InFlight> inflight;
+    size_t rr = 0;              // the batcher starts its scan one connection further every tick (no slot is favoured)
+    uint32_t n_open = 0;        // open streams, for placement
 };
 
 } // namespace
 
 struct ssegw {
-    sse_ctx *ctx = nullptr;
+    std::vector<Ctx> ctxs;
     sse_config cfg{};
+    uint32_t depth = 1;         // batches a context may have uncollected during a pump (a pump leaves at most depth - 1)
     std::vector<Stream> streams;
     std::string last_error;
-    size_t rr = 0;              // the batcher starts its scan one stream further every tick (no slot is favoured)
     sse_counters sum{};         // SSE_FLAG_COUNTERS: every collected batch's counters added up (ssegw_counters)
 };
 
@@ -57,16 +75,115 @@ namespace {
 
 // SSE_FLAG_COUNTERS: adds the counters of the batch just collected in `slot` to the gateway's sums (d_items_per_pull is the
 // launch's choice, not an amount: the last batch's is kept)
-void add_counters(ssegw *g, int slot) {
+void add_counters(ssegw *g, sse_ctx *ctx, int slot) {
     sse_counters k{};
     k.struct_size = sizeof k;
-    if (sse_counters_read(g->ctx, slot, &k) != SSE_OK) return;
+    if (sse_counters_read(ctx, slot, &k) != SSE_OK) return;
     uint64_t *dst = &g->sum.p_segments;
     const uint64_t *src = &k.p_segments;
     const size_t n = (sizeof k - offsetof(sse_counters, p_segments)) / sizeof(uint64_t);
     for (size_t i = 0; i < n; i++) dst[i] += src[i];
     g->sum.d_items_per_pull = k.d_items_per_pull;
     g->sum.decode_passes += k.decode_passes;
+}
+
+// a failed batch fails its streams: the client sees EOF, exactly like an upstream read error (provider.go:323-330). With
+// SSE_FLAG_DEFER a batch does not fail for want of arena space, only on a CUDA or allocation error.
+void fail_batch(ssegw *g, Ctx &x, const InFlight &f) {
+    for (const Member &m : f.who) {
+        Stream &s = g->streams[m.stream];
+        if (s.gen != m.gen) continue;
+        s.in_flight--;
+        s.closed = true;
+    }
+    sse_release(x.ctx, f.slot);
+}
+
+// Step 1 of a tick on context k: fills a batch with what the streams have pending and submits it (nothing when no stream
+// has bytes that may go in). The bytes leave `pending` now.
+int submit_batch(ssegw *g, size_t k) {
+    Ctx &x = g->ctxs[k];
+    int slot; sse_batch b;
+    int rc = sse_acquire(x.ctx, &slot, &b);
+    if (rc != SSE_OK) return rc;
+    InFlight f{ slot, {} };
+    uint32_t off = 0, n = 0;
+    const size_t nc = g->cfg.max_conns, base = k * nc;
+    const size_t start = x.rr++ % nc;
+    const bool defer = (g->cfg.flags & SSE_FLAG_DEFER) != 0;
+    // streams whose bytes a batch deferred (SSE_FLAG_DEFER) go first, so that a flood on other streams cannot keep them waiting
+    for (int pass = 0; pass < 2; pass++)
+    for (size_t q = 0; q < nc && n < b.max_segs; q++) {
+        const size_t i = (start + q) % nc;
+        Stream &s = g->streams[base + i];
+        if (s.deferred != (pass == 0)) continue;
+        if (!s.open || s.closed || s.pending.empty()) continue;
+        if (s.chan.size() >= CHAN_CAP) continue;                      // receiver is slow: leave the bytes queued
+        if (defer && s.in_flight) continue;                           // a deferred rest of that batch must come before these bytes
+        // a stream takes what fits: the rest stays queued for the next tick (the carry state on the device makes any cut legal)
+        const size_t room = b.in_arena_bytes > off + 16u ? (size_t)(b.in_arena_bytes - off - 16u) : 0;
+        const size_t take = s.pending.size() < room ? s.pending.size() : room;
+        if (take == 0) continue;
+        memcpy(b.in_arena + off, s.pending.data(), take);
+        b.segs[n] = sse_seg{ (uint32_t)i, off, (uint32_t)take, s.mode, 0, 0 };
+        f.who.push_back(Member{ (uint32_t)(base + i), s.gen, off, (uint32_t)take });
+        s.pending.erase(0, take);
+        s.in_flight++;
+        off = (off + (uint32_t)take + 15u) & ~15u;
+        n++;
+    }
+    if (!n) return sse_release(x.ctx, slot);
+    rc = sse_submit(x.ctx, slot, n, off);
+    if (rc != SSE_OK) { fail_batch(g, x, f); return rc; }
+    x.inflight.push_back(std::move(f));
+    return SSE_OK;
+}
+
+// Collects the oldest uncollected batch of a context and fans it out: frames to the channels, records to the agent folds.
+// Returns the frames delivered or a negative status (the batch failed).
+int collect_oldest(ssegw *g, Ctx &x) {
+    const InFlight f = std::move(x.inflight.front());
+    x.inflight.pop_front();
+    sse_result res;
+    const int rc = sse_collect(x.ctx, f.slot, &res);
+    if (rc != SSE_OK) { fail_batch(g, x, f); return rc; }
+    if (g->cfg.flags & SSE_FLAG_COUNTERS) add_counters(g, x.ctx, f.slot);
+    int delivered = 0;
+    for (uint32_t k = 0; k < (uint32_t)f.who.size(); k++) {
+        const Member &m = f.who[k];
+        Stream &s = g->streams[m.stream];
+        if (s.gen != m.gen) continue;       // released and reopened since: the connection was reset after this batch, its
+                                            // results belong to nobody
+        s.in_flight--;
+        // released, or failed by an earlier batch or fold: the connection state no longer describes the stream
+        if (!s.open || s.closed) continue;
+        // only the bytes the batch took are gone: a deferred rest goes back to the front of the queue, before anything newer
+        const uint32_t consumed = res.segs[k].consumed;
+        if (consumed < m.len) s.pending.insert(0, (const char *)res.in + m.off + consumed, m.len - consumed);
+        s.deferred = (res.segs[k].flags & SSE_SEG_DEFERRED) != 0;
+        const sse_run *run = &res.segs[k].run;
+        for (;;) {
+            for (uint32_t fr = run->frame_first; fr < run->frame_first + run->frame_count; fr++) {
+                s.chan.emplace_back((const char *)sse_at(&res, res.frames[fr].off), res.frames[fr].len);   // fresh copy per element
+                delivered++;
+            }
+            if (run->next == SSE_NONE) break;
+            run = &res.runs[run->next];
+        }
+        // a record the library could not decode (SSE_ERR_UNDECODED): the accumulators would be silently short, so the stream is failed
+        if ((s.mode & SSE_MODE_R) && sse_agent_feed(s.agent, &res, k) != SSE_OK) s.closed = true;
+        if (res.segs[k].flags & SSE_SEG_TERMINATED) s.terminated = true;
+        if (res.segs[k].flags & SSE_SEG_DEAD) s.closed = true;
+    }
+    sse_release(x.ctx, f.slot);
+    return delivered;
+}
+
+// upstream EOF: the channel closes once no byte of the stream waits on the host or in a batch (the unterminated tail, if
+// any, stays on the device and is dropped)
+void close_drained(ssegw *g) {
+    for (auto &s : g->streams)
+        if (s.open && s.upstream_eof && s.pending.empty() && !s.in_flight) s.closed = true;
 }
 
 } // namespace
@@ -86,31 +203,60 @@ ssegw *ssegw_new_ex(int device, uint32_t max_conns, uint32_t bytes_per_batch, co
 }
 
 ssegw *ssegw_new_cfg(int device, const sse_config *cfg, const sse_line_pool *pool, int *status) {
-    if (!cfg || cfg->struct_size != sizeof(sse_config)) { if (status) *status = SSE_ERR_ARG; return nullptr; }
+    return ssegw_new_multi(&device, 1, cfg, pool, 1, status);
+}
+
+ssegw *ssegw_new_multi(const int *devices, uint32_t n_devices, const sse_config *cfg, const sse_line_pool *pool, uint32_t depth,
+                       int *status) {
+    if (!devices || n_devices == 0 || n_devices > MAX_DEVICES || !cfg || cfg->struct_size != sizeof(sse_config) || depth < 1 ||
+        depth > cfg->n_slots || (uint64_t)n_devices * cfg->max_conns > (uint64_t)INT_MAX) {
+        if (status) *status = SSE_ERR_ARG;
+        return nullptr;
+    }
     ssegw *g = new ssegw();
     g->cfg = *cfg;
-    int rc = sse_init_ex(device, &g->cfg, pool, &g->ctx);
-    if (status) *status = rc;
-    if (rc != SSE_OK) { delete g; return nullptr; }   // no CUDA device: error, never a CPU path
-    g->streams.resize(cfg->max_conns);
+    g->depth = depth;
+    g->ctxs.resize(n_devices);
+    for (uint32_t k = 0; k < n_devices; k++) {
+        const int rc = sse_init_ex(devices[k], &g->cfg, pool, &g->ctxs[k].ctx);
+        if (rc != SSE_OK) {   // no CUDA device: error, never a CPU path
+            if (status) *status = rc;
+            ssegw_free(g);
+            return nullptr;
+        }
+    }
+    g->streams.resize((size_t)n_devices * cfg->max_conns);
+    if (status) *status = SSE_OK;
     return g;
 }
 
 void ssegw_free(ssegw *g) {
     if (!g) return;
+    ssegw_flush(g);   // every slot is released, whatever the batches returned
     for (auto &s : g->streams) if (s.agent) sse_agent_free(s.agent);
-    sse_destroy(g->ctx);
+    for (auto &x : g->ctxs) sse_destroy(x.ctx);
     delete g;
 }
 
-// StreamChatCompletions: allocates a connection slot and its channel. Returns the stream id or -1 (no free slot).
+// StreamChatCompletions: binds a new stream to a free connection of the context with the fewest open streams (the lowest
+// index on a tie), where it stays for its whole life. Returns the stream id or -1 (no free slot).
 int ssegw_stream_chat_completions(ssegw *g, uint8_t mode) {
-    for (size_t i = 0; i < g->streams.size(); i++) {
+    const size_t nc = g->cfg.max_conns;
+    size_t k = g->ctxs.size();
+    for (size_t j = 0; j < g->ctxs.size(); j++)
+        if (g->ctxs[j].n_open < nc && (k == g->ctxs.size() || g->ctxs[j].n_open < g->ctxs[k].n_open)) k = j;
+    if (k == g->ctxs.size()) return -1;
+    for (size_t i = k * nc; i < (k + 1) * nc; i++) {
         Stream &s = g->streams[i];
         if (!s.open) {
             if (s.agent) sse_agent_reset(s.agent); else s.agent = sse_agent_new();
-            s = Stream{ true, false, false, mode, {}, {}, false, s.agent, false, false };
-            if (sse_reset_conn(g->ctx, (uint32_t)i) != SSE_OK) return -1;
+            sse_agent_fold *agent = s.agent;
+            const uint64_t gen = s.gen + 1;
+            s = Stream{};
+            s.open = true; s.mode = mode; s.agent = agent; s.gen = gen;
+            g->ctxs[k].n_open++;
+            // ordered after every batch already submitted, which may still hold bytes of the slot's previous stream
+            if (sse_reset_conn(g->ctxs[k].ctx, (uint32_t)(i - k * nc)) != SSE_OK) return -1;
             return (int)i;
         }
     }
@@ -131,70 +277,41 @@ size_t ssegw_upstream_write(ssegw *g, int id, const uint8_t *data, size_t n) {
 
 void ssegw_upstream_close(ssegw *g, int id) { g->streams[(size_t)id].upstream_eof = true; }
 
-// One batcher tick. Returns the number of frames delivered, or a negative sse_status.
+// One batcher tick. For each context: fill and submit a batch, collect every batch that is done (oldest first), then collect
+// the oldest, blocking, while `depth` are uncollected. At depth 1 the batch submitted is delivered in the same call. Fan-out
+// happens at collect time, in submission order per context. Returns the number of frames delivered, or a negative sse_status.
 int ssegw_pump(ssegw *g) {
-    int slot; sse_batch b;
-    int rc = sse_acquire(g->ctx, &slot, &b);
-    if (rc != SSE_OK) return rc;
-    std::vector<uint32_t> who;
-    uint32_t off = 0, n = 0;
-    const size_t ns = g->streams.size();
-    const size_t start = ns ? g->rr++ % ns : 0;
-    // streams whose bytes a batch deferred (SSE_FLAG_DEFER) go first, so that a flood on other streams cannot keep them waiting
-    for (int pass = 0; pass < 2; pass++)
-    for (size_t q = 0; q < ns && n < b.max_segs; q++) {
-        const size_t i = (start + q) % ns;
-        Stream &s = g->streams[i];
-        if (s.deferred != (pass == 0)) continue;
-        if (!s.open || s.closed || s.pending.empty()) continue;
-        if (s.chan.size() >= CHAN_CAP) continue;                      // receiver is slow: leave the bytes queued
-        // a stream takes what fits: the rest stays queued for the next tick (the carry state on the device makes any cut legal)
-        const size_t room = b.in_arena_bytes > off + 16u ? (size_t)(b.in_arena_bytes - off - 16u) : 0;
-        const size_t take = s.pending.size() < room ? s.pending.size() : room;
-        if (take == 0) continue;
-        memcpy(b.in_arena + off, s.pending.data(), take);
-        b.segs[n] = sse_seg{ (uint32_t)i, off, (uint32_t)take, s.mode, 0, 0 };
-        off = (off + (uint32_t)take + 15u) & ~15u;
-        who.push_back((uint32_t)i);
-        n++;
-    }
     int delivered = 0;
-    if (n) {
-        rc = sse_submit(g->ctx, slot, n, off);
-        sse_result res;
-        if (rc == SSE_OK) rc = sse_collect(g->ctx, slot, &res);
-        if (rc != SSE_OK) {
-            // a failed batch fails its streams: the client sees EOF, exactly like an upstream read error (provider.go:323-330).
-            // With SSE_FLAG_DEFER a batch does not fail for want of arena space, only on a CUDA or allocation error.
-            for (uint32_t i : who) g->streams[i].closed = true;
-            sse_release(g->ctx, slot);
-            return rc;
+    for (size_t k = 0; k < g->ctxs.size(); k++) {
+        Ctx &x = g->ctxs[k];
+        int rc = submit_batch(g, k);
+        if (rc != SSE_OK) return rc;
+        while (!x.inflight.empty() && sse_poll(x.ctx, x.inflight.front().slot) != 0) {   // done, or an error collect reports
+            if ((rc = collect_oldest(g, x)) < 0) return rc;
+            delivered += rc;
         }
-        if (g->cfg.flags & SSE_FLAG_COUNTERS) add_counters(g, slot);
-        for (uint32_t k = 0; k < n; k++) {
-            Stream &s = g->streams[who[k]];
-            // only the bytes the batch took leave the queue: a deferred rest is submitted again, before anything newer
-            s.pending.erase(0, res.segs[k].consumed);
-            s.deferred = (res.segs[k].flags & SSE_SEG_DEFERRED) != 0;
-            const sse_run *run = &res.segs[k].run;
-            for (;;) {
-                for (uint32_t f = run->frame_first; f < run->frame_first + run->frame_count; f++) {
-                    s.chan.emplace_back((const char *)sse_at(&res, res.frames[f].off), res.frames[f].len);   // fresh copy per element
-                    delivered++;
-                }
-                if (run->next == SSE_NONE) break;
-                run = &res.runs[run->next];
-            }
-            // a record the library could not decode (SSE_ERR_UNDECODED): the accumulators would be silently short, so the stream is failed
-            if ((s.mode & SSE_MODE_R) && sse_agent_feed(s.agent, &res, k) != SSE_OK) s.closed = true;
-            if (res.segs[k].flags & SSE_SEG_TERMINATED) s.terminated = true;
-            if (res.segs[k].flags & SSE_SEG_DEAD) s.closed = true;
+        while (x.inflight.size() >= g->depth) {
+            if ((rc = collect_oldest(g, x)) < 0) return rc;
+            delivered += rc;
         }
     }
-    sse_release(g->ctx, slot);
-    for (auto &s : g->streams)
-        if (s.open && s.upstream_eof && s.pending.empty()) s.closed = true;   // tail (if any) stays on the device and is dropped
+    close_drained(g);
     return delivered;
+}
+
+// Collects every uncollected batch of every context. Returns the frames delivered, or the first negative sse_status (the
+// batches after a failed one are still collected).
+int ssegw_flush(ssegw *g) {
+    if (!g) return SSE_ERR_ARG;
+    int delivered = 0, first = SSE_OK;
+    for (auto &x : g->ctxs)
+        while (!x.inflight.empty()) {
+            const int rc = collect_oldest(g, x);
+            if (rc < 0) { if (first == SSE_OK) first = rc; }
+            else delivered += rc;
+        }
+    close_drained(g);
+    return first != SSE_OK ? first : delivered;
 }
 
 // `line, ok := <-streamCh`: 1 = element copied to buf (*n bytes), 0 = nothing available yet, -1 = channel closed and drained.
@@ -211,7 +328,11 @@ int ssegw_recv(ssegw *g, int id, uint8_t *buf, size_t cap, size_t *n) {
     return s.closed ? -1 : 0;
 }
 
-void ssegw_release_stream(ssegw *g, int id) { g->streams[(size_t)id].open = false; }
+void ssegw_release_stream(ssegw *g, int id) {
+    Stream &s = g->streams[(size_t)id];
+    if (s.open) g->ctxs[(size_t)id / g->cfg.max_conns].n_open--;
+    s.open = false;
+}
 
 int ssegw_counters(ssegw *g, sse_counters *out) {
     if (!g || !out || out->struct_size != sizeof(sse_counters) || !(g->cfg.flags & SSE_FLAG_COUNTERS)) return SSE_ERR_ARG;

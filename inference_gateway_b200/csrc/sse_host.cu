@@ -1,7 +1,8 @@
 // sse_host.cu -- C ABI of libssegpu.so (include/sse_gpu.h): context, pinned staging, batch pipeline.
 //
 // One context per GPU. A batch slot owns pinned host staging + device buffers + a CUDA stream:
-//   sse_submit:  H2D(segs, input)  ->  [wait: previous batch's kernel]  ->  kernel  ->  D2H(counters)
+//   sse_submit:  H2D(segs, input)  ->  [wait: previous batch's kernel]  ->  kernel  ->  D2H(counters)  ->  record kernel_done
+//   sse_poll:    query kernel_done (never blocks)
 //   sse_collect: sync, then exact-size D2H of the result arrays, sync.
 // Kernels of consecutive batches are ordered by an event because they share per-connection state
 // (carry, finished flag) -- the per-connection FIFO of provider.go:307-340; H2D of batch k+1 and D2H of
@@ -56,6 +57,7 @@ struct Slot {
     unsigned long long *d_cnt = nullptr, *h_cnt = nullptr;
     uint32_t decode_passes = 0;
     bool cnt_ready = false;                                    // h_cnt holds the counters of the batch last downloaded
+    bool ctr_queued = false;                                   // sse_submit queued the D2H of h_ctr (do_download does not)
 };
 
 } // namespace
@@ -247,7 +249,8 @@ int redecode(sse_ctx *c, Slot &s, Counters &k, cudaStream_t st, uint32_t &grown)
 }
 
 int do_download(sse_ctx *c, Slot &s, sse_result *res, cudaStream_t st) {
-    CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, st));
+    if (!s.ctr_queued) CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, st));
+    s.ctr_queued = false;
     CU(cudaStreamSynchronize(st));
     Counters k = *s.h_ctr;
     memset(res, 0, sizeof *res);
@@ -494,8 +497,23 @@ int sse_submit(sse_ctx *c, int slot, uint32_t n_segs, uint32_t in_bytes) {
     if (rc != SSE_OK) return rc;
     CU(cudaEventRecord(c->last_kernel, s.stream));
     c->have_last = true;
+    // the counters sse_collect reads first travel now, so that a slot sse_poll reports done is one copy away from its result
+    CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, s.stream));
+    CU(cudaEventRecord(s.kernel_done, s.stream));
+    s.ctr_queued = true;
     s.state = SLOT_SUBMITTED;
     return SSE_OK;
+}
+
+int sse_poll(sse_ctx *c, int slot) {
+    if (!c || slot < 0 || slot >= (int)c->slots.size()) return SSE_ERR_ARG;
+    Slot &s = c->slots[slot];
+    if (s.state != SLOT_SUBMITTED) return SSE_ERR_BUSY;
+    CU(cudaSetDevice(c->device));
+    const cudaError_t e = cudaEventQuery(s.kernel_done);
+    if (e == cudaErrorNotReady) return 0;
+    CU(e);
+    return 1;
 }
 
 int sse_collect(sse_ctx *c, int slot, sse_result *res) {
@@ -514,6 +532,7 @@ int sse_release(sse_ctx *c, int slot) {
     if (s.state == SLOT_SUBMITTED) { CU(cudaSetDevice(c->device)); CU(cudaStreamSynchronize(s.stream)); }
     s.state = SLOT_FREE;
     s.cnt_ready = false;
+    s.ctr_queued = false;
     return SSE_OK;
 }
 

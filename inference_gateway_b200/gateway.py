@@ -9,11 +9,14 @@ from . import _abi as A
 
 class Gateway:
     def __init__(self, device: int = 0, max_conns: int = 256, bytes_per_batch: int = 1 << 20, line_pool: dict | None = None,
-                 config: A.Config | None = None):
+                 config: A.Config | None = None, devices: list[int] | None = None, depth: int = 1):
         """line_pool: keyword arguments of engine.make_line_pool() (pool_pages, page_bytes, max_line_bytes): lines longer than the
         64 KiB carry slot continue in a shared device page pool instead of failing their stream.
         config: an sse_config to run on (ssegw_new_cfg; max_conns and bytes_per_batch are then ignored), e.g. default capacities
-        with FLAG_DEFER; None: the worst-case config."""
+        with FLAG_DEFER; None: the worst-case config.
+        devices, depth: one context per entry of devices (a device may repeat), each with up to depth (1 .. config.n_slots)
+        batches in flight (ssegw_new_multi; needs config). Stream id = context index * config.max_conns + connection. With depth
+        above 1 a pump delivers what earlier pumps submitted; flush() collects the rest. depth alone runs on [device]."""
         from .engine import make_line_pool
         self.L = L = A.load()
         vp, i32 = C.c_void_p, C.c_int
@@ -23,6 +26,10 @@ class Gateway:
         L.ssegw_new_ex.restype = vp
         L.ssegw_new_cfg.argtypes = [i32, C.POINTER(A.Config), C.POINTER(A.LinePool), C.POINTER(i32)]
         L.ssegw_new_cfg.restype = vp
+        L.ssegw_new_multi.argtypes = [C.POINTER(i32), C.c_uint32, C.POINTER(A.Config), C.POINTER(A.LinePool), C.c_uint32,
+                                      C.POINTER(i32)]
+        L.ssegw_new_multi.restype = vp
+        L.ssegw_flush.argtypes = [vp]
         L.ssegw_free.argtypes = [vp]
         L.ssegw_free.restype = None
         L.ssegw_stream_chat_completions.argtypes = [vp, C.c_uint8]
@@ -46,7 +53,14 @@ class Gateway:
         L.ssegw_counters.argtypes = [vp, C.POINTER(A.Counters)]
         st = i32()
         self._pool = make_line_pool(**line_pool) if line_pool is not None else None
-        if config is not None:
+        if devices is not None or depth != 1:
+            if config is None:
+                raise ValueError("devices / depth need an sse_config (config=)")
+            devs = list(devices) if devices is not None else [device]
+            arr = (i32 * max(1, len(devs)))(*devs)
+            self.g = L.ssegw_new_multi(arr, len(devs), C.byref(config), C.byref(self._pool) if self._pool is not None else None,
+                                       depth, C.byref(st))
+        elif config is not None:
             self.g = L.ssegw_new_cfg(device, C.byref(config), C.byref(self._pool) if self._pool is not None else None, C.byref(st))
         elif line_pool is None:
             self.g = L.ssegw_new(device, max_conns, bytes_per_batch, C.byref(st))
@@ -77,6 +91,13 @@ class Gateway:
         rc = self.L.ssegw_pump(self.g)
         if rc < 0:
             raise A.SseError(rc, "ssegw_pump")
+        return rc
+
+    def flush(self) -> int:
+        """ssegw_flush: collects every batch still in flight; returns the frames delivered."""
+        rc = self.L.ssegw_flush(self.g)
+        if rc < 0:
+            raise A.SseError(rc, "ssegw_flush")
         return rc
 
     def _recv(self, fn, sid):

@@ -3,13 +3,17 @@
 //
 //   cmd/gateway/main.go:171   providerRegistry := registry.NewProviderRegistry(cfg.Providers, logger)
 // becomes
-//   providerRegistry := ssegpu.WrapRegistry(registry.NewProviderRegistry(cfg.Providers, logger), batcher)
+//   batchers, err := ssegpu.Batchers(newBatcher) // one per entry of GPU_DEVICES
+//   providerRegistry := ssegpu.WrapRegistry(registry.NewProviderRegistry(cfg.Providers, logger), batchers)
 package ssegpu
 
 import (
 	"context"
 	"io"
 	"net/http"
+	"os"
+	"strconv"
+	"strings"
 
 	"github.com/inference-gateway/inference-gateway/providers/client"
 	"github.com/inference-gateway/inference-gateway/providers/core"
@@ -17,28 +21,100 @@ import (
 	"github.com/inference-gateway/inference-gateway/providers/types"
 )
 
-// Batcher owns the per-GPU contexts. Connections shard by hash(conn) % nGPU and stay on their GPU for life
-// (carry state and FIFO order are per device). One goroutine per GPU, locked to its OS thread, runs:
-//   acquire -> drain pending reads of its connections into the batch (<= GPU_BATCH_USEC or GPU_BATCH_BYTES) ->
-//   submit -> collect -> fan frames out to the per-stream channels -> release.
-// With GPU_DEFER=1 (see NewContext) a segment can come back Deferred: its unconsumed tail goes back to the head of that
-// connection's queue, and connections with such a tail are drained first into the next batch.
+// Batcher is one device's batcher: one goroutine, locked to its OS thread, owning one Context whose connections stay on it
+// for life (carry state, line-pool pages and FIFO order are per context). Each tick (RunTick below):
+//  1. acquire -> drain pending reads of its connections into the batch (<= GPU_BATCH_USEC or GPU_BATCH_BYTES) -> submit;
+//  2. collect every batch Poll reports done, oldest first, fan frames out to the per-stream channels, release;
+//  3. while GPU_BATCH_DEPTH batches are still uncollected, collect the oldest one, blocking.
+// At GPU_BATCH_DEPTH=1 (the default) a batch is collected in the tick that submitted it. Deeper, the host fills batch k+1
+// while the device runs batch k. Bytes leave a connection's queue when they are submitted; with GPU_DEFER=1 (see
+// NewContext) a segment can come back Deferred: its unconsumed tail goes back to the head of that connection's queue,
+// connections with such a tail are drained first into the next batch, and a connection is not drained again while it is in
+// an uncollected batch (its tail must come before its newer bytes). The host mirror is ssegw_new_multi / ssegw_pump.
 type Batcher interface {
 	// Open registers a new upstream stream; the returned id addresses its slot until Close.
 	Open(mode uint8) (conn uint32, frames <-chan []byte)
 	// Feed hands over bytes read from the upstream body (any cut points). EOF/err closes the stream after the
-	// lines already queued were delivered; the unterminated tail is dropped (provider.go:323-330).
+	// lines already queued, and those in uncollected batches, were delivered; the unterminated tail is dropped
+	// (provider.go:323-330).
 	Feed(conn uint32, data []byte)
 	Close(conn uint32)
+	// Open streams, for placement.
+	Streams() int
+}
+
+// inFlight is one submitted batch and the connections (with their generation: a connection closed and opened again
+// while the batch was in flight gets nothing of it) whose bytes it holds.
+type inFlight struct {
+	b   *Batch
+	who []member
+}
+
+type member struct {
+	conn uint32
+	gen  uint64
+	data []byte // the bytes submitted (a view of the batch's pinned arena), for the deferred tail
+}
+
+// RunTick is steps 2 and 3 of a tick, after step 1 appended the submitted batch (if any) to q. deliver fans one collected
+// batch out (frames, Deferred tails, agent folds, counters) in submission order; a failed batch closes its streams.
+func RunTick(x *Context, q []inFlight, depth int, deliver func(inFlight, *Result, error)) ([]inFlight, error) {
+	collect := func() {
+		f := q[0]
+		q = q[1:]
+		res, err := x.Collect(f.b)
+		deliver(f, res, err)
+		x.Release(f.b)
+	}
+	for len(q) > 0 {
+		done, err := x.Poll(q[0].b)
+		if err != nil {
+			return q, err
+		}
+		if !done {
+			break
+		}
+		collect()
+	}
+	for len(q) >= depth {
+		collect()
+	}
+	return q, nil
+}
+
+// Batchers builds one Batcher per entry of GPU_DEVICES (comma-separated device ordinals, default "0"; an ordinal may repeat,
+// which gives independent contexts on one GPU), each with GPU_BATCH_DEPTH (1..8, default 1) batches in flight.
+func Batchers(newBatcher func(device int, depth int) (Batcher, error)) ([]Batcher, error) {
+	depth := int(envUint32("GPU_BATCH_DEPTH"))
+	if depth == 0 {
+		depth = 1
+	}
+	devs := os.Getenv("GPU_DEVICES")
+	if devs == "" {
+		devs = "0"
+	}
+	var out []Batcher
+	for _, d := range strings.Split(devs, ",") {
+		dev, err := strconv.Atoi(strings.TrimSpace(d))
+		if err != nil {
+			return nil, err
+		}
+		b, err := newBatcher(dev, depth)
+		if err != nil {
+			return nil, err
+		}
+		out = append(out, b)
+	}
+	return out, nil
 }
 
 type gpuRegistry struct {
 	inner registry.ProviderRegistry
-	b     Batcher
+	bs    []Batcher
 }
 
-func WrapRegistry(inner registry.ProviderRegistry, b Batcher) registry.ProviderRegistry {
-	return &gpuRegistry{inner: inner, b: b}
+func WrapRegistry(inner registry.ProviderRegistry, bs []Batcher) registry.ProviderRegistry {
+	return &gpuRegistry{inner: inner, bs: bs}
 }
 func (g *gpuRegistry) GetProviders() map[types.Provider]*registry.ProviderConfig { return g.inner.GetProviders() }
 func (g *gpuRegistry) BuildProvider(id types.Provider, c client.Client) (core.IProvider, error) {
@@ -46,13 +122,24 @@ func (g *gpuRegistry) BuildProvider(id types.Provider, c client.Client) (core.IP
 	if err != nil {
 		return nil, err
 	}
-	return &gpuProvider{IProvider: p, b: g.b}, nil
+	return &gpuProvider{IProvider: p, bs: g.bs}, nil
+}
+
+// pick is the batcher with the fewest open streams (the first on a tie): a stream stays on it for its whole life.
+func pick(bs []Batcher) Batcher {
+	best := bs[0]
+	for _, b := range bs[1:] {
+		if b.Streams() < best.Streams() {
+			best = b
+		}
+	}
+	return best
 }
 
 // gpuProvider embeds the stock provider (nine methods for free) and replaces only the stream reader.
 type gpuProvider struct {
 	core.IProvider
-	b Batcher
+	bs []Batcher
 	// OpenUpstream re-implements provider.go:277-305 (unexported helpers there): build URL, force
 	// stream_options.include_usage, POST, map non-200 to *core.HTTPError. ~30 lines, unchanged semantics.
 	OpenUpstream func(ctx context.Context, req types.CreateChatCompletionRequest) (*http.Response, error)
@@ -63,15 +150,16 @@ func (p *gpuProvider) StreamChatCompletions(ctx context.Context, req types.Creat
 	if err != nil {
 		return nil, err // before streaming: (nil, err), *core.HTTPError carries the upstream status
 	}
-	conn, frames := p.b.Open(ModeP) // the MCP agent asks for ModeR via a context key instead
+	b := pick(p.bs)
+	conn, frames := b.Open(ModeP) // the MCP agent asks for ModeR via a context key instead
 	go func() {                     // socket reads stay on the host; one goroutine per stream as in provider.go:308
 		defer resp.Body.Close()
-		defer p.b.Close(conn)
+		defer b.Close(conn)
 		buf := make([]byte, 32<<10)
 		for {
 			n, rerr := resp.Body.Read(buf)
 			if n > 0 {
-				p.b.Feed(conn, buf[:n])
+				b.Feed(conn, buf[:n])
 			}
 			if rerr != nil || ctx.Err() != nil { // io.EOF or read error: log only, close (provider.go:323-330)
 				_ = io.EOF

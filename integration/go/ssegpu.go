@@ -62,10 +62,14 @@ func envUint32(name string) uint32 {
 // every stream in it); what does not fit waits for the next batch. The batcher must then keep the unconsumed tail of a
 // deferred segment (data[res.Consumed(i):], see Result.Deferred) at the head of that connection's queue and submit it before
 // any newer bytes of the connection.
-func NewContext(device int, maxConns, bytesPerBatch uint32) (*Context, error) {
+//
+// nSlots (1..8) is how many batches the context can hold at once: the batcher keeps up to that many in flight
+// (GPU_BATCH_DEPTH).
+func NewContext(device int, maxConns, bytesPerBatch, nSlots uint32) (*Context, error) {
 	runtime.LockOSThread()
 	var cfg C.sse_config
 	C.sse_default_config(&cfg, C.uint32_t(maxConns), C.uint32_t(bytesPerBatch))
+	cfg.n_slots = C.uint32_t(nSlots)
 	if os.Getenv("GPU_DEFER") == "1" {
 		cfg.flags |= C.SSE_FLAG_DEFER
 	}
@@ -143,6 +147,17 @@ func (b *Batch) Add(conn uint32, mode uint8, data []byte) error {
 
 func (x *Context) Submit(b *Batch) error {
 	return statusErr("sse_submit", C.sse_submit(x.c, b.Slot, C.uint32_t(b.nSegs), C.uint32_t(b.off)))
+}
+
+// Poll reports, without blocking, whether the work Submit queued for the batch (kernels and the counters' copy to the host)
+// has completed, so that Collect waits only for the batch's own result copies. With GPU_DEFER=1 a Collect after a ready Poll
+// may still run the decode stage again, when the slot's decode arenas grow.
+func (x *Context) Poll(b *Batch) (bool, error) {
+	rc := C.sse_poll(x.c, b.Slot)
+	if rc < 0 {
+		return false, statusErr("sse_poll", rc)
+	}
+	return rc == 1, nil
 }
 
 // Result views the pinned result buffers; valid until Release.
