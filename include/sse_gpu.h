@@ -228,7 +228,8 @@ const char *sse_last_cuda_error(void);
 int  sse_abi_version(void);
 void sse_default_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_per_batch);
 /* Capacities under which NO input can overflow a result arena (a batch of bytes_per_batch bytes on max_conns connections):
- * memory grows to ~30x the batch size, meant for small batcher arenas (sse_gateway.h uses it). With sse_default_config the
+ * memory grows to ~48x the batch size plus ~1.4 MB per connection (every connection may complete a line of its whole carry
+ * slot, whose payload the decode stage reads beyond the batch's input), meant for small batcher arenas (sse_gateway.h uses it). With sse_default_config the
  * capacities fit realistic SSE traffic and a pathological batch fails as a whole with SSE_ERR_OVERFLOW, unless the context
  * runs with SSE_FLAG_DEFER (then what does not fit waits for the next batch, or the decode arenas grow). */
 void sse_worst_case_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_per_batch);

@@ -425,7 +425,9 @@ __device__ __forceinline__ void f_elem_begin(const KParams &P, FLane &L) {
         if (fl_live(L)) {
             if (L.sf & SF_TCOPEN) f_flush_tc(P, L);
             L.sf |= SF_TCOPEN; L.tc_count++; L.tcb = 0;
-            const uint32_t idx = f_tc_alloc(P, L.tc_first == SSE_NONE ? SSE_NONE : L.tc_prev);
+            // a line that can no longer be JSON_OK never has its chain read: once the number in [1,1,...] has set SF_TYPE, the
+            // elements after it take no sse_tc, so every element allocated but the first of a line takes 3 payload bytes ("{},")
+            const uint32_t idx = (L.sf & (SF_SYN | SF_TYPE)) ? SSE_NONE : f_tc_alloc(P, L.tc_first == SSE_NONE ? SSE_NONE : L.tc_prev);
             if (idx != SSE_NONE) { if (L.tc_first == SSE_NONE) L.tc_first = idx; L.tc_prev = idx; }
             L.tc_cur = idx;
         }
@@ -451,14 +453,14 @@ __device__ __forceinline__ void f_null(const KParams &P, FSmem &S, FLane &L) {
     if (tgt == TG_NONE || tgt == TG_FINISH || tgt == TG_CONTENT || tgt == TG_PROMPT || tgt == TG_COMPLETION || tgt == TG_TOTAL ||
         tgt == TG_TC_INDEX || tgt == TG_NAME || tgt == TG_ARGS) return;      // null leaves non-pointer fields untouched
     const bool tco = (L.sf & SF_TCOPEN) && fl_live(L) && L.tc_cur != SSE_NONE;
-    if (tgt != TG_USAGE || L.usage_idx != SSE_NONE) rec_nonsimple(S, L);     // a reset is not something a template replays
+    if (tgt != TG_USAGE || (L.sf & SF_USAGE)) rec_nonsimple(S, L);     // a reset is not something a template replays
     switch (tgt) {
     case TG_CHOICES:
         L.n_choices = 0; L.choices_count = 0; L.finish = SSE_FIN_NONE; L.content_pos = L.content_len = 0;
         L.sf &= ~(SF_CDEC | SF_CBAD | SF_CSET);
         f_drop_tcs(L);
         break;
-    case TG_USAGE: L.sf &= ~SF_USAGE; L.usage_idx = SSE_NONE; break;
+    case TG_USAGE: L.sf &= ~SF_USAGE; break;     // the line keeps its sse_usage slot: a later "usage":{} zeroes and reuses it
     case TG_TOOLCALLS: if (fl_live(L)) f_drop_tcs(L); break;
     case TG_TC_ID:
         if ((L.sf & SF_TCOPEN) && fl_live(L)) { L.tcb &= ~(SSE_TC_HAS_ID | SSE_TC_ID_TEXT); if (tco) { sse_tc *t = &P.tcs[L.tc_cur]; f_cancel_job(S, &t->id_len); t->id_off = t->id_len = 0; } }
@@ -582,8 +584,11 @@ __device__ __forceinline__ void f_open(const KParams &P, FSmem &S, FLane &L, boo
             L.sd++;
             if (tgt != TG_NONE) {
                 if (tgt == TG_USAGE) {
-                    L.sf |= SF_USAGE;      // a fresh CompletionUsage{}; a repeated key decodes into the same struct
+                    // a fresh CompletionUsage{}; a repeated key decodes into the same struct. One slot per line: after
+                    // "usage":null the next object zeroes the line's slot instead of taking another (at most one usage per record)
                     if (L.usage_idx == SSE_NONE) L.usage_idx = f_usage_alloc(P);
+                    else if (!(L.sf & SF_USAGE)) { sse_usage z; z.prompt_tokens = z.completion_tokens = z.total_tokens = 0; P.usages[L.usage_idx] = z; }
+                    L.sf |= SF_USAGE;
                 }
                 else if (tgt == TG_TC_FUNCTION) { if (live && (L.sf & SF_TCOPEN)) L.tcb |= SSE_TC_HAS_FUNC; }
                 else if (tgt == TG_CHOICES) { if (L.n_choices || L.choices_count) rec_nonsimple(S, L); L.choices_count = 0; }
@@ -660,7 +665,7 @@ __device__ __forceinline__ void f_number_end(const KParams &P, FSmem &S, FLane &
         uint32_t op = OP_NONE;
         if (ty == TY_INT) {
             op = OP_CHK_I64;
-            if (L.usage_idx != SSE_NONE && (tgt == TG_PROMPT || tgt == TG_COMPLETION || tgt == TG_TOTAL)) op = OP_U_PROMPT + (tgt - TG_PROMPT);
+            if ((L.sf & SF_USAGE) && L.usage_idx != SSE_NONE && (tgt == TG_PROMPT || tgt == TG_COMPLETION || tgt == TG_TOTAL)) op = OP_U_PROMPT + (tgt - TG_PROMPT);
             else if (tgt == TG_TC_INDEX && (L.sf & SF_TCOPEN) && fl_live(L) && L.tc_cur != SSE_NONE && L.tc_count <= 16u) op = OP_TC_INDEX | ((L.tc_count - 1u) << 4);
         } else if (ty == TY_F32) op = OP_CHK_F32;
         rec_event(S, L, WK_INT, start, end - start, op);

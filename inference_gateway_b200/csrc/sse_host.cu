@@ -173,18 +173,23 @@ int do_launch(sse_ctx *c, Slot &s, uint32_t n_segs, cudaStream_t st) {
     return SSE_OK;
 }
 
-// Upper bounds of what one batch can ask of the decode stage's arenas. Every payload the decode stage reads stands in the batch's
-// input arena or in its out arena (lines completed from the carry slot or the line pool), so the bounds are sse_worst_case_config's
-// rules applied to both arenas together (the out arena already includes the line pool's growth): a tool-call element takes at
-// least 3 payload bytes ("{},"), a decoded string at most 4 text bytes per payload byte (U+FFFD for every invalid byte, 4-byte
-// aligned allocations), and there is at most one usage per record.
-sse_config worst_decode_caps(const sse_ctx *c) {
-    sse_config w = c->cfg;
-    const uint64_t payload = (uint64_t)w.in_arena_bytes + w.out_arena_bytes, cap = 0xF0000000ull;
+// The decode stage's arenas for a batch whose decoded payloads take at most `payload` bytes: a tool-call element is allocated only
+// while its line can still be JSON_OK, so it takes at least 3 payload bytes ("{},"); a decoded string takes at most 4 text bytes per
+// payload byte (U+FFFD for every invalid byte, 4-byte aligned allocations); there is at most one usage per record.
+void decode_caps(sse_config &w, uint64_t payload) {
+    const uint64_t cap = 0xF0000000ull;
     auto clamp = [&](uint64_t v) { return (uint32_t)(v > cap ? cap : v); };
     w.max_usages = w.max_recs;
     w.max_tcs = clamp(payload / 3 + 64);
     w.text_arena_bytes = clamp(4 * payload + 65536);
+}
+
+// Upper bounds of what one batch can ask of the decode stage's arenas. Every payload the decode stage reads stands in the batch's
+// input arena or in its out arena (lines completed from the carry slot or the line pool), so the bounds are decode_caps over both
+// arenas together (the out arena already includes the line pool's growth).
+sse_config worst_decode_caps(const sse_ctx *c) {
+    sse_config w = c->cfg;
+    decode_caps(w, (uint64_t)w.in_arena_bytes + w.out_arena_bytes);
     return w;
 }
 
@@ -332,7 +337,7 @@ void sse_default_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_per_
     cfg->max_tcs = (uint32_t)(in / 256 + 1024);
     cfg->max_usages = cfg->max_recs;
     cfg->text_arena_bytes = (uint32_t)(in / 4 + 65536);
-    cfg->max_runs = (uint32_t)(in / 2048 + max_conns + 1024);   // one extra run per window / 64 lines of a long segment
+    cfg->max_runs = (uint32_t)(in / 2048 + max_conns + 1024);   // one extra run per round of 64 lines: lines of 32 bytes or more
     cfg->carry_slot_bytes = 16384;
     cfg->n_slots = 2;
 }
@@ -344,11 +349,13 @@ void sse_worst_case_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_p
     cfg->carry_slot_bytes = 65536;                                   // longest supported line
     cfg->max_frames = clamp(in + 64);                                // a frame needs its own '\n' in this batch
     cfg->max_recs = clamp(in / 4 + 2ull * max_conns + 64);           // "data: x\n" is 8 bytes; one carried line per segment
-    cfg->max_usages = cfg->max_recs;
-    cfg->max_tcs = clamp(in / 3 + 64);                               // "{}," per element
-    cfg->text_arena_bytes = clamp(4 * in + 65536);                   // U+FFFD for every invalid byte: 1 -> 3, 4-byte aligned
     cfg->out_arena_bytes = clamp(in + in / 4 + (uint64_t)max_conns * (cfg->carry_slot_bytes + 32ull) + (1u << 20));
-    cfg->max_runs = clamp(in / 256 + 2ull * max_conns + 1024);
+    // the decode stage reads the batch's input and, for every connection, at most one line completed from its carry slot
+    decode_caps(*cfg, in + (uint64_t)max_conns * cfg->carry_slot_bytes);
+    // one runs[] entry per round of up to 64 lines after a segment's first: a round per 64 one-byte lines, and at most one more
+    // per window (a window after a segment's first takes half a window of new bytes or more, a line longer than a window
+    // completes once)
+    cfg->max_runs = clamp(in / 64 + in / 2048 + 2ull * max_conns + 1024);
 }
 
 void sse_line_pool_config(sse_config *cfg, const sse_line_pool *pool) {

@@ -155,6 +155,9 @@ template <class Q>
 __device__ void v2_flush_tc(const KParams &P, Lane &L, LaneScratch &S, Q *J) {
     if ((S.tc_flags & SSE_TC_HAS_ID) || ((S.tc_flags & SSE_TC_HAS_FUNC) && (S.name_len || S.args_len))) L.sf |= SF_TCVALID;
     L.sf &= ~SF_TCOPEN;
+    // a line that can no longer be JSON_OK never has its chain read: an element such as the number in [1,1,...] takes no sse_tc,
+    // so every element allocated takes at least 3 payload bytes ("{},")
+    if (L.sf & (SF_SYN | SF_TYPE)) return;
     uint32_t idx = atomicAdd(&P.ctr->n_tcs, 1u);
     if (idx >= P.cap_tcs) { sse_overflow(P.ctr, SSE_OVF_TCS); return; }
     sse_tc *rec = &P.tcs[idx];
