@@ -12,17 +12,33 @@ although its bytes are not in the batch. Every line a generator builds emits a f
 hold "[DONE]"), so every round of lines takes a run."""
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass, field
 
 import numpy as np
 
 from inference_gateway_b200 import _abi as A
+from inference_gateway_b200.engine import make_line_pool
 from tests import seams as S
 
 PP = A.MODE_P | A.MODE_PARSE
 R = A.MODE_R | A.MODE_PARSE
 ARENAS = ("frames", "recs", "items", "runs", "tcs", "usages", "out", "text")
 EXACT = ("frames", "recs", "items", "runs", "tcs", "usages")     # demand() counts these exactly; out and text are bounds
+TILE_SLOT = S.TILE - 32       # the longest carry slot the tile kernel accepts (sse_fused_max_line)
+
+
+def worst(conns: int, batch: int, pool=None, slot=None):
+    """sse_worst_case_config for conns connections and batch bytes, with carry_slot_bytes = slot when given and grown by
+    sse_line_pool_config for a line pool of make_line_pool(**pool) when given."""
+    cfg = A.Config()
+    A.load().sse_worst_case_config(C.byref(cfg), conns, batch)
+    if slot is not None:
+        cfg.carry_slot_bytes = slot
+    if pool is not None:
+        p = make_line_pool(**pool)
+        A.load().sse_line_pool_config(C.byref(cfg), C.byref(p))
+    return cfg
 
 
 def r4(n: int) -> int:

@@ -2,22 +2,11 @@
 layouts, and fails loudly without a CUDA device (no CPU fallback). No compute calls here."""
 import ctypes as C
 import os
-import re
 
 import pytest
 
 from inference_gateway_b200 import _abi as A
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = open(os.path.join(ROOT, "include", "sse_gpu.h")).read()
-
-
-GW_HEADER = open(os.path.join(ROOT, "include", "sse_gateway.h")).read()
-
-
-def declared_functions(text=None, prefix="sse_"):
-    body = re.sub(r"/\*.*?\*/", "", text or HEADER, flags=re.S)
-    return sorted(set(re.findall(r"\b(%s[a-z_0-9]+)\s*\(" % prefix, body)))
+from tests.util import GW_HEADER, declared_functions
 
 
 def test_exports_every_declared_symbol():

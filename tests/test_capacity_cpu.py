@@ -11,33 +11,20 @@ example no tool-call element after a type error). A kernel that allocates more t
 here: only test_gpu_capacity.py, which measures the kernels' own counts against the model, tells a kernel regression from a
 model that is right. test_legacy_bounds_are_broken_by_the_loads shows that the loads would break the earlier formulas and
 the earlier kernels' allocation rates, restated here."""
-import ctypes as C
 import functools
 import json
 
 import pytest
 
 from inference_gateway_b200 import _abi as A
-from inference_gateway_b200.engine import make_line_pool
 from oracle import orc
 from tests import capacity as K
 from tests import seams as S
+from tests.capacity import TILE_SLOT, worst
 
-TILE_SLOT = S.TILE - 32       # the longest carry slot the tile kernel accepts (sse_fused_max_line)
 GRID = [(8, 64 << 10), (8, 1 << 20), (8, 16 << 20), (64, 64 << 10), (64, 1 << 20), (256, 4 << 20), (1024, 64 << 10),
         (1024, 1 << 20), (1024, 16 << 20), (10, 1 << 20)]
 POOL = dict(pool_pages=64, page_bytes=65536)
-
-
-def worst(conns: int, batch: int, pool=None, slot=None):
-    cfg = A.Config()
-    A.load().sse_worst_case_config(C.byref(cfg), conns, batch)
-    if slot is not None:
-        cfg.carry_slot_bytes = slot
-    if pool is not None:
-        p = make_line_pool(**pool)
-        A.load().sse_line_pool_config(C.byref(cfg), C.byref(p))
-    return cfg
 
 
 @functools.lru_cache(None)

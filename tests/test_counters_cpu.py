@@ -3,7 +3,7 @@ import ctypes as C
 import re
 
 from inference_gateway_b200 import _abi as A
-from tests.test_abi import GW_HEADER, HEADER, declared_functions
+from tests.util import GW_HEADER, HEADER, declared_functions
 
 
 def header_counter_fields():

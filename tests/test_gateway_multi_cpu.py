@@ -7,7 +7,7 @@ import pytest
 
 from inference_gateway_b200 import _abi as A
 from inference_gateway_b200.gateway import Gateway
-from tests.test_abi import GW_HEADER, HEADER, declared_functions
+from tests.util import GW_HEADER, HEADER, declared_functions
 
 
 def _cfg(n_slots=4, conns=16):

@@ -20,9 +20,8 @@ from inference_gateway_b200.gateway import Gateway
 from oracle import orc
 from tests import capacity as K
 from tests import seams as S
-from tests.test_capacity_cpu import TILE_SLOT, worst
-from tests.test_gpu_occupancy import ENGINES
-from tests.util import check_result, oracle_digests
+from tests.capacity import TILE_SLOT, worst
+from tests.util import ENGINES, assert_digest_parity, check_result
 
 pytestmark = pytest.mark.gpu
 CONNS, BATCH = 10, 1 << 20
@@ -120,7 +119,7 @@ def _hold_budget(cfg):
 
 def _hold(eng, loads, cut) -> list:
     """Runs each load next to the good streams, in two batches (the prefixes and the good streams' first pieces, then the
-    rest), and returns the batches that overflowed and the connections that differ from the oracle."""
+    rest), and returns the batches that overflowed and the loads that differ from the oracle (assert_digest_parity)."""
     good, gmodes = _good_streams()
     bad = []
     for g in loads:
@@ -140,13 +139,10 @@ def _hold(eng, loads, cut) -> list:
         if st != A.SSE_OK:
             bad.append(f"{g.name}: {msg}")
             continue
-        od, _, _ = oracle_digests(bodies, modes)
-        for key in ("n_frames", "frame_bytes", "frames_h", "n_recs", "recs_h"):
-            diff = np.nonzero(d[0][key] != od[key])[0]
-            if diff.size:
-                bad.append(f"{g.name}: connections {diff.tolist()} differ from the oracle in {key}")
-        assert int(d[0]["inexact"].sum()) == 0, g.name
-        assert not np.any(d[2] & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG)), g.name
+        try:
+            assert_digest_parity(d, bodies, modes, g.name)
+        except AssertionError as e:
+            bad.append(str(e))
     return bad
 
 

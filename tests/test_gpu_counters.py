@@ -7,15 +7,14 @@ import torch
 
 from inference_gateway_b200 import SseEngine, _abi as A, synth
 from inference_gateway_b200.gateway import Gateway
-from tests.test_gpu_long_lines import PAGE, chunk, long_line
-from tests.test_gpu_occupancy import TARGET, dealt, filler_payload, parity, shape_check
-from tests.test_gpu_whole_tokens import documents
-from tests.util import cut_bounds, decode_shape, digest_run, oracle_digests, process_all_checked, run_pieces
+from tests.corpus import documents
+from tests.streams import PAGE, chunk, dealt, filler_payload, long_line
+from tests.util import (TARGET, check_batch, cut_bounds, decode_shape, digest_parity, digest_run, oracle_digests,
+                        process_all_checked, run_pieces, shape_check)
 
 pytestmark = pytest.mark.gpu
 R, PP, P = A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE, A.MODE_P
 MiB = 1 << 20
-CYCLES = ("c_pull", "c_skip", "c_coop", "c_steps", "c_finish", "c_unquote")
 LINE_ONLY = ("d_actions", "d_action_redos", "d_unquote_jobs", "d_unquote_bytes")   # depend on the lines alone
 
 
@@ -23,52 +22,6 @@ def counting(flags=0, **kw):
     """An engine with SSE_FLAG_COUNTERS and one slot (so that an on_batch hook knows the slot: 0)."""
     kw.setdefault("n_slots", 1)
     return SseEngine(device=0, flags=A.FLAG_COUNTERS | flags, **kw)
-
-
-def text_spans(res):
-    """(spans flagged SSE_F_CONTENT_TEXT or SSE_TC_*_TEXT, records with at least one, whether any tool-call element has two)"""
-    recs, tcs = res.recs, res.tcs
-    content = (recs["flags"] & A.F_CONTENT_TEXT) != 0
-    per_tc = np.array([bin(int(f) & 0xF0).count("1") for f in tcs["flags"]], dtype=np.int64)
-    with_text = content.copy()
-    for i in np.nonzero(~content)[0]:
-        t = int(recs["tc_first"][i])
-        while t != A.NONE and t < len(tcs) and not with_text[i]:
-            with_text[i] = per_tc[t] > 0
-            t = int(tcs["next"][t])
-    return int(content.sum() + per_tc.sum()), int(with_text.sum()), bool((per_tc > 1).any())
-
-
-def check_batch(k, res, submitted=None, one_job_per_span=True):
-    """The identities every batch satisfies. submitted: the batch's input bytes (their '\\n' are the complete lines when no
-    segment stopped early)."""
-    raw = res.raw
-    assert k["decode_passes"] == (1 if raw.n_segs else 0) or k["decode_passes"] > 1, k
-    assert k["p_segments"] == raw.n_segs, (k, raw.n_segs)
-    assert k["p_items"] == raw.n_decoded, (k, raw.n_decoded)
-    assert k["p_frames_zero_copy"] + k["p_frames_materialised"] == raw.n_frames, (k, raw.n_frames)
-    mat = res.frames["off"] < res.in_base
-    assert k["p_bytes_materialised"] == int(res.frames["len"][mat].sum()), (k, int(res.frames["len"][mat].sum()))
-    if submitted is not None:
-        nl = submitted.count(b"\n")
-        stopped = int(np.count_nonzero(res.segs["flags"] & (A.SEG_TERMINATED | A.SEG_FINISHED | A.SEG_DEAD | A.SEG_DEFERRED)))
-        assert k["p_lines"] == nl if not stopped else k["p_lines"] <= nl, (k, nl, stopped)
-    decoded = (res.recs["flags"] & A.F_DONE_EXACT) == 0          # an exact "data: [DONE]" gets a record but no work item
-    moved = (k["d_skip_bytes"] + k["d_coop_bytes"] + k["d_plain_steps"] + k["d_actions"] + k["d_abandoned_bytes"]
-             + k["d_template_bytes"])
-    assert moved == int(res.recs["payload_len"][decoded].sum()), k
-    assert k["d_items"] == k["d_lines_finished"] == raw.n_decoded, (k, raw.n_decoded)
-    assert k["d_busy_lane_rounds"] <= 32 * k["d_warp_rounds"], k
-    assert sum(k[c] for c in CYCLES) <= k["c_total"], k
-    if raw.n_decoded:
-        assert k["d_items_per_pull"] in (8, 16, 32) and k["d_pulls"] > 0, k
-    # every unquote job yields one text span. A lane queues one job at a time (the warp drains the queues every two rounds), so
-    # a line's first string to unquote is always a job, and a tool-call element with two such strings, or a line replayed
-    # from a template (all its captures at once), unquotes the rest on its lane
-    spans, lines, two = text_spans(res)
-    assert lines <= k["d_unquote_jobs"] <= spans, (k, lines, spans)
-    if one_job_per_span and not two:
-        assert k["d_unquote_jobs"] == spans, (k, spans)
 
 
 def counter_hook(eng, bodies, bounds, got, one_job_per_span=True, on_batch=None):
@@ -84,10 +37,9 @@ def counter_hook(eng, bodies, bounds, got, one_job_per_span=True, on_batch=None)
 
 
 def counted_parity(eng, bodies, modes, bounds, label, one_job_per_span=True, on_batch=None):
-    """parity() (oracle digests and orc_check_result per batch) collecting every batch's counters, checked by check_batch."""
+    """digest_parity (oracle digests and orc_check_result per batch) collecting every batch's counters, checked by check_batch."""
     got = []
-    modes_arr = np.broadcast_to(np.asarray(modes, dtype=np.uint8), (len(bodies),))
-    parity(eng, bodies, modes_arr, bounds, on_batch=counter_hook(eng, bodies, bounds, got, one_job_per_span, on_batch), label=label)
+    digest_parity(eng, bodies, modes, bounds, label, on_batch=counter_hook(eng, bodies, bounds, got, one_job_per_span, on_batch))
     return got
 
 
@@ -100,7 +52,7 @@ def total(ks, name):
 def test_full_size_results_unchanged_and_counted(name, n_streams, mode):
     bodies = [b for b, _, _ in synth.make_config(name, n_streams=n_streams)[0]]
     nbytes = sum(map(len, bodies))
-    od, _, _ = oracle_digests(bodies, mode)
+    oracle = oracle_digests(bodies, mode)
     plain = SseEngine(device=0, max_conns=n_streams, bytes_per_batch=nbytes, n_slots=1, carry_slot_bytes=16384)
     try:
         ref = {nb: digest_run(plain, bodies, mode, cut_bounds(bodies, nb, seed=700 + nb)) for nb in (1, 4)}
@@ -111,12 +63,10 @@ def test_full_size_results_unchanged_and_counted(name, n_streams, mode):
         for nb in (1, 4):
             bounds = cut_bounds(bodies, nb, seed=700 + nb)
             ks = []
-            gd, carry, flags = digest_run(eng, bodies, mode, bounds, on_batch=counter_hook(eng, bodies, bounds, ks))
+            got = digest_parity(eng, bodies, mode, bounds, f"{name} x{nb} counting", oracle=oracle,
+                                on_batch=counter_hook(eng, bodies, bounds, ks))
             assert len(ks) == nb
-            rd, rcarry, rflags = ref[nb]
-            for key in ("n_frames", "frame_bytes", "frames_h", "n_recs", "recs_h"):
-                assert np.array_equal(gd[key], rd[key]) and np.array_equal(gd[key], od[key]), (name, nb, key)
-            assert np.array_equal(carry, rcarry) and np.array_equal(flags, rflags)
+            assert all(np.array_equal(x, y) for x, y in zip(got, ref[nb])), (name, nb)      # the plain engine's results
             if mode == R:                 # valid documents only (mode P|PARSE also decodes the payload of "data: [DONE]")
                 assert total(ks, "d_abandoned_bytes") == 0
             assert total(ks, "d_template_lines") == 0 and total(ks, "p_long_lines") == 0

@@ -10,16 +10,14 @@ from inference_gateway_b200 import SseEngine, _abi as A, synth
 from inference_gateway_b200.gateway import Gateway
 from inference_gateway_b200.synth import random_cuts
 from oracle import orc
-from tests.corpus import TRICKY, mutate
-from tests.util import ConnOut, agent_results, check_stream, fold_segment, process_all_checked, process_checked, telemetry_results
+from tests.corpus import adversarial_bodies
+from tests.util import (ENGINES, TINY_DECODE, TINY_PRODUCE, ConnOut, check_streams, fold_segment, process_all_checked,
+                        process_checked)
 
 pytestmark = pytest.mark.gpu
 
 P, R, PP = A.MODE_P, A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
 MiB = 1 << 20
-# produce-side capacities far below what a batch of these streams needs, but enough for one round (64 lines) of one segment
-TINY_PRODUCE = dict(max_frames=128, max_recs=64, out_arena_bytes=32 * 1024, max_runs=16)
-TINY_DECODE = dict(max_tcs=8, max_usages=4, text_arena_bytes=512)
 
 
 def run_deferred(eng, bodies, modes, n_batches=1, seed=0, with_folds=False, n_folds=None):
@@ -52,34 +50,6 @@ def run_deferred(eng, bodies, modes, n_batches=1, seed=0, with_folds=False, n_fo
     return outs, stats
 
 
-def check_all(eng, bodies, modes, outs, label):
-    views = [check_stream(b, m, o, label=f"{label} stream {i} mode {m}") for i, (b, m, o) in enumerate(zip(bodies, modes, outs))]
-    L = eng.L
-    for i, (m, o, v) in enumerate(zip(modes, outs, views)):
-        if o.agent is None:
-            continue
-        if m == R:
-            content, has, term, fin, calls = agent_results(L, o.agent)
-            assert content == v.acc_content and has == v.has_tool_calls and term == v.terminated, i
-            assert calls == orc.parse_tool_calls(v.builder), i
-            done = b"data: [DONE]\n\n"
-            A.check(L.sse_telemetry_feed_bytes(o.tele, done, len(done)), "sse_telemetry_feed_bytes")
-            assert telemetry_results(L, o.tele) == (0, *orc.telemetry(b"".join(o.frames) + done)), i
-        elif m == PP:
-            assert telemetry_results(L, o.tele) == (0, *orc.telemetry(b"".join(o.frames))), i
-    return views
-
-
-def adversarial_bodies(rng, n):
-    out = []
-    for k in range(n):
-        docs = [TRICKY[int(rng.integers(0, len(TRICKY)))] for _ in range(int(rng.integers(4, 40)))]
-        docs = [mutate(rng, d) if rng.random() < 0.4 else d for d in docs]
-        sep = [b"\n\n", b"\n", b"\r\n\r\n", b"\n: ping\n\n"][k % 4]
-        out.append(b"".join(b"data: " + d + sep for d in docs) + (b"data: [DONE]\n\n" if k % 3 else b"data: {\"tail"))
-    return out
-
-
 N_C4 = 160
 
 
@@ -95,7 +65,7 @@ def mixed_bodies(seed, n_c4=N_C4, n_adv=60):
 
 @pytest.fixture(scope="module", params=["split", "templates", "copy"])
 def tiny(request):
-    flags = A.FLAG_DEFER | {"split": 0, "templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT}[request.param]
+    flags = A.FLAG_DEFER | ENGINES[request.param]
     e = SseEngine(device=0, max_conns=512, bytes_per_batch=4 * MiB, flags=flags, **TINY_PRODUCE)
     yield e
     e.close()
@@ -105,7 +75,7 @@ def tiny(request):
 def test_produce_side_deferral_is_bit_exact(tiny, n_batches):
     bodies, modes = mixed_bodies(n_batches)
     outs, st = run_deferred(tiny, bodies, modes, n_batches=n_batches, seed=n_batches, with_folds=True, n_folds=N_C4)
-    check_all(tiny, bodies, modes, outs, f"tiny batches={n_batches}")
+    check_streams(bodies, modes, outs, f"tiny batches={n_batches}", tiny.L)
     assert st["deferred"] > 0 and st["overflow"] & (A.OVF_OUT | A.OVF_RUNS)
     assert not any(o.flags & A.SEG_DEAD for o in outs)
 
@@ -139,12 +109,12 @@ def test_decode_side_arenas_grow_and_the_batch_is_decoded_again(flags):
     e = SseEngine(device=0, max_conns=64, bytes_per_batch=1 * MiB, flags=A.FLAG_DEFER | flags, n_slots=1, **TINY_DECODE)
     try:
         outs, st = run_deferred(e, bodies, modes, n_batches=2, seed=1, with_folds=True)
-        check_all(e, bodies, modes, outs, "decode growth")
+        check_streams(bodies, modes, outs, "decode growth", e.L)
         grown = A.OVF_TCS | A.OVF_USAGES | A.OVF_TEXT
         assert st["overflow"] & grown == grown and st["deferred"] == 0
         # the slot keeps what it grew to: the same batches again need no second pass
         outs, st = run_deferred(e, bodies, modes, n_batches=2, seed=1, with_folds=True)
-        check_all(e, bodies, modes, outs, "decode growth, second run")
+        check_streams(bodies, modes, outs, "decode growth, second run", e.L)
         assert st["overflow"] == 0
     finally:
         e.close()
@@ -177,8 +147,7 @@ def test_deferral_at_a_first_line_that_starts_in_the_carried_tail():
                 fold_segment(outs[c], res, i)
         process_all_checked(e, [(c, PP, rest) for c in range(len(bodies))], on_batch)
         assert len(seen) >= len(bodies) - 2 and set(seen) == {len(head)}
-        for i, (b, o) in enumerate(zip(bodies, outs)):
-            check_stream(b, PP, o, label=f"carry stream {i}")
+        check_streams(bodies, PP, outs, "carry")
     finally:
         e.close()
 
@@ -240,9 +209,8 @@ def test_pooled_line_whose_completion_does_not_fit_waits_at_its_newline():
         # one line waited, at its '\n' (consumed 0); the other completed, and what followed it may have waited too (the failed
         # reservation left the out-arena counter past the capacity)
         assert n == 2 and stops.count(0) == 1 and all(c in (0, 1) for c in stops)
-        for i, (b, o) in enumerate(zip(bodies, outs)):
-            check_stream(b, R, o, label=f"pooled {i}")
-            assert o.terminated
+        check_streams(bodies, R, outs, "pooled")
+        assert all(o.terminated for o in outs)
         assert e.pool_stats()[0] == 0
     finally:
         e.close()
@@ -290,9 +258,8 @@ def test_line_whose_newline_would_leave_the_carry_slot_keeps_its_bytes_when_defe
         second[0] = True
         assert process_all_checked(e, [(c, PP, b[10000:]) for c, b in enumerate(bodies)], on_batch) >= 8
         assert len(waited) >= 7 and taken == [len(b) - 10000 for b in bodies]
-        for i, (b, o) in enumerate(zip(bodies, outs)):
-            check_stream(b, PP, o, label=f"keep={keep} stream {i}")
-            assert not o.flags & A.SEG_DEAD
+        check_streams(bodies, PP, outs, f"keep={keep}")
+        assert not any(o.flags & A.SEG_DEAD for o in outs)
         assert e.pool_stats()[0] == 0
     finally:
         e.close()

@@ -10,7 +10,8 @@ from inference_gateway_b200 import _abi as A, synth
 from inference_gateway_b200.gateway import Gateway
 from inference_gateway_b200.synth import random_cuts
 from oracle import orc
-from tests.test_gpu_defer import TINY_PRODUCE, adversarial_bodies
+from tests.corpus import adversarial_bodies
+from tests.util import TINY_PRODUCE, check_agent
 
 pytestmark = pytest.mark.gpu
 
@@ -81,11 +82,7 @@ def check_oracle(bodies, modes, outs, label):
         if m == R:
             v = orc.reframe(b)
             want = [l.out for l in v.lines if l.kind == orc.L_EMITTED]
-            content, has, term, fin, calls = o.agent
-            assert content == v.acc_content and has == v.has_tool_calls and term == v.terminated, f"{label} stream {i}"
-            assert calls == orc.parse_tool_calls(v.builder), f"{label} stream {i}"
-            if v.terminated:
-                assert fin == v.term_finish, f"{label} stream {i}"
+            check_agent(o.agent, v, f"{label} stream {i}")
         else:
             want = [l.out for l in orc.passthrough(b, parse=bool(m & A.MODE_PARSE)).lines]
         assert o.frames == want, f"{label} stream {i} mode {m}: {len(o.frames)} frames, oracle {len(want)}"

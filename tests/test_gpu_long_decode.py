@@ -10,12 +10,10 @@ import pytest
 
 from inference_gateway_b200 import SseEngine, _abi as A, synth
 from inference_gateway_b200.gateway import Gateway
-from tests.test_gpu_counters import check_batch, text_spans
-from tests.test_gpu_long_lines import USAGE, _filler, chunk, long_line, stream_with
 from oracle import orc
-from tests.test_gpu_occupancy import parity
-from tests.util import (agent_results, check_stream, cut_bounds, digest_run_pipelined, oracle_digests, run_streams,
-                        telemetry_results)
+from tests.streams import USAGE, chunk, filler, long_line, stream_with
+from tests.util import (ENGINES, check_agent, check_batch, check_folds, check_stream, check_streams, cut_bounds, digest_parity,
+                        run_streams, text_spans)
 
 pytestmark = pytest.mark.gpu
 P, R, PP = A.MODE_P, A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
@@ -41,7 +39,7 @@ def engine(flags=0, **kw):
 
 @pytest.fixture(scope="module", params=["split", "templates", "copy"])
 def eng(request):
-    e = engine({"split": 0, "templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT}[request.param])
+    e = engine(ENGINES[request.param])
     yield e
     e.close()
 
@@ -71,7 +69,7 @@ def streams_of(lines, tail=b""):
 def check_all(e, bodies, modes=(R, PP), nbs=(1, 3), label=""):
     for m in modes:
         for nb in nbs:
-            parity(e, bodies, m, cut_bounds(bodies, nb, seed=nb), label=f"{label} mode {m} x{nb}")
+            digest_parity(e, bodies, m, cut_bounds(bodies, nb, seed=nb), f"{label} mode {m} x{nb}")
 
 
 # ------------------------------------------------------------------ the seam
@@ -79,7 +77,7 @@ def test_seam(eng):
     rng = np.random.default_rng(1)
     lines = []
     for n in (LONG - 1, LONG, LONG + 1):
-        lines.append(sized(lambda k: _filler(rng, k), n))
+        lines.append(sized(lambda k: filler(rng, k), n))
         lines.append(sized(lambda k: b"x" * k, n))
         lines.append(sized(lambda k: ("中\U0001F600".encode() * k)[:k // 7 * 7] + b"y" * (k % 7), n))
         tc = long_line("toolcall", n + 7, rng)[:-1]
@@ -132,7 +130,7 @@ def test_errors_across_a_whole_step():
         lines += [content_line(b"x" * (LONG + off) + end, closed=False) for end in ENDS for off in range(528)]
         for k in range(0, len(lines), 2000):
             bodies = streams_of(lines[k:k + 2000])
-            parity(e, bodies, R, cut_bounds(bodies, 1, seed=k), label=f"errors across a step, lines {k}..")
+            digest_parity(e, bodies, R, cut_bounds(bodies, 1, seed=k), f"errors across a step, lines {k}..")
     finally:
         e.close()
 
@@ -143,7 +141,6 @@ def test_folds_of_long_tool_calls():
     e = engine(max_conns=64, bytes_per_batch=16 * MiB)
     try:
         rng = np.random.default_rng(14)
-        done = b"data: [DONE]\n\n"
         bodies = [chunk(b"Writing.") + long_line("toolcall", n, rng) + b"\n" +
                   b'data: {"choices":[{"index":0,"delta":{},"finish_reason":"tool_calls"}]}\n\n' + USAGE
                   for n in (LONG + 6, LONG + 7, LONG + 8, 5 * LONG, 2 * MiB)]   # payloads LONG - 1, LONG, LONG + 1, ...
@@ -151,12 +148,8 @@ def test_folds_of_long_tool_calls():
             outs = run_streams(e, bodies, [R] * len(bodies), n_batches=nb, seed=nb, with_folds=True)
             for i, (b, o) in enumerate(zip(bodies, outs)):
                 v = check_stream(b, R, o, label=f"folds stream {i} x{nb}")
-                content, has, term, fin, calls = agent_results(e.L, o.agent)
-                assert content == v.acc_content and has and term and fin == 2
-                assert calls == orc.parse_tool_calls(v.builder) and len(calls) == 1
-                A.check(e.L.sse_telemetry_feed_bytes(o.tele, done, len(done)), "sse_telemetry_feed_bytes")
-                rc, usage, tcalls = telemetry_results(e.L, o.tele)
-                assert rc == 0 and (usage, tcalls) == orc.telemetry(b"".join(o.frames) + done)
+                _, has, term, fin, calls = check_folds(e.L, o, R, v, f"folds stream {i} x{nb}")
+                assert has and term and fin == 2 and len(calls) == 1
                 e.L.sse_agent_free(o.agent)
                 e.L.sse_telemetry_free(o.tele)
     finally:
@@ -165,7 +158,7 @@ def test_folds_of_long_tool_calls():
 
 # ------------------------------------------------------------------ long strings in every capture
 def esc(n, rng):
-    return _filler(rng, n)
+    return filler(rng, n)
 
 
 def tc_elem(i, parts):
@@ -201,8 +194,7 @@ def test_every_capture(eng):
     bodies = streams_of(lines, USAGE)
     check_all(eng, bodies, label="captures")
     outs = run_streams(eng, bodies, [R] * len(bodies), n_batches=2, seed=4)
-    for i, (b, o) in enumerate(zip(bodies, outs)):
-        check_stream(b, R, o, label=f"capture line {i}")
+    check_streams(bodies, R, outs, "captures")
 
 
 def test_terminating_long_chunk():
@@ -258,7 +250,7 @@ def test_deferred_redecode_runs_the_long_kernel():
             k = e.counters(0)
             check_batch(k, res)
             passes.append(k["decode_passes"])
-        parity(e, bodies, R, cut_bounds(bodies, 1, seed=1), on_batch=hook, label="deferred")
+        digest_parity(e, bodies, R, cut_bounds(bodies, 1, seed=1), "deferred", on_batch=hook)
         assert max(passes) > 1, passes
     finally:
         e.close()
@@ -272,11 +264,7 @@ def test_batches_in_flight():
         bodies[i] = bodies[i][:cut] + long_line("toolcall", LONG + int(rng.integers(0, 4 * LONG)), rng) + b"\n" + bodies[i][cut:]
     e = engine(max_conns=len(bodies), bytes_per_batch=32 * MiB, n_slots=4)
     try:
-        bounds = cut_bounds(bodies, 4, seed=9)
-        od, _, _ = oracle_digests(bodies, R)
-        gd, _, _ = digest_run_pipelined(e, bodies, R, bounds, depth=4)
-        for key in ("n_frames", "frame_bytes", "frames_h", "n_recs", "recs_h"):
-            assert np.array_equal(gd[key], od[key]), key
+        digest_parity(e, bodies, R, cut_bounds(bodies, 4, seed=9), "batches in flight", depth=4)
     finally:
         e.close()
 
@@ -291,8 +279,8 @@ def test_mixed_traffic_and_a_context_without_long_lines():
         bodies[i] = bodies[i][:cut] + long_line("toolcall", 200_000, rng) + b"\n" + bodies[i][cut:]
     e = engine(max_conns=len(bodies), bytes_per_batch=sum(map(len, bodies)))
     try:
-        parity(e, bodies, R, cut_bounds(bodies, 4, seed=11), label="mixed")
-        parity(e, plain, R, cut_bounds(plain, 4, seed=12), label="no long line")
+        digest_parity(e, bodies, R, cut_bounds(bodies, 4, seed=11), "mixed")
+        digest_parity(e, plain, R, cut_bounds(plain, 4, seed=12), "no long line")
     finally:
         e.close()
 
@@ -309,10 +297,11 @@ def test_gateway_folds_a_long_tool_call():
             g.pump()
         g.upstream_close(sid)
         g.pump()
-        content, has, term, fin, calls = g.agent_state(sid)
-        v = orc.reframe(body)
-        assert has and term and fin == 2 and content == v.acc_content == b"Saving."
-        assert calls == orc.parse_tool_calls(v.builder) and len(calls) == 1 and len(calls[0]["args"]) > 2 * LONG
+        state = g.agent_state(sid)
+        check_agent(state, orc.reframe(body), "gateway")
+        content, has, term, fin, calls = state
+        assert has and term and fin == 2 and content == b"Saving."
+        assert len(calls) == 1 and len(calls[0]["args"]) > 2 * LONG
         g.release(sid)
     finally:
         g.close()

@@ -7,14 +7,13 @@ import pytest
 
 from inference_gateway_b200 import SseEngine, _abi as A, synth
 from oracle import orc
-from tests.util import agent_results, check_stream, run_pieces, run_streams, telemetry_results
+from tests.streams import PAGE, SLOT, USAGE, chunk, long_line, stream_with
+from tests.util import ENGINES, check_folds, check_stream, check_streams, run_pieces, run_streams
 
 pytestmark = pytest.mark.gpu
 
 P, R, PP = A.MODE_P, A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
 MODES = (P, R, PP)
-SLOT = 32768
-PAGE = 65536
 MiB = 1 << 20
 
 
@@ -23,76 +22,9 @@ def eng(request):
     """The default pipeline, with skeleton templates, and with SSE_FLAG_COPY_OUT, each with a 64 MiB line pool. Decoded text
     of a line may take 3 bytes per input byte (invalid UTF-8 -> U+FFFD), so the text arena is raised for 16 MiB lines."""
     e = SseEngine(device=0, max_conns=1024, bytes_per_batch=64 * MiB, carry_slot_bytes=SLOT, n_slots=2,
-                  text_arena_bytes=128 * MiB, flags={"split": 0, "templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT}[request.param],
-                  line_pool=dict(pool_pages=1024, page_bytes=PAGE))
+                  text_arena_bytes=128 * MiB, flags=ENGINES[request.param], line_pool=dict(pool_pages=1024, page_bytes=PAGE))
     yield e
     e.close()
-
-
-# ------------------------------------------------------------------ stream builders
-UNITS = [b"ab", b"cdef", b"\\n", b'\\"', b"\\\\", b"\\u00e9", "é".encode(), "€".encode(), "😀".encode(), b"\\t", b" "]
-
-
-def _filler(rng, n):
-    """n bytes of a JSON string body: escapes and multi-byte UTF-8 mixed into ASCII."""
-    parts, k = [], 0
-    idx = rng.integers(0, len(UNITS), size=n // 2 + 8)
-    for i in idx:
-        u = UNITS[i]
-        if k + len(u) > n - 6:
-            break
-        parts.append(u)
-        k += len(u)
-    parts.append(b"x" * (n - k))
-    return b"".join(parts)
-
-
-def _ascii_args(rng, n):
-    """JSON text of n bytes, escaped as a JSON string body (a file written whole through an MCP tool)."""
-    head = b'{\\"path\\":\\"notes.md\\",\\"content\\":\\"'
-    tail = b'\\"}'
-    line = b"line of the file\\n"
-    body = (line * ((n - len(head) - len(tail)) // len(line) + 1))[:n - len(head) - len(tail)]
-    if body.endswith(b"\\"):
-        body = body[:-1] + b"x"
-    return head + body + tail
-
-
-def long_line(kind, n, rng):
-    """One line of exactly n bytes ('\\n' or '\\r\\n' included)."""
-    end = b"\r\n" if kind == "crlf" else b"\n"
-    if kind in ("toolcall", "terminal"):
-        fin = b'"tool_calls"' if kind == "terminal" else b"null"
-        pre = b'data: {"choices":[{"index":0,"delta":{"tool_calls":[{"index":0,"id":"call_big","type":"function","function":{"name":"write_file","arguments":"'
-        post = b'"}}]},"finish_reason":' + fin + b"}]}" + end
-        return pre + _ascii_args(rng, n - len(pre) - len(post)) + post
-    pre = b'data: {"id":"c","choices":[{"index":0,"delta":{"content":"'
-    post = b'"},"finish_reason":null}]}' + end
-    body = _filler(rng, n - len(pre) - len(post))
-    if kind == "done":       # "[DONE]" inside the line: mode R swallows it (agent.go:181-184), it is still decoded
-        mid = len(body) // 2
-        while body[mid - 1:mid] == b"\\" or (body[mid] & 0xC0) == 0x80:
-            mid += 1
-        body = body[:mid] + b"[DONE]" + body[mid + 6:]
-    return pre + body + post
-
-
-def chunk(content, fin="null"):
-    return b'data: {"choices":[{"index":0,"delta":{"content":"%s"},"finish_reason":%s}]}\n\n' % (content, fin.encode())
-
-
-USAGE = b'data: {"choices":[],"usage":{"prompt_tokens":11,"completion_tokens":22,"total_tokens":33}}\n\n'
-
-
-def stream_with(line, kind):
-    body = chunk(b"Hello") + chunk(b"world") + line + (b"\r\n" if kind == "crlf" else b"\n")
-    if kind == "terminal":    # the long line itself ends the agent loop: what follows is never read in mode R
-        return body + chunk(b"never read") + b"data: [DONE]\n\n"
-    return body + chunk(b"bye", '"stop"') + USAGE + b"data: [DONE]\n\n"
-
-
-def _check_all(bodies, modes, outs, label):
-    return [check_stream(b, m, o, label=f"{label} stream {i} mode {m}") for i, (b, m, o) in enumerate(zip(bodies, modes, outs))]
 
 
 LENGTHS = [64 * 1024 + 1, 100_000, MiB, 8 * MiB, A.MAX_LINE_BYTES]
@@ -116,7 +48,7 @@ def test_long_line_lengths(eng, length, n_batches):
             bodies.append(stream_with(line, kind))
             modes.append(m)
     outs = run_streams(eng, bodies, modes, n_batches=n_batches, seed=length + n_batches, with_folds=True)
-    _check_all(bodies, modes, outs, f"L={length} batches={n_batches}")
+    check_streams(bodies, modes, outs, f"L={length} batches={n_batches}")
     assert not any(o.flags & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG) for o in outs)
     assert eng.pool_stats()[0] == 0          # every line completed: every page is back
 
@@ -128,18 +60,12 @@ def test_one_mib_tool_call_folds(eng):
     body = chunk(b"Writing the file.") + line + b"\n" + b'data: {"choices":[{"index":0,"delta":{},"finish_reason":"tool_calls"}]}\n\n' + USAGE
     for nb in (1, 8):
         outs = run_streams(eng, [body, body], [R, PP], n_batches=nb, seed=nb, with_folds=True)
-        vr, vp = _check_all([body, body], [R, PP], outs, f"folds batches={nb}")
-        content, has, term, fin, calls = agent_results(eng.L, outs[0].agent)
-        assert content == vr.acc_content and has and term and fin == 2
-        assert calls == orc.parse_tool_calls(vr.builder)
+        views = check_streams([body, body], [R, PP], outs, f"folds batches={nb}")
+        content, has, term, fin, calls = check_folds(eng.L, outs[0], R, views[0], f"folds batches={nb}")
+        check_folds(eng.L, outs[1], PP, views[1], f"folds batches={nb} mode {PP}")
+        assert has and term and fin == 2
         args = json.loads(line[6:])["choices"][0]["delta"]["tool_calls"][0]["function"]["arguments"].encode()
         assert len(calls) == 1 and calls[0]["args"] == args and len(args) > 900_000
-        done = b"data: [DONE]\n\n"
-        A.check(eng.L.sse_telemetry_feed_bytes(outs[0].tele, done, len(done)), "sse_telemetry_feed_bytes")
-        rc, usage, tcalls = telemetry_results(eng.L, outs[0].tele)
-        assert rc == 0 and (usage, tcalls) == orc.telemetry(b"".join(outs[0].frames) + done)
-        rc, usage, tcalls = telemetry_results(eng.L, outs[1].tele)
-        assert rc == 0 and (usage, tcalls) == orc.telemetry(b"".join(outs[1].frames))
         for o in outs:
             eng.L.sse_agent_free(o.agent)
             eng.L.sse_telemetry_free(o.tele)
@@ -159,7 +85,7 @@ def test_mixed_workload_with_rare_long_tool_calls(eng):
         bodies.append(b)
     assert n_long >= 5
     outs = run_streams(eng, bodies, [mode] * len(bodies), n_batches=6, seed=3)
-    _check_all(bodies, [mode] * len(bodies), outs, "mixed C4")
+    check_streams(bodies, [mode] * len(bodies), outs, "mixed C4")
     assert not any(o.flags & A.SEG_DEAD for o in outs)
     eng.reset_all()
     assert eng.pool_stats()[0] == 0
@@ -311,7 +237,7 @@ def test_empty_segments_while_a_line_is_held(page):
             if held % page == 0 and held > SLOT:       # the pooled prefix is a whole number of pages when the empty segment comes
                 pieces = [body[:cut], b"", b"", body[cut:]]
             outs = run_pieces(e, [pieces] * 3, list(MODES))
-            _check_all([body] * 3, list(MODES), outs, f"held={held} page={page}")
+            check_streams([body] * 3, list(MODES), outs, f"held={held} page={page}")
             assert not any(o.flags & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG) for o in outs), held
             assert e.pool_stats()[0] == 0
         # a pooled line of exactly k pages, then only empty segments: still held, its pages still owned

@@ -20,22 +20,16 @@ import pytest
 import torch
 
 from inference_gateway_b200 import SseEngine, _abi as A, synth
-from tests.corpus import TRICKY, _plain, mutate, string_alignment_docs, template_near_misses
-from tests.util import (ConnOut, check_stream, cut_bounds, decode_shape, digest_run, fold_segment, item_class, item_sort_key,
-                        oracle_digests)
+from tests.corpus import TRICKY, mutate, string_alignment_docs, template_near_misses
+from tests.streams import dealt, filler_payload
+from tests.util import ENGINES, TARGET, cut_bounds, digest_parity, item_class, item_sort_key, one_context_at_a_time, shape_check
 
 pytestmark = pytest.mark.gpu
 R, PP = A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
-ENGINES = {"split": 0, "templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT, "fused": A.FLAG_KERNEL_FUSED,
-           "fused_templates": A.FLAG_KERNEL_FUSED | A.FLAG_TEMPLATES}
 BATCH_BYTES = 96 << 20
 MAX_CONNS = 65536
-FILLER_CONNS = 4096
 TWINS = 8
 SPARSE_ADV_BYTES = (80 << 20) // (TWINS + 1)     # the sampled adversarial bodies and their twins take at most 80 MiB
-# decoded lines per launch, in items per warp of the grid: 10 % or more inside each shape's range (8: up to 8, 16: above 8 up
-# to 16, 32: above 16)
-TARGET = {8: 6.5, 16: 12.0, 32: 20.0}
 LONG = 600                  # a payload at least this long holds a string that outlasts a lane's own skip (4 x 16 bytes)
 BUF, LT_MAX = 8192, 64      # the produce kernel's line window and lines per round (csrc/sse_common.cuh:15-16)
 
@@ -48,18 +42,8 @@ def sm_count():
 @pytest.fixture(scope="module")
 def engines():
     """engines(name): a context with that engine's flags; one context lives at a time."""
-    live = {}
-
-    def get(name):
-        if name not in live:
-            for e in live.values():
-                e.close()
-            live.clear()
-            live[name] = SseEngine(device=0, max_conns=MAX_CONNS, bytes_per_batch=BATCH_BYTES, n_slots=1, flags=ENGINES[name])
-        return live[name]
-    yield get
-    for e in live.values():
-        e.close()
+    yield from one_context_at_a_time(
+        lambda name: SseEngine(device=0, max_conns=MAX_CONNS, bytes_per_batch=BATCH_BYTES, n_slots=1, flags=ENGINES[name]))
 
 
 # ------------------------------------------------------------------ inputs
@@ -103,18 +87,6 @@ def adversarial():
     return bodies, np.array(modes, dtype=np.uint8), lines
 
 
-def filler_payload(kind: str, n: int) -> bytes:
-    """A valid chunk of about n bytes: "strings" carries them in a plain content string. "nostring" is exactly n bytes of a
-    number array under a key the decoder does not know (below 16 bytes: a number), so its lane is never inside a string."""
-    if kind == "strings":
-        head, tail = b'{"choices":[{"index":0,"delta":{"content":"', b'"},"finish_reason":null}]}'
-        return head + _plain(max(1, n - len(head) - len(tail))) + tail
-    if n < 16:
-        return b"1" * n
-    nums = (b"1234567," * (n // 8))[:n - 15]
-    return b'{"x_filler":[' + (nums[:-1] + b"8" if nums.endswith(b",") else nums) + b"]}"
-
-
 def twin(body: bytes, ents) -> bytes:
     """body with every data payload replaced by a "nostring" payload of the same length."""
     out, at = [], 0
@@ -122,23 +94,6 @@ def twin(body: bytes, ents) -> bytes:
         out += [body[at:ps], filler_payload("nostring", n)]
         at = ps + n
     return b"".join(out + [body[at:]])
-
-
-def dealt(per_batch):
-    """per_batch[b]: the payloads micro-batch b carries, dealt over FILLER_CONNS connections as "data: " events. Returns
-    (bodies, bounds, lines): batch b takes exactly connection c's share of per_batch[b]; lines as adversarial() gives them."""
-    pieces = [[pl[c::FILLER_CONNS] for c in range(FILLER_CONNS)] for pl in per_batch]
-    bodies, bounds, lines = [], [], []
-    for c in range(FILLER_CONNS):
-        at, row, ents = 0, [0], []
-        for p in pieces:
-            for pay in p[c]:
-                ents.append((at, at + 6 + len(pay), at + 6, len(pay)))
-                at += len(pay) + 8
-            row.append(at)
-        bodies.append(b"".join(b"data: " + pay + b"\n\n" for p in pieces for pay in p[c]))
-        bounds.append(row); lines.append(ents)
-    return bodies, np.array(bounds, dtype=np.int64), lines
 
 
 def decoded(lines, bounds, providers, n_batches):
@@ -217,53 +172,6 @@ def mix(shape: int, kind: str, n_batches: int, sm_count: int):
     return cb + fb, np.concatenate([np.array(cm, dtype=np.uint8), np.full(len(fb), R, dtype=np.uint8)]), bounds, providers, adv, lanes
 
 
-# ------------------------------------------------------------------ checks
-def shape_check(eng, sm_count, shape, log):
-    """on_batch hook: the launch's decoded lines must put it in `shape`, at least 10 % inside that shape's range. A record
-    is written for each decoded line and for each exact "data: [DONE]" line, which gets no work item."""
-    warps = sm_count * 32
-    lo, hi = {8: (0, 8 * warps), 16: (8 * warps, 16 * warps), 32: (16 * warps, None)}[shape]
-
-    def on_batch(b, res):
-        n_items = int(res.raw.n_recs) - int(np.count_nonzero(res.recs["flags"] & A.F_DONE_EXACT))
-        log.append(int(res.raw.n_recs))
-        if eng.cfg.flags & A.FLAG_KERNEL_FUSED:          # the tile kernel has no decode launch
-            return
-        got = decode_shape(n_items, sm_count)
-        assert got == shape, f"batch {b}: {n_items} decoded lines on {sm_count} SMs decode {got} items per warp, not {shape}"
-        assert n_items >= 1.1 * lo and (hi is None or n_items <= 0.9 * hi), \
-            f"batch {b}: {n_items} decoded lines are within 10 % of a boundary of the {shape}-item shape ({lo}, {hi}]"
-    return on_batch
-
-
-def parity(eng, bodies, modes, bounds, providers=None, on_batch=None, label=""):
-    modes = np.ascontiguousarray(np.broadcast_to(np.asarray(modes, dtype=np.uint8), (len(bodies),)))
-    od, oterm, otail = oracle_digests(bodies, modes)
-    gd, carry, flags = digest_run(eng, bodies, modes, bounds, providers=providers, on_batch=on_batch)
-    bad = np.nonzero((gd["n_frames"] != od["n_frames"]) | (gd["frame_bytes"] != od["frame_bytes"]) | (gd["frames_h"] != od["frames_h"])
-                     | (gd["n_recs"] != od["n_recs"]) | (gd["recs_h"] != od["recs_h"]))[0]
-    if bad.size:
-        _explain(eng, bodies, modes, bounds, providers, bad[:8], label)
-    assert bad.size == 0, f"{label}: {bad.size} connections differ from the oracle, first {bad[:8]}"
-    gterm = (flags & A.SEG_TERMINATED) != 0
-    assert np.array_equal(gterm, oterm.astype(bool)), label
-    assert not np.any(flags & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG)), label
-    assert np.array_equal(carry[~gterm], otail[~gterm]), label
-    return od
-
-
-def _explain(eng, bodies, modes, bounds, providers, conns, label):
-    """Runs the same batches again, keeping the output of the differing connections, and compares them field by field."""
-    outs = {int(c): ConnOut() for c in conns}
-
-    def keep(b, res):
-        for c, o in outs.items():
-            fold_segment(o, res, c)
-    digest_run(eng, bodies, modes, bounds, providers=providers, on_batch=keep)
-    for c, o in outs.items():
-        check_stream(bodies[c], int(modes[c]), o, label=f"{label} connection {c}")
-
-
 # ------------------------------------------------------------------ tests
 CASES = [(e, s, nb) for e in ENGINES for s in (8, 16, 32) for nb in (1, 3)]
 
@@ -281,10 +189,10 @@ def test_adversarial_corpus_in_each_decode_shape(engines, sm_count, engine_name,
             else:
                 assert coop > 0.9, f"sparse: only {coop:.0%} of the long-string lanes share their pull with 8 or fewer"
         log = []
-        od = parity(eng, bodies, modes, bounds, providers, shape_check(eng, sm_count, shape, log),
-                    label=f"{engine_name} {shape}-item shape {kind} x{n_batches}")
+        gd, _, _ = digest_parity(eng, bodies, modes, bounds, f"{engine_name} {shape}-item shape {kind} x{n_batches}",
+                                 providers=providers, on_batch=shape_check(eng, sm_count, shape, log))
         assert len(log) == n_batches
-        assert int(od["n_recs"][adv].sum()) > 0
+        assert int(gd["n_recs"][adv].sum()) > 0
         print(f"{engine_name} {kind} shape {shape} batches {n_batches}: {int(adv.sum())} adversarial of {len(bodies)} connections, "
               f"{len(lanes)} long-string lanes, {np.mean(lanes <= 8):.0%} of them in pulls with <= 8, n_recs per launch {log}")
 
@@ -302,7 +210,6 @@ def test_template_near_misses_after_learning(engines, sm_count, engine_name):
     mixed = [mixed[i] for i in rng.permutation(len(mixed))]
     bodies, bounds, _ = dealt([teach, mixed, teach])
     log = []
-    parity(eng, bodies, PP, bounds, on_batch=shape_check(eng, sm_count, 32, log),
-           label=f"{engine_name} near-misses")
+    digest_parity(eng, bodies, PP, bounds, f"{engine_name} near-misses", on_batch=shape_check(eng, sm_count, 32, log))
     assert len(log) == 3
     print(f"{engine_name}: {len(canon)} canonical chunks, {len(miss)} near-misses, n_recs per launch {log}")

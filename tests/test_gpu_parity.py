@@ -14,7 +14,7 @@ from inference_gateway_b200 import _abi as A
 from inference_gateway_b200 import synth
 from oracle import orc
 from tests.corpus import TRICKY, mutate as _mutate
-from tests.util import agent_results, check_stream, run_streams, telemetry_results
+from tests.util import agent_results, check_agent, check_streams, run_streams
 
 pytestmark = pytest.mark.gpu
 
@@ -24,8 +24,7 @@ GOLD = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "ref_fix
 
 def _run_and_check(engine, bodies, modes, n_batches=1, seed=0, folds=False):
     outs = run_streams(engine, bodies, modes, n_batches=n_batches, seed=seed, with_folds=folds)
-    views = [check_stream(b, m, o, label=f"stream {i} mode {m} batches {n_batches}")
-             for i, (b, m, o) in enumerate(zip(bodies, modes, outs))]
+    views = check_streams(bodies, modes, outs, f"batches {n_batches}")
     return outs, views
 
 
@@ -144,27 +143,10 @@ def test_mixed_modes_and_folds(engine):
     streams, _ = synth.make_config("C4", n_streams=300)
     bodies = [b for b, _, _ in streams]
     modes = [(R, PP, P)[i % 3] for i in range(len(bodies))]
-    outs, views = _run_and_check(engine, bodies, modes, n_batches=4, seed=3, folds=True)
-    L = engine.L
-    for i, (b, m, o, v) in enumerate(zip(bodies, modes, outs, views)):
-        if m == R:
-            content, has, term, fin, calls = agent_results(L, o.agent)
-            assert content == v.acc_content and has == v.has_tool_calls and term == v.terminated
-            assert calls == orc.parse_tool_calls(v.builder)
-            # telemetry over what the MCP path would have written (frames + final [DONE], mcp.go:253-299)
-            done = b"data: [DONE]\n\n"                                      # agent.go:140-143, written by the host
-            A.check(L.sse_telemetry_feed_bytes(o.tele, done, len(done)), "sse_telemetry_feed_bytes")
-            rc, usage, tcalls = telemetry_results(L, o.tele)
-            eusage, ecalls = orc.telemetry(b"".join(o.frames) + done)       # telemetry.go:190-277 over the body the client got
-            assert rc == 0
-            assert usage == eusage, i
-            assert tcalls == ecalls, i
-        elif m == PP:
-            rc, usage, tcalls = telemetry_results(L, o.tele)
-            eusage, ecalls = orc.telemetry(b"".join(o.frames))
-            assert rc == 0
-            assert usage == eusage, i
-            assert tcalls == ecalls, i
+    outs = run_streams(engine, bodies, modes, n_batches=4, seed=3, with_folds=True)
+    # mode R: telemetry over what the MCP path would have written (frames + the final [DONE] the host writes, mcp.go:253-299,
+    # agent.go:140-143); telemetry.go:190-277 over the body the client got
+    check_streams(bodies, modes, outs, "mixed", engine.L)
 
 
 def test_bare_done_line_does_not_stop_tool_call_parsing(engine):
@@ -180,8 +162,10 @@ def test_bare_done_line_does_not_stop_tool_call_parsing(engine):
         outs, views = _run_and_check(engine, bodies, [R] * len(bodies), n_batches=nb, seed=nb, folds=True)
         names = []
         for o, v in zip(outs, views):
-            content, has, term, fin_code, calls = agent_results(engine.L, o.agent)
-            assert calls == orc.parse_tool_calls(v.builder) and term and fin_code == 2
+            state = agent_results(engine.L, o.agent)
+            check_agent(state, v, f"bare [DONE] x{nb}")
+            content, has, term, fin_code, calls = state
+            assert term and fin_code == 2
             names.append([c["name"] for c in calls])
         # "data: [DONE] " trims to the exact line too (strings.TrimSpace first, agent.go:178)
         assert names == [[b"first", b"second"], [b"first", b"second"], [b"first"], [b"first"], [b"first", b"second"]]

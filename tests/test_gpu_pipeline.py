@@ -13,37 +13,23 @@ import pytest
 import bench
 from inference_gateway_b200 import SseEngine, _abi as A, synth
 from oracle import orc
-from tests.test_gpu_counters import check_batch
-from tests.test_gpu_defer import TINY_DECODE
-from tests.test_gpu_long_lines import PAGE, SLOT, chunk, long_line, stream_with
-from tests.util import (CHECKED, ConnOut, PipelinedDigests, check_result, check_stream, cut_bounds, digest_run,
-                        digest_run_pipelined, fill_pieces, fold_segment, oracle_digests)
+from tests.streams import PAGE, SLOT, chunk, long_line, stream_with
+from tests.util import (CHECKED, ENGINES, TINY_DECODE, ConnOut, PipelinedDigests, assert_digest_parity, check_batch, check_result,
+                        check_stream, check_streams, cut_bounds, digest_parity, digest_run, digest_run_pipelined, fill_pieces,
+                        fold_segment, one_context_at_a_time, oracle_digests, parity_faults)
 
 pytestmark = pytest.mark.gpu
 
 P, R, PP = A.MODE_P, A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
 MiB = 1 << 20
 GROW = A.OVF_TCS | A.OVF_USAGES | A.OVF_TEXT
-ENGINES = {"split": 0, "templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT, "fused": A.FLAG_KERNEL_FUSED,
-           "fused_templates": A.FLAG_KERNEL_FUSED | A.FLAG_TEMPLATES}
 
 
 @pytest.fixture(scope="module")
 def contexts():
     """contexts(key, **SseEngine arguments): the context of that key; building one closes the one before, so that one large
     context lives at a time. contexts(None) closes it."""
-    live = {}
-
-    def get(key, **kw):
-        if key not in live:
-            for e in live.values():
-                e.close()
-            live.clear()
-            if key is not None:
-                live[key] = SseEngine(device=0, **kw)
-        return live.get(key)
-    yield get
-    get(None)
+    yield from one_context_at_a_time(lambda key, **kw: SseEngine(device=0, **kw))
 
 
 @pytest.fixture(scope="module")
@@ -62,27 +48,6 @@ def populations():
 def c4_oracle(populations):
     """The oracle's digests of the whole C4 population in bench.py's mode (3: R + parse)."""
     return oracle_digests(populations("C4"), 3)
-
-
-def assert_oracle_parity(got, bodies, modes, label, oracle=None, skip=()):
-    """digest_run's (digests, carry_len, seg_flags) against the oracle's single pass over every whole body: digests, frame and
-    record counts, termination, the held-back tail. skip: connections left out (compared some other way)."""
-    gd, carry, flags = got
-    od, oterm, otail = oracle if oracle is not None else oracle_digests(bodies, modes)
-    keep = np.ones(len(bodies), dtype=bool)
-    keep[list(skip)] = False
-    assert int(gd["inexact"][keep].sum()) == 0, label
-    for key in ("n_frames", "frame_bytes", "frames_h", "n_recs", "recs_h"):
-        bad = np.nonzero((gd[key] != od[key]) & keep)[0]
-        assert bad.size == 0, (f"{label}: {bad.size} streams differ in {key}, first {bad[:5]}: gpu {gd[key][bad[:5]]} "
-                               f"oracle {od[key][bad[:5]]}")
-    gterm = (flags & A.SEG_TERMINATED) != 0
-    assert np.array_equal(gterm[keep], oterm.astype(bool)[keep]), label
-    assert not np.any(flags[keep] & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG | A.SEG_DEFERRED)), label
-    assert not np.any((flags & A.SEG_FINISHED != 0) & ~gterm), label          # only a terminated connection ignores bytes
-    live = keep & ~gterm
-    assert np.array_equal(carry[live], otail[live]), label
-    return od
 
 
 def max_batch_bytes(bounds) -> int:
@@ -110,10 +75,10 @@ def test_batches_in_flight_match_the_oracle(contexts, populations, name, n_strea
     bounds = cut_bounds(bodies, 8 if name == "C3" else 4, seed=2000 + depth)
     assert max_batch_bytes(bounds) <= eng.cfg.in_arena_bytes
     checked = CHECKED[0]
-    got = digest_run_pipelined(eng, bodies, mode, bounds, depth, order)
+    gd, _, _ = digest_parity(eng, bodies, mode, bounds, f"{name} x{n_streams} {engine} depth {depth} {order}", depth=depth,
+                             collect_order=order)
     assert CHECKED[0] - checked == bounds.shape[1] - 1
-    od = assert_oracle_parity(got, bodies, mode, f"{name} x{n_streams} {engine} depth {depth} {order}")
-    assert int(od["n_recs"].sum()) > 0
+    assert int(gd["n_recs"].sum()) > 0
 
 
 def test_fold_order_is_seen_by_the_digests(contexts, populations):
@@ -126,12 +91,11 @@ def test_fold_order_is_seen_by_the_digests(contexts, populations):
 
     def on_batch(b, res, slot):
         seen[b] = (res.segs["frame_count"] + res.segs["rec_count"]) > 0
-    gd, _, _ = digest_run_pipelined(eng, bodies, R, bounds, 4, fold_order=[0, 1, 3, 2, 4, 5, 6, 7], on_batch=on_batch)
-    od, _, _ = oracle_digests(bodies, R)
+    got = digest_run_pipelined(eng, bodies, R, bounds, 4, fold_order=[0, 1, 3, 2, 4, 5, 6, 7], on_batch=on_batch)
+    differ = parity_faults(got, oracle_digests(bodies, R)).get("digests", [])
     shared = seen[2] & seen[3]
-    differ = (gd["frames_h"] != od["frames_h"]) | (gd["recs_h"] != od["recs_h"])
     assert shared.sum() > 500
-    assert np.array_equal(differ, shared)
+    assert np.array_equal(differ, np.nonzero(shared)[0])
 
 
 # ------------------------------------------------------------------ long lines in the line pool across in-flight batches
@@ -176,10 +140,8 @@ def test_long_lines_span_batches_in_flight(contexts, engine):
     def on_batch(b, res, slot):
         for i, o in enumerate(outs):
             fold_segment(o, res, i)
-    got = digest_run_pipelined(eng, bodies, np.array(modes, dtype=np.uint8), bounds, 4, between=between, on_batch=on_batch)
-    for i, (b, m, o) in enumerate(zip(bodies, modes, outs)):
-        check_stream(b, m, o, label=f"{engine} stream {i} mode {m} line {lens[i]}")
-    assert_oracle_parity(got, bodies, np.array(modes, dtype=np.uint8), f"pool {engine}")
+    digest_parity(eng, bodies, modes, bounds, f"pool {engine}", depth=4, between=between, on_batch=on_batch)
+    check_streams(bodies, modes, outs, f"pool {engine}")
     # a line that left its carry slot is held whole in pages (tests/test_gpu_long_lines.py)
     want = sum(-(-int(bounds[i, 4] - s) // PAGE) for i, s in enumerate(starts) if bounds[i, 4] - s > SLOT)
     used, hw = held["stats"]
@@ -220,8 +182,7 @@ def _reset_run(eng, others, xs, ys, boundaries, reset_every, modes, seed, pool_c
     def on_batch(b, res, slot):
         for c in reset:
             fold_segment((outs_x if b < 3 else outs_y)[c], res, c)
-    got = digest_run_pipelined(eng, bodies, modes, bounds, 4, between=between, on_batch=on_batch)
-    assert_oracle_parity(got, bodies, modes, "connections not reset", skip=reset)
+    digest_parity(eng, bodies, modes, bounds, "connections not reset", skip=reset, depth=4, between=between, on_batch=on_batch)
     mode_of = np.broadcast_to(np.asarray(modes, dtype=np.uint8), (n,))
     for c in reset:
         # the reset drops X's unterminated tail: X's frames and records up to the piece boundary, then Y from its start
@@ -364,8 +325,7 @@ def test_deferred_regrowth_behind_later_batches(contexts, flags):
             check_batch(k, res, b"".join(p[b] for p in pieces))
             passes[b] = k["decode_passes"]
             p_lines.append(k["p_lines"])
-    got = digest_run_pipelined(eng, bodies, modes, bounds, 3, on_batch=on_batch)
-    assert_oracle_parity(got, bodies, modes, f"defer flags {flags}")
+    got = digest_parity(eng, bodies, modes, bounds, f"defer flags {flags}", depth=3, on_batch=on_batch)
     # every batch outgrew its slot, the first use of a slot and every later one (that slot had already grown)
     assert all(grew[b] for b in range(len(EVENTS_PER_BATCH))), grew
     assert all(grew[b] & A.OVF_USAGES for b in range(3, len(EVENTS_PER_BATCH))), grew
@@ -397,8 +357,7 @@ def test_steady_state_ticks_in_flight(contexts, populations, engine):
     eng = contexts(f"ticks-{engine}", max_conns=len(bodies), bytes_per_batch=max_batch_bytes(bounds), n_slots=3,
                    carry_slot_bytes=16384, flags=ENGINES[engine])
     providers = (np.arange(len(bodies)) % 4).astype(np.uint8)
-    got = digest_run_pipelined(eng, bodies, R, bounds, 3, providers=providers)
-    assert_oracle_parity(got, bodies, R, f"ticks {engine}")
+    digest_parity(eng, bodies, R, bounds, f"ticks {engine}", providers=providers, depth=3)
 
 
 # ------------------------------------------------------------------ two contexts on one device
@@ -415,7 +374,7 @@ def test_two_contexts_interleaved(contexts, populations):
         while any([r.step() for r in runs]):
             pass
         for k, r in enumerate(runs):
-            assert_oracle_parity(r.finish(), bodies, R, f"context {k}")
+            assert_digest_parity(r.finish(), bodies, R, f"context {k}")
     finally:
         for r in runs:
             r.abort()
@@ -482,7 +441,7 @@ def _fresh_parity(eng, res, segs, bodies, mode, oracle, label):
     n = len(bodies)
     d, carry, flags = orc.new_digests(n), np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint32)
     assert orc.digest_result(res.raw, np.arange(n, dtype=np.uint32), d, carry, flags) == n
-    assert_oracle_parity((d, carry, flags), bodies, mode, label, oracle=oracle)
+    assert_digest_parity((d, carry, flags), bodies, mode, label, oracle=oracle)
     return d, carry, flags
 
 
@@ -610,7 +569,7 @@ def test_bench_replay_path(contexts, populations, c4_oracle, engine, tmp_path):
             check_result(eng, res, g)
             assert orc.digest_result(res.raw, np.arange(n, dtype=np.uint32), d, carry, flags) == n
             frames += bench.delivered(res)[0]
-        assert_oracle_parity((d, carry, flags), bodies, mode, f"segmented {engine}", oracle=oracle)
+        assert_digest_parity((d, carry, flags), bodies, mode, f"segmented {engine}", oracle=oracle)
         assert frames == int(oracle[0]["n_frames"].sum())
     finally:
         torch.cuda.synchronize()

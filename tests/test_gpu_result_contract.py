@@ -7,7 +7,8 @@ import pytest
 
 from inference_gateway_b200 import SseEngine, _abi as A
 from tests.corpus import nesting_docs
-from tests.util import check_stream, digest_run, oracle_digests, run_pieces, run_streams
+from tests.streams import chunk
+from tests.util import ENGINES, check_stream, check_streams, digest_parity, run_pieces, run_streams
 
 pytestmark = pytest.mark.gpu
 
@@ -15,11 +16,7 @@ R, PP = A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
 MiB = 1 << 20
 
 
-def chunk(content: bytes, finish: bytes = b"null") -> bytes:
-    return b'data: {"choices":[{"index":0,"delta":{"content":"' + content + b'"},"finish_reason":' + finish + b"}]}\n\n"
-
-
-STOP = chunk(b"bye", b'"stop"')
+STOP = chunk(b"bye", '"stop"')
 DONE = b"data: [DONE]\n\n"
 
 
@@ -34,8 +31,7 @@ def test_nesting_limit_is_flagged_exactly(engine, mode, n_batches):
               for k in range(0, len(docs), 12)]
     modes = [mode] * len(bodies)
     outs = run_streams(engine, bodies, modes, n_batches=n_batches, seed=n_batches)
-    for i, (b, m, o) in enumerate(zip(bodies, modes, outs)):
-        check_stream(b, m, o, label=f"nesting stream {i} mode {m}")
+    check_streams(bodies, modes, outs, "nesting")
     flagged = sum(r["depth_limit"] for o in outs for r in o.recs)
     assert flagged > 300, flagged
 
@@ -51,7 +47,7 @@ def long_segment(n_lines: int, term_at: int | None, seed: int) -> bytes:
     parts = []
     for i in range(n_lines):
         if i == term_at:
-            parts.append(chunk(b"end %d" % i, b'"stop"' if i & 1 else b'"tool_calls"'))
+            parts.append(chunk(b"end %d" % i, '"stop"' if i & 1 else '"tool_calls"'))
         elif i in (62, 63, 65, 127, 128, 129, 191, 192):
             parts.append(SWALLOWED[int(rng.integers(len(SWALLOWED)))])
         elif i % 17 == 5:
@@ -73,8 +69,7 @@ def test_links_across_runs(engine, n_batches):
                 bodies.append(body)
                 modes.append(m)
     outs = run_streams(engine, bodies, modes, n_batches=n_batches, seed=7 + n_batches)
-    for i, (b, m, o) in enumerate(zip(bodies, modes, outs)):
-        check_stream(b, m, o, label=f"runs stream {i} mode {m}")
+    check_streams(bodies, modes, outs, "runs")
     assert sum(o.terminated for o in outs) == 4 * 6
 
 
@@ -82,7 +77,7 @@ def test_terminating_chunk_completed_from_the_carry_slot(engine):
     """The terminating chunk is a line the batch completes from the connection's carry slot: its head came in the previous
     batch, cut at every kind of place (inside "data: ", inside the payload, before the '\\n', before the blank line)."""
     head = long_segment(70, None, 3)
-    stop = chunk(b"the end " * 300, b'"stop"')
+    stop = chunk(b"the end " * 300, '"stop"')
     body = head + stop + chunk(b"never read") + DONE
     cuts = [1, 3, 6, 7, 100, len(stop) - 3, len(stop) - 2, len(stop) - 1]
     pieces = [[body[:len(head) + c], body[len(head) + c:]] for c in cuts]
@@ -96,8 +91,7 @@ def test_terminating_chunk_completed_from_the_carry_slot(engine):
 @pytest.fixture(scope="module", params=["split", "templates", "copy"])
 def pooled(request):
     e = SseEngine(device=0, max_conns=64, bytes_per_batch=8 * MiB, carry_slot_bytes=32768, n_slots=2, text_arena_bytes=16 * MiB,
-                  flags={"split": 0, "templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT}[request.param],
-                  line_pool=dict(pool_pages=64, page_bytes=65536))
+                  flags=ENGINES[request.param], line_pool=dict(pool_pages=64, page_bytes=65536))
     yield e
     e.close()
 
@@ -105,7 +99,7 @@ def pooled(request):
 def test_terminating_chunk_completed_from_the_line_pool(pooled):
     """The terminating chunk is a 200 KB line assembled in line-pool pages over several batches, after 70 lines (two runs)."""
     head = long_segment(70, None, 5)
-    stop = chunk(b"0123456789abcdef" * 12800, b'"tool_calls"')
+    stop = chunk(b"0123456789abcdef" * 12800, '"tool_calls"')
     body = head + stop + chunk(b"never read") + DONE
     a = len(head)
     pieces = [[body[:a + 10], body[a + 10:a + 40000], body[a + 40000:a + 150000], body[a + 150000:]],
@@ -130,9 +124,4 @@ def test_identical_connections_are_not_cross_wired(engine, mode):
     bodies = [body] * n
     row = np.array([0, 17, 1300, 2600, 3900, 5200, len(body)], dtype=np.int64)
     bounds = np.tile(row, (n, 1))
-    gd, carry, flags = digest_run(engine, bodies, mode, bounds)
-    od, term, tail = oracle_digests(bodies, mode)
-    for k in ("frames_h", "recs_h", "n_frames", "n_recs", "frame_bytes"):
-        assert np.array_equal(gd[k], od[k]), k
-    assert int(gd["inexact"].sum()) == 0 and not np.any(flags & A.SEG_DEAD)
-    assert np.array_equal((flags & A.SEG_TERMINATED) != 0, term.astype(bool))
+    digest_parity(engine, bodies, mode, bounds, f"identical connections mode {mode}")

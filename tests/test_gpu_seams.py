@@ -10,14 +10,12 @@ from inference_gateway_b200 import SseEngine, _abi as A
 from inference_gateway_b200.synth import random_cuts
 from oracle import orc
 from tests import seams as S
-from tests.util import ConnOut, check_stream, cut_bounds, digest_run, fold_segment, oracle_digests, run_pieces
+from tests.util import ENGINES, check_stream, cut_bounds, digest_parity, line_limit, oracle_digests, run_pieces
 
 pytestmark = pytest.mark.gpu
 
 P, R, PP = A.MODE_P, A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
 MODES = (P, R, PP)
-FLAGS = {"split": 0, "templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT, "fused": A.FLAG_KERNEL_FUSED,
-         "fused_templates": A.FLAG_KERNEL_FUSED | A.FLAG_TEMPLATES}
 PRODUCE = ("split", "templates", "copy")
 TILED = ("fused", "fused_templates")
 SLOT = 32768
@@ -32,7 +30,7 @@ def engines():
     def get(name):
         if name not in made:
             made[name] = SseEngine(device=0, max_conns=MAX_CONNS, bytes_per_batch=64 << 20, carry_slot_bytes=SLOT, n_slots=2,
-                                   flags=FLAGS[name])
+                                   flags=ENGINES[name])
         return made[name]
     yield get
     for e in made.values():
@@ -56,30 +54,6 @@ def _groups(bodies):
         i = j
 
 
-def parity(eng, bodies, mode, bounds, label, ref=None):
-    """digest_run against the oracle's digests (ref: oracle_digests already computed); the first differing connections are run
-    again and compared field by field."""
-    modes = np.full(len(bodies), mode, dtype=np.uint8)
-    od, oterm, otail = ref if ref is not None else oracle_digests(bodies, modes)
-    gd, carry, flags = digest_run(eng, bodies, modes, bounds)
-    bad = np.nonzero((gd["n_frames"] != od["n_frames"]) | (gd["frame_bytes"] != od["frame_bytes"]) | (gd["frames_h"] != od["frames_h"])
-                     | (gd["n_recs"] != od["n_recs"]) | (gd["recs_h"] != od["recs_h"]))[0]
-    if bad.size:
-        outs = {int(c): ConnOut() for c in bad[:4]}
-
-        def keep(b, res):
-            for c, o in outs.items():
-                fold_segment(o, res, c)
-        digest_run(eng, bodies, modes, bounds, on_batch=keep)
-        for c, o in outs.items():
-            check_stream(bodies[c], mode, o, label=f"{label} connection {c}")
-    assert bad.size == 0, f"{label}: {bad.size} connections differ from the oracle, first {bad[:8]}"
-    gterm = (flags & A.SEG_TERMINATED) != 0
-    assert np.array_equal(gterm, oterm.astype(bool)), label
-    assert not np.any(flags & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG)), label
-    assert np.array_equal(carry[~gterm], otail[~gterm]), label
-
-
 def bulk(eng, cases, label, modes=MODES, seed=0):
     """Every case in one batch, in its explicit pieces (when it has any) and in four seeded pieces, in every mode."""
     for i, j in _groups([c.body for c in cases]):
@@ -89,9 +63,9 @@ def bulk(eng, cases, label, modes=MODES, seed=0):
         if any(c.cuts for c in part):
             runs.append(("explicit pieces", _bounds(part)))
         for m in modes:
-            ref = oracle_digests(bodies, np.full(len(bodies), m, dtype=np.uint8))
+            ref = oracle_digests(bodies, m)
             for name, b in runs:
-                parity(eng, bodies, m, b, f"{label} [{i}:{j}] mode {m} {name}", ref)
+                digest_parity(eng, bodies, m, b, f"{label} [{i}:{j}] mode {m} {name}", oracle=ref)
 
 
 def focused(eng, cases, label, modes=MODES, seed=0, alone=False):
@@ -173,9 +147,9 @@ def _batch_parity(eng, bt, label):
     if bt.first_cut is not None:
         runs.append(("explicit", np.array([[0, c, len(b)] for b, c in zip(bodies, bt.first_cut)], dtype=np.int64)))
     for m in MODES:
-        ref = oracle_digests(bodies, np.full(len(bodies), m, dtype=np.uint8))
+        ref = oracle_digests(bodies, m)
         for name, b in runs:
-            parity(eng, bodies, m, b, f"{label} {bt.meta} mode {m} {name}", ref)
+            digest_parity(eng, bodies, m, b, f"{label} {bt.meta} mode {m} {name}", oracle=ref)
 
 
 @pytest.mark.parametrize("name", TILED + PRODUCE)
@@ -289,7 +263,7 @@ def test_template_store_fills(name):
     wins = S.tile_windows(b"", body)
     assert sum(w[0] for w in words) > room
     assert len(wins) * S.NREC * min(w[0] for w in words) > room and all(len(w.lines) <= S.LCAP for w in wins)
-    eng = SseEngine(device=0, max_conns=16, bytes_per_batch=4 << 20, carry_slot_bytes=SLOT, n_slots=2, flags=FLAGS[name])
+    eng = SseEngine(device=0, max_conns=16, bytes_per_batch=4 << 20, carry_slot_bytes=SLOT, n_slots=2, flags=ENGINES[name])
     try:
         rng = np.random.default_rng(3)
         for m in MODES:
@@ -306,11 +280,10 @@ NEIGHBOURS = [S.chunk(b"left") * 3 + S.END, S.data_line(5000) + S.END]
 
 
 @pytest.mark.parametrize("slot", [16384, 32768])
-@pytest.mark.parametrize("name", list(FLAGS))
+@pytest.mark.parametrize("name", list(ENGINES))
 def test_line_length_limit(name, slot):
-    eng = SseEngine(device=0, max_conns=64, bytes_per_batch=4 << 20, carry_slot_bytes=slot, n_slots=2, flags=FLAGS[name])
+    eng = SseEngine(device=0, max_conns=64, bytes_per_batch=4 << 20, carry_slot_bytes=slot, n_slots=2, flags=ENGINES[name])
     try:
-        from tests.util import line_limit
         limit = line_limit(eng)
         assert limit == slot
         cases = S.limit_cases(limit)

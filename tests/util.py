@@ -4,12 +4,31 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 from unittest import mock
 
 import numpy as np
 
 from inference_gateway_b200 import _abi as A
 from oracle import orc
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = open(os.path.join(ROOT, "include", "sse_gpu.h")).read()
+GW_HEADER = open(os.path.join(ROOT, "include", "sse_gateway.h")).read()
+
+# the engine variants, by the names of the `engine` fixture (tests/conftest.py): split = produce / sort / decode / finalize
+# pipeline, templates = the same with SSE_FLAG_TEMPLATES, copy = SSE_FLAG_COPY_OUT, fused = the single-pass tile kernel
+ENGINES = {"split": 0, "templates": A.FLAG_TEMPLATES, "copy": A.FLAG_COPY_OUT, "fused": A.FLAG_KERNEL_FUSED,
+           "fused_templates": A.FLAG_KERNEL_FUSED | A.FLAG_TEMPLATES}
+# capacities far below what a batch of many streams needs: the produce side's still hold one round (64 lines) of one segment
+TINY_PRODUCE = dict(max_frames=128, max_recs=64, out_arena_bytes=32 * 1024, max_runs=16)
+TINY_DECODE = dict(max_tcs=8, max_usages=4, text_arena_bytes=512)
+
+
+def declared_functions(text=None, prefix="sse_"):
+    """The functions a C header (default include/sse_gpu.h) declares whose names start with prefix."""
+    body = re.sub(r"/\*.*?\*/", "", text or HEADER, flags=re.S)
+    return sorted(set(re.findall(r"\b(%s[a-z_0-9]+)\s*\(" % prefix, body)))
 
 
 class ConnOut:
@@ -87,6 +106,23 @@ def fold_segment(o: ConnOut, res, i: int):
 
 # ------------------------------------------------------------------ structural check of every batch result
 CHECKED = [0]     # batch results orc_check_result has passed in this process
+
+
+def one_context_at_a_time(make):
+    """Body of a module fixture: yields get(key, **kw), the context make(key, **kw) built for key. Building one closes the one
+    before, so that one large context lives at a time; get(None) closes it."""
+    live = {}
+
+    def get(key, **kw):
+        if key not in live:
+            for e in live.values():
+                e.close()
+            live.clear()
+            if key is not None:
+                live[key] = make(key, **kw)
+        return live.get(key)
+    yield get
+    get(None)
 
 
 def line_limit(eng) -> int:
@@ -350,6 +386,94 @@ def oracle_digests(bodies, modes):
     return orc.digest_streams(arena, offs, lens, modes, max(1, len(os.sched_getaffinity(0))))
 
 
+# ------------------------------------------------------------------ the digest verdict
+DIGEST_FIELDS = ("n_frames", "frame_bytes", "frames_h", "n_recs", "recs_h")
+RULES = {
+    "digests": "frames or records differ from the oracle's",
+    "inexact": "records left undecoded (SSE_F_TOO_LONG) or with a broken tool-call chain",
+    "termination": "termination differs from the oracle's",
+    "seg_flags": "SSE_SEG_DEAD, SSE_SEG_LINE_TOO_LONG or SSE_SEG_DEFERRED set",
+    "finished": "SSE_SEG_FINISHED on a connection that did not terminate",
+    "carry": "the carried tail of a live connection differs from the oracle's",
+}
+
+
+def parity_faults(got, oracle, skip=()) -> dict:
+    """The rules of RULES that a run's (digests, carry_len, seg_flags) breaks against the oracle's (digests, terminated,
+    tail_len): {rule: the connections that break it}, empty when the run is the oracle's. skip: connections left out."""
+    gd, carry, flags = got
+    od, oterm, otail = oracle
+    keep = np.ones(len(gd), dtype=bool)
+    keep[list(skip)] = False
+    gterm = (flags & A.SEG_TERMINATED) != 0
+    broken = {
+        "digests": np.any([gd[k] != od[k] for k in DIGEST_FIELDS], axis=0),
+        "inexact": gd["inexact"] != 0,
+        "termination": gterm != oterm.astype(bool),
+        "seg_flags": (flags & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG | A.SEG_DEFERRED)) != 0,
+        "finished": ((flags & A.SEG_FINISHED) != 0) & ~gterm,
+        "carry": ~gterm & (carry != otail),
+    }
+    return {rule: np.nonzero(bad & keep)[0] for rule, bad in broken.items() if np.any(bad & keep)}
+
+
+def parity_message(label, faults, got, oracle) -> str:
+    """Each broken rule with its first connections, and what the run and the oracle hold for the first of them."""
+    gd, carry, flags = got
+    od, oterm, otail = oracle
+    out = [f"{label}: the run differs from the oracle"]
+    for rule, conns in faults.items():
+        c = conns[0]
+        out += [f"  {RULES[rule]}: {conns.size} connection(s), first {conns[:8].tolist()}",
+                f"    connection {c}: gpu {DIGEST_FIELDS} {gd[list(DIGEST_FIELDS)][c]} inexact {gd['inexact'][c]} seg_flags "
+                f"{int(flags[c]):#x} carry {carry[c]}; oracle {od[list(DIGEST_FIELDS)][c]} terminated {bool(oterm[c])} tail {otail[c]}"]
+    return "\n".join(out)
+
+
+def assert_digest_parity(got, bodies, modes, label, *, oracle=None, skip=()):
+    """The digest verdict: got, a run's (digests, carry_len, seg_flags), breaks no rule of RULES against the oracle's single
+    pass over every whole body (oracle: oracle_digests(bodies, modes) when already computed) on any connection but those in
+    skip. Returns the oracle's digests."""
+    oracle = oracle if oracle is not None else oracle_digests(bodies, modes)
+    faults = parity_faults(got, oracle, skip)
+    assert not faults, parity_message(label, faults, got, oracle)
+    return oracle[0]
+
+
+def digest_parity(eng, bodies, modes, bounds, label, *, providers=None, on_batch=None, oracle=None, skip=(), depth=1,
+                  **pipelined):
+    """Feeds the bodies in the pieces bounds gives (digest_run, or digest_run_pipelined with depth batches in flight and its
+    other arguments) and applies assert_digest_parity. When a rule is broken, the same engine runs the same batches again
+    and the first connections that break one are compared field by field (check_stream); if they compare equal, the digest
+    message is the failure. Returns the run's (digests, carry_len, seg_flags)."""
+    modes = np.ascontiguousarray(np.broadcast_to(np.asarray(modes, dtype=np.uint8), (len(bodies),)))
+    oracle = oracle if oracle is not None else oracle_digests(bodies, modes)
+
+    def run(hook):
+        if depth == 1 and not pipelined:
+            return digest_run(eng, bodies, modes, bounds, providers, hook)
+        return digest_run_pipelined(eng, bodies, modes, bounds, depth, providers=providers, on_batch=hook, **pipelined)
+    got = run(on_batch)
+    faults = parity_faults(got, oracle, skip)
+    if faults:
+        outs = {int(c): ConnOut() for c in np.unique(np.concatenate(list(faults.values())))[:4]}
+
+        def keep(b, res, *slot):
+            for c, o in outs.items():
+                fold_segment(o, res, c)
+        run(keep)
+        for c, o in outs.items():
+            check_stream(bodies[c], int(modes[c]), o, label=f"{label} connection {c}")
+    assert not faults, parity_message(label, faults, got, oracle)
+    return got
+
+
+# ------------------------------------------------------------------ decode launch shapes
+# decoded lines per launch, in items per warp of the grid: 10 % or more inside each shape's range (8: up to 8, 16: above 8 up
+# to 16, 32: above 16)
+TARGET = {8: 6.5, 16: 12.0, 32: 20.0}
+
+
 def decode_shape(n_items: int, sm_count: int) -> int:
     """Work items a warp of sse_decode_kernel pulls at a time for a batch of n_items decoded lines (csrc/sse_kernel2.cu:823-832).
     The kernel runs one CTA of 32 warps per SM. A batch with fewer items than 32 per warp spreads them over every warp, 8 or 16
@@ -360,6 +484,24 @@ def decode_shape(n_items: int, sm_count: int) -> int:
         return 32
     per = -(-n_items // warps)
     return 8 if per <= 8 else (16 if per <= 16 else 32)
+
+
+def shape_check(eng, sm_count, shape, log):
+    """digest_run hook: the launch's decoded lines must put it in `shape`, at least 10 % inside that shape's range. A record
+    is written for each decoded line and for each exact "data: [DONE]" line, which gets no work item."""
+    warps = sm_count * 32
+    lo, hi = {8: (0, 8 * warps), 16: (8 * warps, 16 * warps), 32: (16 * warps, None)}[shape]
+
+    def on_batch(b, res):
+        n_items = int(res.raw.n_recs) - int(np.count_nonzero(res.recs["flags"] & A.F_DONE_EXACT))
+        log.append(int(res.raw.n_recs))
+        if eng.cfg.flags & A.FLAG_KERNEL_FUSED:          # the tile kernel has no decode launch
+            return
+        got = decode_shape(n_items, sm_count)
+        assert got == shape, f"batch {b}: {n_items} decoded lines on {sm_count} SMs decode {got} items per warp, not {shape}"
+        assert n_items >= 1.1 * lo and (hi is None or n_items <= 0.9 * hi), \
+            f"batch {b}: {n_items} decoded lines are within 10 % of a boundary of the {shape}-item shape ({lo}, {hi}]"
+    return on_batch
 
 
 def item_class(rel: int, provider: int) -> int:
@@ -446,3 +588,94 @@ def check_stream(body: bytes, mode: int, o: ConnOut, label=""):
     if not o.terminated and not (o.flags & A.SEG_DEAD):
         assert o.carry_len == v.tail_len, f"{label}: carry {o.carry_len} != tail {v.tail_len}"
     return v
+
+
+def check_streams(bodies, modes, outs, label="", L=None):
+    """check_stream on every connection (modes: one for all or one per body) and, given the library L, check_folds on every
+    connection that has folds. Returns the oracle's views."""
+    modes = np.broadcast_to(np.asarray(modes), (len(bodies),))
+    views = [check_stream(b, int(m), o, label=f"{label} stream {i} mode {m}") for i, (b, m, o) in enumerate(zip(bodies, modes, outs))]
+    for i, (m, o, v) in enumerate(zip(modes, outs, views)):
+        if L is not None and o.agent is not None:
+            check_folds(L, o, int(m), v, f"{label} stream {i} mode {m}")
+    return views
+
+
+# ------------------------------------------------------------------ the fold verdict
+DONE = b"data: [DONE]\n\n"
+
+
+def check_agent(state, v, label=""):
+    """An agent fold's (content, has_tool_calls, terminated, finish, tool calls), as agent_results or Gateway.agent_state
+    gives them, against the oracle's reframe of the same body (v, as check_stream returns it in mode R)."""
+    content, has, term, fin, calls = state
+    assert content == v.acc_content, f"{label}: agent content differs from the oracle's"
+    assert (has, term) == (v.has_tool_calls, v.terminated), \
+        f"{label}: has_tool_calls, terminated {(has, term)}, oracle {(v.has_tool_calls, v.terminated)}"
+    assert not term or fin == v.term_finish, f"{label}: finish {fin}, oracle {v.term_finish}"
+    assert calls == orc.parse_tool_calls(v.builder), f"{label}: tool calls differ from the oracle's"
+
+
+def check_folds(L, o: ConnOut, mode: int, v, label=""):
+    """The agent and telemetry folds run_streams(with_folds=True) fed for one connection, against the oracle (v: what
+    check_stream returned). Mode R: the agent fold (check_agent), and the telemetry over the frames and the [DONE] the agent
+    writes at the end; mode P|PARSE: the telemetry over the frames. Returns the agent fold's state (None outside mode R)."""
+    state = None
+    if mode & A.MODE_R:
+        state = agent_results(L, o.agent)
+        check_agent(state, v, label)
+        A.check(L.sse_telemetry_feed_bytes(o.tele, DONE, len(DONE)), "sse_telemetry_feed_bytes")
+        assert telemetry_results(L, o.tele) == (0, *orc.telemetry(b"".join(o.frames) + DONE)), f"{label}: telemetry differs"
+    elif mode & A.MODE_PARSE:
+        assert telemetry_results(L, o.tele) == (0, *orc.telemetry(b"".join(o.frames))), f"{label}: telemetry differs"
+    return state
+
+
+# ------------------------------------------------------------------ SSE_FLAG_COUNTERS
+CYCLES = ("c_pull", "c_skip", "c_coop", "c_steps", "c_finish", "c_unquote")
+
+
+def text_spans(res):
+    """(spans flagged SSE_F_CONTENT_TEXT or SSE_TC_*_TEXT, records with at least one, whether any tool-call element has two)"""
+    recs, tcs = res.recs, res.tcs
+    content = (recs["flags"] & A.F_CONTENT_TEXT) != 0
+    per_tc = np.array([bin(int(f) & 0xF0).count("1") for f in tcs["flags"]], dtype=np.int64)
+    with_text = content.copy()
+    for i in np.nonzero(~content)[0]:
+        t = int(recs["tc_first"][i])
+        while t != A.NONE and t < len(tcs) and not with_text[i]:
+            with_text[i] = per_tc[t] > 0
+            t = int(tcs["next"][t])
+    return int(content.sum() + per_tc.sum()), int(with_text.sum()), bool((per_tc > 1).any())
+
+
+def check_batch(k, res, submitted=None, one_job_per_span=True):
+    """The identities the counters k of every batch result res satisfy. submitted: the batch's input bytes (their '\\n' are the
+    complete lines when no segment stopped early)."""
+    raw = res.raw
+    assert k["decode_passes"] == (1 if raw.n_segs else 0) or k["decode_passes"] > 1, k
+    assert k["p_segments"] == raw.n_segs, (k, raw.n_segs)
+    assert k["p_items"] == raw.n_decoded, (k, raw.n_decoded)
+    assert k["p_frames_zero_copy"] + k["p_frames_materialised"] == raw.n_frames, (k, raw.n_frames)
+    mat = res.frames["off"] < res.in_base
+    assert k["p_bytes_materialised"] == int(res.frames["len"][mat].sum()), (k, int(res.frames["len"][mat].sum()))
+    if submitted is not None:
+        nl = submitted.count(b"\n")
+        stopped = int(np.count_nonzero(res.segs["flags"] & (A.SEG_TERMINATED | A.SEG_FINISHED | A.SEG_DEAD | A.SEG_DEFERRED)))
+        assert k["p_lines"] == nl if not stopped else k["p_lines"] <= nl, (k, nl, stopped)
+    decoded = (res.recs["flags"] & A.F_DONE_EXACT) == 0          # an exact "data: [DONE]" gets a record but no work item
+    moved = (k["d_skip_bytes"] + k["d_coop_bytes"] + k["d_plain_steps"] + k["d_actions"] + k["d_abandoned_bytes"]
+             + k["d_template_bytes"])
+    assert moved == int(res.recs["payload_len"][decoded].sum()), k
+    assert k["d_items"] == k["d_lines_finished"] == raw.n_decoded, (k, raw.n_decoded)
+    assert k["d_busy_lane_rounds"] <= 32 * k["d_warp_rounds"], k
+    assert sum(k[c] for c in CYCLES) <= k["c_total"], k
+    if raw.n_decoded:
+        assert k["d_items_per_pull"] in (8, 16, 32) and k["d_pulls"] > 0, k
+    # every unquote job yields one text span. A lane queues one job at a time (the warp drains the queues every two rounds), so
+    # a line's first string to unquote is always a job, and a tool-call element with two such strings, or a line replayed
+    # from a template (all its captures at once), unquotes the rest on its lane
+    spans, lines, two = text_spans(res)
+    assert lines <= k["d_unquote_jobs"] <= spans, (k, lines, spans)
+    if one_job_per_span and not two:
+        assert k["d_unquote_jobs"] == spans, (k, spans)
