@@ -371,6 +371,9 @@ int  sse_telemetry_feed(sse_telemetry_fold *f, const sse_result *res, uint32_t s
  * They are part of the body telemetry.go:190-198 splits into pieces, so they move its last-4-pieces window; they are not decoded
  * (feed only frames that hold no chunk: "[DONE]", comments, error text). n must end on a '\n'. */
 int  sse_telemetry_feed_bytes(sse_telemetry_fold *f, const uint8_t *bytes, size_t n);
+/* The usage and the tool calls (at most cap written to calls; *n_calls is how many there are). Returns 1 when a piece was irregular
+ * (DESIGN.md section 5, deviation 4), else SSE_OK. It closes the body's last piece once: called again, e.g. with a larger array,
+ * it gives the same answer. Feed nothing after it. */
 int  sse_telemetry_finish(sse_telemetry_fold *f, sse_usage *usage, sse_tool_call *calls, size_t cap, size_t *n_calls);
 
 #ifdef __cplusplus

@@ -596,7 +596,8 @@ __device__ __noinline__ void append_run(const KParams &P, RunChain &rc, uint32_t
 // fit may leave its counters past a capacity (sse_download clamps them) and holes below it. Out bytes, frames and records in a hole
 // are never referenced by a run. Work items are read by the sort and decode stages whatever references them, so every work item a
 // deferred allocation got below cap_items becomes an empty item that decodes into the sink record recs[cap_recs], which is
-// allocated past the capacity and never returned.
+// allocated past the capacity and never returned. So does every work item of an allocation that overflowed without the flag:
+// the batch fails, but its decode stage still runs over the items below cap_items.
 
 __device__ __noinline__ void empty_items(const KParams &P, uint32_t qb, uint32_t n) {
     const uint32_t e = min(qb + n, P.cap_items);
@@ -697,7 +698,11 @@ __device__ __noinline__ bool process_long_line(const KParams &P, RunChain &rc, c
         ob = __shfl_sync(FULL, ob, 0); fb = __shfl_sync(FULL, fb, 0); rb = __shfl_sync(FULL, rb, 0); qb = __shfl_sync(FULL, qb, 0);
         bool ovf = (!in_place && (nf || extra) && (ob + (uint32_t)flen + extra + 16u > P.cap_out)) || (nf && fb >= P.cap_frames) ||
                    (nr && rb >= P.cap_recs) || (item && qb >= P.cap_items);
-        if (ovf) { if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT); return false; }
+        if (ovf) {
+            if (item) empty_items(P, qb, 1u);      // the sort and decode stages read it all the same: it decodes into the sink
+            if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT);
+            return false;
+        }
     }
     // frame and payload offsets in the out arena
     const uint32_t fo = in_place ? at + (uint32_t)((mode & SSE_MODE_R) ? a : 0) : ob;

@@ -39,6 +39,13 @@ inline sse_bytes span(const sse_result *r, uint32_t off, uint32_t len, bool text
     return b;
 }
 
+// The tool-call elements of a record, in order. tc_count saturates at 0xFFFF: a saturated chain is walked to its end.
+template <class F> void for_each_tc(const sse_result *res, const sse_rec &r, F f) {
+    const uint32_t want = r.tc_count < 0xFFFFu ? r.tc_count : 0xFFFFFFFFu;
+    uint32_t t = r.tc_first;
+    for (uint32_t k = 0; k < want && t != SSE_NONE; k++) { f(res->tcs[t]); t = res->tcs[t].next; }
+}
+
 template <class F> void for_each_run(const sse_result *res, uint32_t seg, F f) {
     const sse_run *run = &res->segs[seg].run;
     for (;;) {
@@ -91,6 +98,7 @@ struct sse_telemetry_fold {
     std::vector<uint32_t> cur_tc_flags;
     uint32_t nl_run = 0;
     uint64_t irregular = 0;      // multi-line pieces that start with "data: " (not decodable from per-line records)
+    bool finished = false;       // sse_telemetry_finish closed the last piece
     AccMap calls;
     std::vector<Acc> store;
 };
@@ -129,9 +137,7 @@ void tele_take_rec(sse_telemetry_fold *f, const sse_result *res, const sse_rec &
     if (r.flags & SSE_F_HAS_USAGE) { f->cur_has_usage = true; f->cur_usage = res->usages[r.usage]; }
     if (r.n_choices > 0 && (r.flags & SSE_F_TC_NONNIL)) {
         f->cur_tc = true;
-        uint32_t t = r.tc_first;
-        for (uint32_t k = 0; k < r.tc_count && t != SSE_NONE; k++) {
-            const sse_tc &tc = res->tcs[t];
+        for_each_tc(res, r, [&](const sse_tc &tc) {
             Acc a;
             a.index = tc.index;
             sse_bytes id = span(res, tc.id_off, tc.id_len, tc.flags & SSE_TC_ID_TEXT);
@@ -139,8 +145,7 @@ void tele_take_rec(sse_telemetry_fold *f, const sse_result *res, const sse_rec &
             sse_bytes ar = span(res, tc.args_off, tc.args_len, tc.flags & SSE_TC_ARGS_TEXT);
             a.id.assign((const char *)id.p, id.n); a.name.assign((const char *)nm.p, nm.n); a.args.assign((const char *)ar.p, ar.n);
             f->cur_tcs.push_back(a); f->cur_tc_flags.push_back(tc.flags);
-            t = tc.next;
-        }
+        });
     }
 }
 
@@ -192,8 +197,7 @@ int sse_agent_feed(sse_agent_fold *f, const sse_result *res, uint32_t seg) {
             if (r.flags & SSE_F_DONE_EXACT) { f->done_break = true; continue; }   // :394-396
             if (!ok || r.n_choices == 0 || !(r.flags & SSE_F_TC_NONNIL)) continue; // :398-406
             std::vector<const sse_tc *> els;
-            uint32_t t = r.tc_first;
-            for (uint32_t k = 0; k < r.tc_count && t != SSE_NONE; k++) { els.push_back(&res->tcs[t]); t = res->tcs[t].next; }
+            for_each_tc(res, r, [&](const sse_tc &tc) { els.push_back(&tc); });
             for (const sse_tc *tc : els) {
                 Acc &a = f->calls.get(tc->index);                                  // :409-421
                 if (tc->flags & SSE_TC_HAS_ID) {                                   // :424-426
@@ -269,9 +273,9 @@ int sse_telemetry_feed_bytes(sse_telemetry_fold *f, const uint8_t *bytes, size_t
 
 int sse_telemetry_finish(sse_telemetry_fold *f, sse_usage *usage, sse_tool_call *calls, size_t cap, size_t *n_calls) {
     if (!f || !usage) return SSE_ERR_ARG;
-    // strings.Split always yields a final piece (possibly empty, possibly "X\n")
-    tele_close_piece(f);
-    f->nl_run = 0;
+    // strings.Split always yields a final piece (possibly empty, possibly "X\n"); closed once, so that a second call (with a
+    // larger array) gives the same answer
+    if (!f->finished) { tele_close_piece(f); f->nl_run = 0; f->finished = true; }
     usage->prompt_tokens = usage->completion_tokens = usage->total_tokens = 0;
     uint64_t n = f->n_pieces, first = n > 4 ? n - 4 : 0;                  // telemetry.go:195-198
     for (uint64_t k = first; k < n; k++) {

@@ -447,6 +447,14 @@ __device__ __noinline__ void f_cancel_job(FSmem &S, uint32_t *patch) {
     for (uint32_t i = 0; i < n; i++) if (S.jq[i].patch == patch) S.jq[i].patch = nullptr;
 }
 
+// choices[0] starts anew: "choices":null, and the close of an empty "choices" array (decode.go array() sets a fresh slice of
+// capacity 0, so a later "choices" array grows new, zeroed storage)
+__device__ __forceinline__ void f_choices_reset(FLane &L) {
+    L.n_choices = 0; L.choices_count = 0; L.finish = SSE_FIN_NONE; L.content_pos = L.content_len = 0;
+    L.sf &= ~(SF_CDEC | SF_CBAD | SF_CSET);
+    f_drop_tcs(L);
+}
+
 __device__ __forceinline__ void f_null(const KParams &P, FSmem &S, FLane &L) {
     const uint32_t ty = L.cur & 15u, tgt = (L.cur >> 9) & 15u;
     if (ty == TY_TS) { L.sf &= ~SF_GBAD; return; }
@@ -455,11 +463,7 @@ __device__ __forceinline__ void f_null(const KParams &P, FSmem &S, FLane &L) {
     const bool tco = (L.sf & SF_TCOPEN) && fl_live(L) && L.tc_cur != SSE_NONE;
     if (tgt != TG_USAGE || (L.sf & SF_USAGE)) rec_nonsimple(S, L);     // a reset is not something a template replays
     switch (tgt) {
-    case TG_CHOICES:
-        L.n_choices = 0; L.choices_count = 0; L.finish = SSE_FIN_NONE; L.content_pos = L.content_len = 0;
-        L.sf &= ~(SF_CDEC | SF_CBAD | SF_CSET);
-        f_drop_tcs(L);
-        break;
+    case TG_CHOICES: f_choices_reset(L); break;
     case TG_USAGE: L.sf &= ~SF_USAGE; break;     // the line keeps its sse_usage slot: a later "usage":{} zeroes and reuses it
     case TG_TOOLCALLS: if (fl_live(L)) f_drop_tcs(L); break;
     case TG_TC_ID:
@@ -605,7 +609,7 @@ __device__ __forceinline__ void f_close(const KParams &P, FLane &L) {
     else {
         const uint32_t node = fl_top(L);
         L.sd--;
-        if (node == A_CHOICES) L.n_choices = L.choices_count;
+        if (node == A_CHOICES) { if (L.choices_count) L.n_choices = L.choices_count; else f_choices_reset(L); }
         else if (node == A_TOOLCALLS) { if (fl_live(L) && (L.sf & SF_TCOPEN)) f_flush_tc(P, L); }
         else if (node == N_GOOGLE) { if (L.sf & SF_GBAD) L.sf |= SF_TYPE; }
     }

@@ -309,6 +309,9 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                 if constexpr (CNT) T.add(CN_P_ROUNDS, 1);
                 if (!DEFER) {
                     if (ob + tot_b + 16 > P.cap_out || fb + tot_f > P.cap_frames || rb + tot_r > P.cap_recs || qb + tot_q > P.cap_items) {
+                        // the sort and decode stages still read every work item below cap_items: the round's decode into the sink
+                        // record instead of whatever an earlier batch left in the slot
+                        empty_items(P, qb, tot_q);
                         if (lane == 0) sse_overflow(P.ctr, SSE_OVF_OUT);
                         overflow = true; break;
                     }

@@ -196,6 +196,14 @@ __device__ void v2_elem_begin(const KParams &P, Lane &L, LaneScratch &S, Q *J) {
     else L.cur = TY_INT;
 }
 
+// choices[0] starts anew: "choices":null, and the close of an empty "choices" array (decode.go array() sets a fresh slice of
+// capacity 0, so a later "choices" array grows new, zeroed storage)
+__device__ __forceinline__ void v2_choices_reset(Lane &L) {
+    L.n_choices = 0; L.choices_count = 0; L.finish = SSE_FIN_NONE; L.content_off = L.content_len = 0;
+    L.sf &= ~(SF_CDEC | SF_CBAD | SF_CSET | SF_TCNONNIL | SF_TCOPEN | SF_TCVALID);
+    L.tc_count = 0; L.tc_first = SSE_NONE;
+}
+
 template <bool REC>
 __device__ void v2_null(Lane &L, LaneScratch &S) {
     uint32_t ty = L.cur & 15u, tgt = (L.cur >> 9) & 15u;
@@ -203,11 +211,7 @@ __device__ void v2_null(Lane &L, LaneScratch &S) {
     // a reset of captured state is not something a template replays
     if (tgt == TG_CHOICES || (tgt == TG_USAGE && (L.sf & SF_USAGE)) || tgt == TG_TOOLCALLS || tgt == TG_TC_ID || tgt == TG_TC_TYPE || tgt == TG_TC_FUNCTION) rec_nonsimple<REC>(S);
     switch (tgt) {
-    case TG_CHOICES:
-        L.n_choices = 0; L.choices_count = 0; L.finish = SSE_FIN_NONE; L.content_off = L.content_len = 0;
-        L.sf &= ~(SF_CDEC | SF_CBAD | SF_CSET | SF_TCNONNIL | SF_TCOPEN | SF_TCVALID);
-        L.tc_count = 0; L.tc_first = SSE_NONE;
-        break;
+    case TG_CHOICES: v2_choices_reset(L); break;
     case TG_USAGE: L.sf &= ~SF_USAGE; S.u_prompt = S.u_completion = S.u_total = 0; break;
     case TG_TOOLCALLS:
         if (lane_live(L)) { L.sf &= ~(SF_TCNONNIL | SF_TCOPEN | SF_TCVALID); L.tc_count = 0; L.tc_first = SSE_NONE; }
@@ -292,7 +296,7 @@ __device__ bool v2_action(const KParams &P, const DfaTables &T, Lane &L, LaneScr
         else {
             const uint32_t node = lane_top(L);
             L.sd--;
-            if (node == A_CHOICES) L.n_choices = L.choices_count;
+            if (node == A_CHOICES) { if (L.choices_count) L.n_choices = L.choices_count; else v2_choices_reset(L); }
             else if (node == A_TOOLCALLS) { if (lane_live(L) && (L.sf & SF_TCOPEN)) v2_flush_tc(P, L, S, J); }
             else if (node == N_GOOGLE) { if (L.sf & SF_GBAD) L.sf |= SF_TYPE; }
         }

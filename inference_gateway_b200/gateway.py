@@ -137,10 +137,11 @@ class Gateway:
         content = C.string_at(b.p, b.n) if b.n else b""
         fin = C.c_int()
         term = bool(self.L.ssegw_agent_terminated(self.g, sid, C.byref(fin)))
-        arr = (A.ToolCall * 64)()
-        n = self.L.ssegw_agent_tool_calls(self.g, sid, arr, 64)
+        n = self.L.ssegw_agent_tool_calls(self.g, sid, None, 0)
+        arr = (A.ToolCall * max(1, n))()
+        n = min(n, self.L.ssegw_agent_tool_calls(self.g, sid, arr, n))
         g = lambda x: C.string_at(x.p, x.n) if x.n else b""
-        calls = [dict(id=g(arr[i].id), type=g(arr[i].type), name=g(arr[i].name), args=g(arr[i].arguments)) for i in range(min(n, 64))]
+        calls = [dict(id=g(arr[i].id), type=g(arr[i].type), name=g(arr[i].name), args=g(arr[i].arguments)) for i in range(n)]
         return content, bool(self.L.ssegw_agent_has_tool_calls(self.g, sid)), term, fin.value, calls
 
     def counters(self) -> dict:

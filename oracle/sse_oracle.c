@@ -522,7 +522,11 @@ static void d_array(dec *d, int ety, int esub, int tgt, int live, int depth) {
         if (d->s[d->p] == ',') { d->p++; continue; }
         d->p++; break;
     }
-    if (tgt == TG_CHOICES) d->n_choices = (uint32_t)count;
+    if (tgt == TG_CHOICES) {
+        d->n_choices = (uint32_t)count;
+        /* decode.go array(): an empty array sets a fresh slice of capacity 0, so a later "choices" array grows new, zeroed storage */
+        if (count == 0) reset_choice0(d);
+    }
 }
 static void d_value(dec *d, int ty, int sub, int ety, int esub, int tgt, int live, int depth) {
     (void)depth;

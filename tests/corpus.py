@@ -53,6 +53,14 @@ TRICKY = [
     b'{"choices":[{"delta":{"content":"first"}},{"delta":{"content":"second","tool_calls":[{"id":"x"}]},"finish_reason":"stop"}]}',
     b'{"choices":[{"delta":{"content":"a"}}],"choices":[{"finish_reason":"stop"}]}',
     b'{"choices":[{"delta":{"content":"a"}}],"choices":null}', b'{"choices":[{"delta":{"content":"a"}}],"choices":[]}',
+    # an empty "choices" array is a fresh slice of capacity 0 (decode.go array()): a later array's element 0 starts empty
+    b'{"choices":[{"delta":{"content":"a"},"finish_reason":"stop"}],"choices":[],"choices":[{"delta":{}}]}',
+    b'{"choices":[{"delta":{"content":"a"},"finish_reason":"stop"}],"choices":[],"choices":null}',
+    b'{"choices":[{"delta":{"content":"a"},"finish_reason":"stop"}],"choices":[]}',
+    b'{"choices":[{"delta":{"tool_calls":[{"index":0,"id":"c","function":{"name":"f","arguments":"x"}}]},"finish_reason":"tool_calls"}],'
+    b'"choices":[ ],"choices":[{"delta":{"content":"b"}}]}',
+    b'{"choices":[{"delta":{"content":"a"}}],"choices":[],"choices":[{"finish_reason":"stop"}],"choices":[{"delta":{"content":"c"}}]}',
+    b'{"choices":[],"choices":[{"delta":{"content":"b"},"finish_reason":"stop"}]}',
     b'{"unknown":{"deep":[1,2,{"x":[true,false,null,"s",1.5e-3]}]},"choices":[{"delta":{"content":"ok"}}]}',
     b'\t\r\n {"choices" : [ { "delta" : { "content" : "ws" } , "finish_reason" : null } ] } \r',
     b"[" * 128 + b"]" * 128, b"[" * 129 + b"]" * 129, b'{"a":' * 100 + b"1" + b"}" * 100,

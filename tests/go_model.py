@@ -303,6 +303,8 @@ class Decoder:
                     self.err = True
                 else:
                     res["n_choices"] = len(x)
+                    if not x:              # decode.go array(): [] sets a fresh slice of capacity 0; a later array starts anew
+                        res["st"] = self._fresh()
                     for i, e in enumerate(x):
                         self.choice(e, res["st"] if i == 0 else self._fresh())
             elif f == "int":

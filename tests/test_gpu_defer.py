@@ -8,46 +8,15 @@ import pytest
 
 from inference_gateway_b200 import SseEngine, _abi as A, synth
 from inference_gateway_b200.gateway import Gateway
-from inference_gateway_b200.synth import random_cuts
 from oracle import orc
 from tests.corpus import adversarial_bodies
 from tests.util import (ENGINES, TINY_DECODE, TINY_PRODUCE, ConnOut, check_streams, fold_segment, process_all_checked,
-                        process_checked)
+                        process_checked, run_deferred)
 
 pytestmark = pytest.mark.gpu
 
 P, R, PP = A.MODE_P, A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
 MiB = 1 << 20
-
-
-def run_deferred(eng, bodies, modes, n_batches=1, seed=0, with_folds=False, n_folds=None):
-    """run_streams (tests/util.py) on an engine with SSE_FLAG_DEFER: every micro-batch of pieces is run to the end with
-    SseEngine.process_all, which submits deferred remainders again until every byte was taken. The agent and telemetry folds
-    are fed for the first n_folds streams (all by default). Returns (outs, stats)."""
-    rng = np.random.default_rng(seed)
-    L = eng.L
-    outs = [ConnOut() for _ in bodies]
-    eng.reset_all()
-    pieces = [random_cuts(rng, b, n_batches) for b in bodies]
-    if with_folds:
-        for o in outs[:n_folds]:
-            o.agent, o.tele = L.sse_agent_new(), L.sse_telemetry_new()
-    stats = dict(batches=0, deferred=0, overflow=0)
-
-    def on_batch(res, conns):
-        stats["overflow"] |= res.overflow
-        for i, c in enumerate(conns):
-            o = outs[c]
-            fold_segment(o, res, i)
-            stats["deferred"] += bool(int(res.segs[i]["flags"]) & A.SEG_DEFERRED)
-            if o.agent is not None:
-                A.check(L.sse_agent_feed(o.agent, C.byref(res.raw), i), "sse_agent_feed")
-                A.check(L.sse_telemetry_feed(o.tele, C.byref(res.raw), i), "sse_telemetry_feed")
-
-    for b in range(max(len(p) for p in pieces)):
-        items = [(c, modes[c], pieces[c][b]) for c in range(len(bodies)) if b < len(pieces[c])]
-        stats["batches"] += process_all_checked(eng, items, on_batch)
-    return outs, stats
 
 
 N_C4 = 160

@@ -40,6 +40,18 @@ class ConnOut:
         self.flags = 0
         self.agent = None
         self.tele = None
+        self.fold_rcs = []     # (piece index, sse_agent_feed rc, sse_telemetry_feed rc) of every segment fed to the folds
+        self.piece_ends = []   # end offset in the body of every piece submitted, in piece order
+
+
+def feed_folds(L, o: ConnOut, res, i: int, piece: int, keep_codes: bool):
+    """Feeds segment i of a batch result, which holds bytes of piece `piece`, to the connection's folds. keep_codes: their
+    return codes go to o.fold_rcs (check_folds judges them); otherwise a code other than SSE_OK raises."""
+    rcs = (L.sse_agent_feed(o.agent, C.byref(res.raw), i), L.sse_telemetry_feed(o.tele, C.byref(res.raw), i))
+    o.fold_rcs.append((piece, *rcs))
+    if not keep_codes:
+        A.check(rcs[0], "sse_agent_feed")
+        A.check(rcs[1], "sse_telemetry_feed")
 
 
 def rec_to_dict(res, ri: int) -> dict:
@@ -60,7 +72,9 @@ def rec_to_dict(res, ri: int) -> dict:
         d["tc_valid"] = bool(fl & A.F_TC_VALID)
         tcs = []
         t = int(r["tc_first"])
-        for _ in range(int(r["tc_count"])):
+        count = int(r["tc_count"])
+        # tc_count saturates at 0xFFFF: a saturated chain is walked to its end
+        while len(tcs) < count or (count == 0xFFFF and t != A.NONE):
             assert t != A.NONE, "tool-call chain shorter than tc_count"
             tc = res.tcs[t]
             tf = int(tc["flags"])
@@ -159,10 +173,11 @@ def process_all_checked(eng, items, on_batch=None) -> int:
         return eng.process_all(items, on_batch)
 
 
-def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False):
+def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False, keep_codes=False):
     """streams: list of bytes (one upstream body per connection); modes: list of mode bits.
     Feeds every stream in n_batches randomly cut pieces (simulated TCP segmentation), one micro-batch per
-    piece index. Returns list[ConnOut]."""
+    piece index, and with_folds, every segment to the connection's agent and telemetry folds (feed_folds: keep_codes keeps
+    their return codes for check_folds instead of raising). Returns list[ConnOut]."""
     from inference_gateway_b200.synth import random_cuts
     rng = np.random.default_rng(seed)
     L = engine.L
@@ -170,6 +185,8 @@ def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False):
     outs = [ConnOut() for _ in range(n)]
     engine.reset_all()
     pieces = [random_cuts(rng, s, n_batches) for s in streams]
+    for o, p in zip(outs, pieces):
+        o.piece_ends = np.cumsum([len(x) for x in p]).tolist()
     if with_folds:
         for o in outs:
             o.agent = L.sse_agent_new()
@@ -189,11 +206,44 @@ def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False):
                 o = outs[c]
                 fold_segment(o, res, i)
                 if with_folds:
-                    A.check(L.sse_agent_feed(o.agent, C.byref(res.raw), i), "sse_agent_feed")
-                    A.check(L.sse_telemetry_feed(o.tele, C.byref(res.raw), i), "sse_telemetry_feed")
+                    feed_folds(L, o, res, i, b, keep_codes)
         finally:
             engine.release(slot)
     return outs
+
+
+def run_deferred(eng, bodies, modes, n_batches=1, seed=0, with_folds=False, n_folds=None, keep_codes=False):
+    """run_streams on an engine with SSE_FLAG_DEFER: every micro-batch of pieces is run to the end with SseEngine.process_all,
+    which submits deferred remainders again until every byte was taken. The agent and telemetry folds are fed for the first
+    n_folds streams (all by default). Returns (outs, stats)."""
+    from inference_gateway_b200.synth import random_cuts
+    rng = np.random.default_rng(seed)
+    L = eng.L
+    outs = [ConnOut() for _ in bodies]
+    eng.reset_all()
+    pieces = [random_cuts(rng, b, n_batches) for b in bodies]
+    for o, p in zip(outs, pieces):
+        o.piece_ends = np.cumsum([len(x) for x in p]).tolist()
+    if with_folds:
+        for o in outs[:n_folds]:
+            o.agent, o.tele = L.sse_agent_new(), L.sse_telemetry_new()
+    stats = dict(batches=0, deferred=0, overflow=0)
+    piece = [0]
+
+    def on_batch(res, conns):
+        stats["overflow"] |= res.overflow
+        for i, c in enumerate(conns):
+            o = outs[c]
+            fold_segment(o, res, i)
+            stats["deferred"] += bool(int(res.segs[i]["flags"]) & A.SEG_DEFERRED)
+            if o.agent is not None:
+                feed_folds(L, o, res, i, piece[0], keep_codes)
+
+    for b in range(max(len(p) for p in pieces)):
+        piece[0] = b
+        items = [(c, modes[c], pieces[c][b]) for c in range(len(bodies)) if b < len(pieces[c])]
+        stats["batches"] += process_all_checked(eng, items, on_batch)
+    return outs, stats
 
 
 def run_pieces(eng, pieces, modes):
@@ -523,26 +573,36 @@ def _bytes(b: A.Bytes) -> bytes:
     return C.string_at(b.p, b.n) if b.n else b""
 
 
+def _calls(arr, n):
+    return [dict(id=_bytes(arr[i].id), type=_bytes(arr[i].type), name=_bytes(arr[i].name), args=_bytes(arr[i].arguments))
+            for i in range(n)]
+
+
 def agent_results(L, fold):
+    """An agent fold's (content, has_tool_calls, terminated, finish, every merged tool call)."""
     content = _bytes(L.sse_agent_content(fold))
     has = bool(L.sse_agent_has_tool_calls(fold))
     fin = C.c_int()
     term = bool(L.sse_agent_terminated(fold, C.byref(fin)))
-    arr = (A.ToolCall * 64)()
-    n = L.sse_agent_tool_calls(fold, arr, 64)
-    calls = [dict(id=_bytes(arr[i].id), type=_bytes(arr[i].type), name=_bytes(arr[i].name), args=_bytes(arr[i].arguments))
-             for i in range(min(n, 64))]
-    return content, has, term, fin.value, calls
+    n = L.sse_agent_tool_calls(fold, None, 0)
+    arr = (A.ToolCall * max(1, n))()
+    assert L.sse_agent_tool_calls(fold, arr, n) == n
+    return content, has, term, fin.value, _calls(arr, n)
 
 
 def telemetry_results(L, fold):
+    """sse_telemetry_finish: (rc, usage, every tool call). The call array is sized from the count a first call returns; the
+    fold closes its open piece once, so the second call sees the same state."""
     u = A.Usage()
-    arr = (A.ToolCall * 64)()
     n = C.c_size_t()
+    arr = (A.ToolCall * 64)()
     rc = L.sse_telemetry_finish(fold, C.byref(u), arr, 64, C.byref(n))
-    calls = [dict(id=_bytes(arr[i].id), type=_bytes(arr[i].type), name=_bytes(arr[i].name), args=_bytes(arr[i].arguments))
-             for i in range(min(n.value, 64))]
-    return rc, (u.prompt_tokens, u.completion_tokens, u.total_tokens), calls
+    if n.value > 64:
+        arr = (A.ToolCall * n.value)()
+        m = C.c_size_t()
+        rc = L.sse_telemetry_finish(fold, C.byref(u), arr, n.value, C.byref(m))
+        assert m.value == n.value
+    return rc, (u.prompt_tokens, u.completion_tokens, u.total_tokens), _calls(arr, n.value)
 
 
 def _expect(l, frame: int, done: bool, mode_r: bool) -> dict:
@@ -616,18 +676,55 @@ def check_agent(state, v, label=""):
     assert calls == orc.parse_tool_calls(v.builder), f"{label}: tool calls differ from the oracle's"
 
 
+def irregular_telemetry(body: bytes) -> bool:
+    """Whether telemetry's "\n\n" pieces of body hold one of several non-blank lines that starts with "data: " (DESIGN.md §5,
+    deviation 4): the telemetry fold then finishes with 1 and its usage and tool calls are not the reference's."""
+    return any(p.startswith(b"data: ") and sum(1 for x in p.split(b"\n") if x) > 1 for p in body.split(b"\n\n"))
+
+
+def first_limited_piece(v, piece_ends):
+    """The piece that completes the oracle's first line past the nesting limit (v: its view of the body; piece_ends: the end
+    offset of every piece), or None when no line is."""
+    end = 0
+    for l in v.lines:
+        end += len(l.line)
+        if l.kind != orc.L_UNREAD and l.depth_limited:
+            return next(k for k, e in enumerate(piece_ends) if e >= end)
+    return None
+
+
 def check_folds(L, o: ConnOut, mode: int, v, label=""):
     """The agent and telemetry folds run_streams(with_folds=True) fed for one connection, against the oracle (v: what
-    check_stream returned). Mode R: the agent fold (check_agent), and the telemetry over the frames and the [DONE] the agent
-    writes at the end; mode P|PARSE: the telemetry over the frames. Returns the agent fold's state (None outside mode R)."""
+    check_stream returned).
+    - A stream without a line past the nesting limit: every feed returns SSE_OK. Mode R: the agent fold (check_agent), and
+      the telemetry over the frames and the [DONE] the agent writes at the end; mode P|PARSE: the telemetry over the frames.
+      The telemetry finishes with 1 exactly when those bytes have an irregular piece (irregular_telemetry), and is then not
+      compared further; else with 0 and the oracle's usage and tool calls.
+    - A stream with one: both feeds return SSE_OK up to the piece that completes the first such line and SSE_ERR_UNDECODED in
+      it; the accumulators are short and are not compared.
+    Returns the agent fold's state (None outside mode R, or when the stream has a line past the nesting limit)."""
+    limited = first_limited_piece(v, o.piece_ends)
+    bad = [(p, a, t) for p, a, t in o.fold_rcs if (a, t) != (A.SSE_OK, A.SSE_OK)]
+    if limited is not None:
+        assert bad and bad[0][0] == limited and bad[0][1:] == (A.SSE_ERR_UNDECODED,) * 2, \
+            f"{label}: first failed feeds {bad[:1]}, oracle: a line past the nesting limit in piece {limited}"
+        return None
+    assert not bad, f"{label}: feeds failed {bad[:4]} (piece, agent rc, telemetry rc) on a stream the decoder can take whole"
     state = None
     if mode & A.MODE_R:
         state = agent_results(L, o.agent)
         check_agent(state, v, label)
         A.check(L.sse_telemetry_feed_bytes(o.tele, DONE, len(DONE)), "sse_telemetry_feed_bytes")
-        assert telemetry_results(L, o.tele) == (0, *orc.telemetry(b"".join(o.frames) + DONE)), f"{label}: telemetry differs"
+        body = b"".join(o.frames) + DONE
     elif mode & A.MODE_PARSE:
-        assert telemetry_results(L, o.tele) == (0, *orc.telemetry(b"".join(o.frames))), f"{label}: telemetry differs"
+        body = b"".join(o.frames)
+    else:
+        return None
+    rc, usage, calls = telemetry_results(L, o.tele)
+    if irregular_telemetry(body):
+        assert rc == 1, f"{label}: telemetry finished with {rc} on a body with an irregular piece"
+    else:
+        assert (rc, usage, calls) == (0, *orc.telemetry(body)), f"{label}: telemetry differs"
     return state
 
 
