@@ -3,6 +3,8 @@
  * (implemented in inference_gateway_b200/csrc/sse_gateway.cpp, exported by libssegpu.so).
  *
  *   ssegw_stream_chat_completions   core.IProvider.StreamChatCompletions (providers/core/interfaces.go:22; provider.go:277-344)
+ *   ssegw_stream_with_telemetry     the same, with the response's telemetry fold fed from the stream's records
+ *                                   (api/middlewares/telemetry.go:37-54, :190-277)
  *   ssegw_upstream_write / _close   response.Body bytes / EOF-or-error (provider.go:322-330)
  *   ssegw_pump                      one tick of the per-GPU batchers (INTEGRATION.md section 2), batches in flight per context
  *   ssegw_flush                     collects every batch still in flight
@@ -41,8 +43,9 @@ ssegw *ssegw_new_cfg(int device, const sse_config *cfg, const sse_line_pool *poo
  * whole life (carry state and line-pool pages are per context).
  * depth (1 .. cfg->n_slots) is how many batches a context may have uncollected. ssegw_pump then runs, per context: fill and
  * submit a batch if any stream has bytes that may go in; collect every batch sse_poll reports done, oldest first; collect the
- * oldest, blocking, while depth batches are uncollected. Frames reach the channels, the agent folds and the counters at
- * collect time, in submission order per context. At depth 1 this is ssegw_new_cfg's tick: a pump delivers what it submitted.
+ * oldest, blocking, while depth batches are uncollected. Frames reach the channels, the agent folds, the telemetry taps and
+ * the counters at collect time, in submission order per context. At depth 1 this is ssegw_new_cfg's tick: a pump delivers
+ * what it submitted.
  * Bytes leave a stream's queue when they are submitted. Without SSE_FLAG_DEFER a stream may have bytes in several uncollected
  * batches (the device keeps their order); with it, a stream is not offered again while it is in an uncollected batch, and its
  * deferred rest goes back to the front of its queue when that batch is collected. A failed batch closes its streams, and
@@ -56,7 +59,30 @@ ssegw *ssegw_new_multi(const int *devices, uint32_t n_devices, const sse_config 
  * batches after a failed one are still collected). ssegw_free flushes before it destroys the contexts. */
 int    ssegw_flush(ssegw *g);
 void   ssegw_free(ssegw *g);
+/* Opens a stream on a free connection (placement as in ssegw_new_multi) and resets the connection. Returns the stream id,
+ * or -1 when no connection is free. */
 int    ssegw_stream_chat_completions(ssegw *g, uint8_t mode);
+/* The telemetry tap (api/middlewares/telemetry.go:190-277 without buffering the body): opens a stream like
+ * ssegw_stream_chat_completions(g, mode) whose records also feed the caller's fold `tel`.
+ *   Modes: mode must carry SSE_MODE_PARSE or SSE_MODE_R (a mode P stream has no records); otherwise, or when tel is NULL,
+ *     SSE_ERR_ARG. Placement, reset and the return value are those of ssegw_stream_chat_completions: the stream id, or -1
+ *     when no connection is free.
+ *   One feeder at a time: a fold feeds at most one open stream. Attaching it while another stream it feeds is open returns
+ *     SSE_ERR_BUSY; once that stream is released, the fold may be attached to the next one (the next agent iteration).
+ *   What is fed: at collect time, the segments whose frames the gateway delivers to this stream's channel, in submission
+ *     order per context at any depth. Nothing is fed after ssegw_release_stream, including what batches still in flight
+ *     return for the released stream. A segment the fold cannot decode (sse_telemetry_feed returns SSE_ERR_UNDECODED: a
+ *     line past the nesting limit) closes the stream, as it does for the agent fold of a mode R stream.
+ *   Host-written bytes: the gateway feeds only bytes it received from upstream. What the caller writes to the client itself
+ *     goes in with sse_telemetry_feed_bytes: the agent's single final "data: [DONE]\n\n" (ssegw_agent_recv synthesises one
+ *     per iteration; only the last iteration's belongs in the client's body) and any error frames.
+ *   Ownership: the caller creates, finishes and frees the fold (sse_telemetry_new / _finish / _free). It must outlive every
+ *     stream it is attached to until that stream is released or ssegw_free runs; ssegw_free does not free it.
+ *   Proxy route: ssegw_proxy_step works on any stream id, so a tapped SSE_MODE_P | SSE_MODE_PARSE stream serves the raw
+ *     proxy loop too (its frames are those of mode P). Whether proxy responses are recorded is the caller's decision: the
+ *     reference's path filter (telemetry.go:60-63) matches some proxy paths, e.g. /compatibility/v1/chat/completions.
+ * Streams opened without a tap behave as before: a mode P | PARSE stream ignores its records and is never closed by them. */
+int    ssegw_stream_with_telemetry(ssegw *g, uint8_t mode, sse_telemetry_fold *tel);
 size_t ssegw_upstream_write(ssegw *g, int stream, const uint8_t *data, size_t n);
 void   ssegw_upstream_close(ssegw *g, int stream);
 int    ssegw_pump(ssegw *g);

@@ -41,6 +41,7 @@ struct Stream {
     std::deque<std::string> chan;
     bool terminated = false;    // mode R: agent loop left (finish_reason stop/tool_calls)
     sse_agent_fold *agent = nullptr;
+    sse_telemetry_fold *tel = nullptr;   // the caller's tap (ssegw_stream_with_telemetry), not owned; null: no tap
     bool done_sent = false;
     bool deferred = false;      // SSE_FLAG_DEFER: the last batch left bytes of this stream in `pending`; offered first next tick
     uint64_t gen = 0;           // bumped at every open: a batch that holds bytes of an earlier stream on the slot delivers nothing here
@@ -171,7 +172,9 @@ int collect_oldest(ssegw *g, Ctx &x) {
             run = &res.runs[run->next];
         }
         // a record the library could not decode (SSE_ERR_UNDECODED): the accumulators would be silently short, so the stream is failed
-        if ((s.mode & SSE_MODE_R) && sse_agent_feed(s.agent, &res, k) != SSE_OK) s.closed = true;
+        bool undecoded = (s.mode & SSE_MODE_R) && sse_agent_feed(s.agent, &res, k) != SSE_OK;
+        if (s.tel && sse_telemetry_feed(s.tel, &res, k) != SSE_OK) undecoded = true;
+        if (undecoded) s.closed = true;
         if (res.segs[k].flags & SSE_SEG_TERMINATED) s.terminated = true;
         if (res.segs[k].flags & SSE_SEG_DEAD) s.closed = true;
     }
@@ -239,8 +242,9 @@ void ssegw_free(ssegw *g) {
 }
 
 // StreamChatCompletions: binds a new stream to a free connection of the context with the fewest open streams (the lowest
-// index on a tie), where it stays for its whole life. Returns the stream id or -1 (no free slot).
-int ssegw_stream_chat_completions(ssegw *g, uint8_t mode) {
+// index on a tie), where it stays for its whole life; tel (may be null) is its telemetry tap. Returns the stream id or -1
+// (no free slot).
+static int open_stream(ssegw *g, uint8_t mode, sse_telemetry_fold *tel) {
     const size_t nc = g->cfg.max_conns;
     size_t k = g->ctxs.size();
     for (size_t j = 0; j < g->ctxs.size(); j++)
@@ -257,10 +261,20 @@ int ssegw_stream_chat_completions(ssegw *g, uint8_t mode) {
             g->ctxs[k].n_open++;
             // ordered after every batch already submitted, which may still hold bytes of the slot's previous stream
             if (sse_reset_conn(g->ctxs[k].ctx, (uint32_t)(i - k * nc)) != SSE_OK) return -1;
+            s.tel = tel;
             return (int)i;
         }
     }
     return -1;
+}
+
+int ssegw_stream_chat_completions(ssegw *g, uint8_t mode) { return open_stream(g, mode, nullptr); }
+
+int ssegw_stream_with_telemetry(ssegw *g, uint8_t mode, sse_telemetry_fold *tel) {
+    if (!g || !tel || !(mode & (SSE_MODE_PARSE | SSE_MODE_R))) return SSE_ERR_ARG;
+    for (const Stream &s : g->streams)
+        if (s.open && s.tel == tel) return SSE_ERR_BUSY;     // one feeder at a time: the pieces of two bodies would interleave
+    return open_stream(g, mode, tel);
 }
 
 // Bytes from response.Body. Returns the number of bytes accepted (0 when the channel is full: back-pressure).
@@ -332,6 +346,7 @@ void ssegw_release_stream(ssegw *g, int id) {
     Stream &s = g->streams[(size_t)id];
     if (s.open) g->ctxs[(size_t)id / g->cfg.max_conns].n_open--;
     s.open = false;
+    s.tel = nullptr;      // the caller may free or reattach its fold now: nothing collected later feeds it
 }
 
 int ssegw_counters(ssegw *g, sse_counters *out) {

@@ -7,6 +7,44 @@ import ctypes as C
 from . import _abi as A
 
 
+def _bytes(b: A.Bytes) -> bytes:
+    return C.string_at(b.p, b.n) if b.n else b""
+
+
+class Telemetry:
+    """One telemetry fold (sse_telemetry_*): api/middlewares/telemetry.go:190-277 over one client response. Attach it to the
+    upstream streams that make up the response (Gateway.stream_chat_completions / proxy_stream, one open at a time) and
+    feed what the handler writes itself (the agent's final [DONE], error frames) with feed_bytes."""
+
+    def __init__(self):
+        self.L = A.load()
+        self.f = self.L.sse_telemetry_new()
+        if not self.f:
+            raise MemoryError("sse_telemetry_new")
+
+    def feed_bytes(self, b: bytes):
+        A.check(self.L.sse_telemetry_feed_bytes(self.f, b, len(b)), "sse_telemetry_feed_bytes")
+
+    def finish(self):
+        """(rc, (prompt, completion, total), tool calls): rc 1 when a piece of the body was irregular (DESIGN.md §5,
+        deviation 4), else 0. Feed nothing after it."""
+        u, n = A.Usage(), C.c_size_t()
+        rc = self.L.sse_telemetry_finish(self.f, C.byref(u), None, 0, C.byref(n))
+        arr = (A.ToolCall * max(1, n.value))()
+        if n.value:
+            rc = self.L.sse_telemetry_finish(self.f, C.byref(u), arr, n.value, C.byref(n))
+        if rc < 0:
+            raise A.SseError(rc, "sse_telemetry_finish")
+        calls = [dict(id=_bytes(c.id), type=_bytes(c.type), name=_bytes(c.name), args=_bytes(c.arguments)) for c in arr[:n.value]]
+        return rc, (u.prompt_tokens, u.completion_tokens, u.total_tokens), calls
+
+    def close(self):
+        """Frees the fold: only once no open stream of a gateway feeds it."""
+        if self.f:
+            self.L.sse_telemetry_free(self.f)
+            self.f = None
+
+
 class Gateway:
     def __init__(self, device: int = 0, max_conns: int = 256, bytes_per_batch: int = 1 << 20, line_pool: dict | None = None,
                  config: A.Config | None = None, devices: list[int] | None = None, depth: int = 1):
@@ -33,6 +71,7 @@ class Gateway:
         L.ssegw_free.argtypes = [vp]
         L.ssegw_free.restype = None
         L.ssegw_stream_chat_completions.argtypes = [vp, C.c_uint8]
+        L.ssegw_stream_with_telemetry.argtypes = [vp, C.c_uint8, vp]
         L.ssegw_upstream_write.argtypes = [vp, i32, C.c_char_p, C.c_size_t]
         L.ssegw_upstream_write.restype = C.c_size_t
         L.ssegw_upstream_close.argtypes = [vp, i32]
@@ -69,17 +108,31 @@ class Gateway:
         if not self.g:
             raise A.SseError(st.value, "ssegw_new")
         self._buf = C.create_string_buffer(1 << 20)
+        self._taps = {}          # stream id -> the Telemetry it feeds, kept alive until the stream is released
 
     def close(self):
         if self.g:
             self.L.ssegw_free(self.g)
             self.g = None
+            self._taps.clear()
 
-    def stream_chat_completions(self, mode: int) -> int:
-        sid = self.L.ssegw_stream_chat_completions(self.g, mode)
+    def _open(self, mode: int, telemetry: Telemetry | None) -> int:
+        if telemetry is None:
+            sid = self.L.ssegw_stream_chat_completions(self.g, mode)
+        else:
+            sid = self.L.ssegw_stream_with_telemetry(self.g, mode, telemetry.f)
+            if sid < -1:
+                raise A.SseError(sid, "ssegw_stream_with_telemetry")
         if sid < 0:
             raise RuntimeError("no free connection slot")
+        if telemetry is not None:
+            self._taps[sid] = telemetry
         return sid
+
+    def stream_chat_completions(self, mode: int, telemetry: Telemetry | None = None) -> int:
+        """telemetry: the response's fold, fed from this stream's records (mode must have MODE_PARSE or MODE_R; a fold
+        feeds one open stream at a time: SseError SSE_ERR_BUSY otherwise)."""
+        return self._open(mode, telemetry)
 
     def upstream_write(self, sid: int, data: bytes) -> int:
         return self.L.ssegw_upstream_write(self.g, sid, data, len(data))
@@ -118,8 +171,11 @@ class Gateway:
         """One channel element, None if nothing is available yet; raises EOFError when the channel is closed."""
         return self._recv(self.L.ssegw_recv, sid)
 
-    def proxy_stream(self) -> int:
-        """handleStreamingRequest (api/routes.go:129-232): the raw /proxy stream."""
+    def proxy_stream(self, telemetry: Telemetry | None = None) -> int:
+        """handleStreamingRequest (api/routes.go:129-232): the raw /proxy stream. With telemetry, a MODE_P | MODE_PARSE
+        stream (same frames) whose records feed the fold."""
+        if telemetry is not None:
+            return self._open(A.MODE_P | A.MODE_PARSE, telemetry)
         sid = self.L.ssegw_proxy_stream(self.g)
         if sid < 0:
             raise RuntimeError("no free connection slot")
@@ -140,7 +196,7 @@ class Gateway:
         n = self.L.ssegw_agent_tool_calls(self.g, sid, None, 0)
         arr = (A.ToolCall * max(1, n))()
         n = min(n, self.L.ssegw_agent_tool_calls(self.g, sid, arr, n))
-        g = lambda x: C.string_at(x.p, x.n) if x.n else b""
+        g = _bytes
         calls = [dict(id=g(arr[i].id), type=g(arr[i].type), name=g(arr[i].name), args=g(arr[i].arguments)) for i in range(n)]
         return content, bool(self.L.ssegw_agent_has_tool_calls(self.g, sid)), term, fin.value, calls
 
@@ -154,6 +210,7 @@ class Gateway:
 
     def release(self, sid: int):
         self.L.ssegw_release_stream(self.g, sid)
+        self._taps.pop(sid, None)
 
     def mcp_write_loop(self, sid: int):
         """handleMCPStreamingRequest's writer (api/middlewares/mcp.go:253-299) over the agent channel of one stream:

@@ -32,12 +32,16 @@ import (
 // connections with such a tail are drained first into the next batch, and a connection is not drained again while it is in
 // an uncollected batch (its tail must come before its newer bytes). The host mirror is ssegw_new_multi / ssegw_pump.
 type Batcher interface {
-	// Open registers a new upstream stream; the returned id addresses its slot until Close.
-	Open(mode uint8) (conn uint32, frames <-chan []byte)
+	// Open registers a new upstream stream; the returned id addresses its slot until Close. tel, when not nil, is the
+	// client response's telemetry fold (mode must then carry ModeParse or ModeR): the deliver step feeds it every segment
+	// whose frames it delivers to this connection, until Close (ssegw_stream_with_telemetry is the host mirror). One fold
+	// feeds one open connection at a time; an MCP session attaches it to each iteration's connection in turn.
+	Open(mode uint8, tel *Telemetry) (conn uint32, frames <-chan []byte)
 	// Feed hands over bytes read from the upstream body (any cut points). EOF/err closes the stream after the
 	// lines already queued, and those in uncollected batches, were delivered; the unterminated tail is dropped
 	// (provider.go:323-330).
 	Feed(conn uint32, data []byte)
+	// Close releases the connection; once it returns, nothing collected later is delivered or fed to its fold.
 	Close(conn uint32)
 	// Open streams, for placement.
 	Streams() int
@@ -53,11 +57,21 @@ type inFlight struct {
 type member struct {
 	conn uint32
 	gen  uint64
-	data []byte // the bytes submitted (a view of the batch's pinned arena), for the deferred tail
+	data []byte     // the bytes submitted (a view of the batch's pinned arena), for the deferred tail
+	tel  *Telemetry // the connection's telemetry fold at submit time, nil without a tap
+}
+
+// feedTap is the telemetry half of the deliver step for segment i of a collected batch, held by m. The deliver step calls
+// it next to the agent fold's feed, after the segment's frames went to the connection's channel, and only when m.gen is
+// still the connection's generation and the connection is neither closed nor failed, so that nothing is fed after Close.
+// It reports whether the stream must be closed: the fold met a line past the nesting limit (SSE_ERR_UNDECODED).
+func feedTap(m member, res *Result, i uint32) (closeStream bool) {
+	return m.tel != nil && m.tel.Feed(res, i) != nil
 }
 
 // RunTick is steps 2 and 3 of a tick, after step 1 appended the submitted batch (if any) to q. deliver fans one collected
-// batch out (frames, Deferred tails, agent folds, counters) in submission order; a failed batch closes its streams.
+// batch out (frames, Deferred tails, agent folds, telemetry taps through feedTap, counters) in submission order; a failed
+// batch closes its streams.
 func RunTick(x *Context, q []inFlight, depth int, deliver func(inFlight, *Result, error)) ([]inFlight, error) {
 	collect := func() {
 		f := q[0]
@@ -136,6 +150,24 @@ func pick(bs []Batcher) Batcher {
 	return best
 }
 
+type modeKey struct{}
+type telemetryKey struct{}
+
+// WithMode is how the MCP agent asks for ModeR on its provider stream.
+func WithMode(ctx context.Context, mode uint8) context.Context { return context.WithValue(ctx, modeKey{}, mode) }
+
+// WithTelemetry puts the client response's telemetry fold into the request context (StreamingTelemetry does, for
+// streaming chat completions): the provider attaches it to the stream it opens.
+func WithTelemetry(ctx context.Context, t *Telemetry) context.Context {
+	return context.WithValue(ctx, telemetryKey{}, t)
+}
+
+// TelemetryFrom is the response's fold, or nil when telemetry is off or the request is not a streaming chat completion.
+func TelemetryFrom(ctx context.Context) *Telemetry {
+	t, _ := ctx.Value(telemetryKey{}).(*Telemetry)
+	return t
+}
+
 // gpuProvider embeds the stock provider (nine methods for free) and replaces only the stream reader.
 type gpuProvider struct {
 	core.IProvider
@@ -151,9 +183,20 @@ func (p *gpuProvider) StreamChatCompletions(ctx context.Context, req types.Creat
 		return nil, err // before streaming: (nil, err), *core.HTTPError carries the upstream status
 	}
 	b := pick(p.bs)
-	conn, frames := b.Open(ModeP) // the MCP agent asks for ModeR via a context key instead
+	mode, _ := ctx.Value(modeKey{}).(uint8) // ModeP, or ModeR when the MCP agent asked for it (WithMode)
+	tel := TelemetryFrom(ctx)
+	if tel != nil && mode&ModeR == 0 {
+		mode |= ModeParse // the tap needs the records: same frames as ModeP
+	}
+	if tel != nil {
+		tel.open.Add(1)
+	}
+	conn, frames := b.Open(mode, tel)
 	go func() {                     // socket reads stay on the host; one goroutine per stream as in provider.go:308
 		defer resp.Body.Close()
+		if tel != nil {
+			defer tel.open.Done() // after b.Close: the middleware may then finish and free the fold
+		}
 		defer b.Close(conn)
 		buf := make([]byte, 32<<10)
 		for {

@@ -18,6 +18,7 @@ import (
 	"os"
 	"runtime"
 	"strconv"
+	"sync"
 	"unsafe"
 )
 
@@ -199,6 +200,60 @@ func (r *Result) Frames(i uint32, fn func(line []byte)) (terminated bool) {
 	}
 	return segs[i].flags&C.SSE_SEG_TERMINATED != 0
 }
+
+// Telemetry is one client response's telemetry fold (sse_telemetry_*): api/middlewares/telemetry.go:190-277 evaluated from
+// the records of the upstream streams that make up the response (one at a time: a plain stream, or each iteration of an MCP
+// agent) and from the frames the handler writes itself. The batcher of the connection it is attached to feeds it while the
+// connection is open; the handler feeds it after that and finishes it once the response is written. Never concurrently.
+type Telemetry struct {
+	f    *C.sse_telemetry_fold
+	open sync.WaitGroup // connections attached and not yet closed: Finish and Free wait for none
+}
+
+func NewTelemetry() *Telemetry { return &Telemetry{f: C.sse_telemetry_new()} }
+
+// Feed folds segment i of a collected batch: the deliver step calls it for a tapped connection, after the segment's frames
+// went to the connection's channel. An error (SSE_ERR_UNDECODED: a line past the nesting limit) means the fold is short:
+// the batcher closes the stream, as for the agent fold.
+func (t *Telemetry) Feed(r *Result, i uint32) error {
+	return statusErr("sse_telemetry_feed", C.sse_telemetry_feed(t.f, &r.r, C.uint32_t(i)))
+}
+
+// FeedBytes folds frames the handler writes to the client itself: the MCP agent's error frames and its single final
+// "data: [DONE]\n\n". b must end on a '\n'.
+func (t *Telemetry) FeedBytes(b []byte) error {
+	if len(b) == 0 {
+		return nil
+	}
+	return statusErr("sse_telemetry_feed_bytes", C.sse_telemetry_feed_bytes(t.f, (*C.uint8_t)(unsafe.Pointer(&b[0])), C.size_t(len(b))))
+}
+
+// ToolCall is one merged tool call of the response (telemetry.go:268-274).
+type ToolCall struct{ ID, Type, Name, Arguments string }
+
+func goBytes(b C.sse_bytes) string { return C.GoStringN((*C.char)(unsafe.Pointer(b.p)), C.int(b.n)) }
+
+// Finish returns the response's usage (prompt, completion, total) and tool calls. irregular is true when a "\n\n" piece held
+// several lines starting with "data: " (DESIGN.md section 5, deviation 4): the figures are then not the reference's.
+// Feed nothing after it.
+func (t *Telemetry) Finish() (usage [3]int64, calls []ToolCall, irregular bool, err error) {
+	var u C.sse_usage
+	var n C.size_t
+	rc := C.sse_telemetry_finish(t.f, &u, nil, 0, &n)
+	if n > 0 {
+		arr := make([]C.sse_tool_call, int(n))
+		rc = C.sse_telemetry_finish(t.f, &u, &arr[0], n, &n)
+		for _, a := range arr[:int(n)] {
+			calls = append(calls, ToolCall{ID: goBytes(a.id), Type: goBytes(a._type), Name: goBytes(a.name), Arguments: goBytes(a.arguments)})
+		}
+	}
+	if rc < 0 {
+		return usage, nil, false, statusErr("sse_telemetry_finish", rc)
+	}
+	return [3]int64{int64(u.prompt_tokens), int64(u.completion_tokens), int64(u.total_tokens)}, calls, rc == 1, nil
+}
+
+func (t *Telemetry) Free() { C.sse_telemetry_free(t.f) }
 
 // Deferred reports whether the batch took only the first Consumed(i) bytes of segment i (SSE_FLAG_DEFER): the rest has to be
 // submitted again, first in the connection's queue.
