@@ -12,6 +12,7 @@
  *   ssegw_agent_recv and friends    mcp.Agent.RunWithStream for one iteration (mcp/agent.go:126-290, final [DONE] :140-143)
  *   ssegw_proxy_stream / _step    handleStreamingRequest, the raw /proxy/:provider/... stream loop (api/routes.go:129-232)
  *   ssegw_counters                  what the device did for the collected batches (SSE_FLAG_COUNTERS), for export as metrics
+ *   ssegw_line_pool_growth          lets the line pools grow on demand (SSE_FLAG_DEFER) instead of failing streams when full
  *   ssegw_mcp_writer_step           one turn of handleMCPStreamingRequest's writer (api/middlewares/mcp.go:253-299): the
  *                                   terminal-frame rule (:261-268) and the upstream-error sniff that may set 503 (:272-280)
  */
@@ -97,6 +98,11 @@ size_t ssegw_agent_tool_calls(ssegw *g, int stream, sse_tool_call *calls, size_t
  * the last batch's), e.g. for export as monotonic counters. SSE_ERR_ARG unless the gateway was made by ssegw_new_cfg or
  * ssegw_new_multi with a config that has the flag, or when out->struct_size != sizeof(sse_counters). */
 int    ssegw_counters(ssegw *g, sse_counters *out);
+/* sse_line_pool_set_growth(ctx, max_pages) on every context of the gateway: a gateway made by ssegw_new_cfg or ssegw_new_multi
+ * with SSE_FLAG_DEFER and a line pool lets each context's pool grow up to max_pages (0: no growth) instead of failing a stream
+ * whose line finds no free page; the stream's rest waits in its queue, like any deferred rest, until the pool has grown.
+ * Returns the first error (SSE_ERR_ARG: no gateway, no pool, no SSE_FLAG_DEFER, or max_pages below a pool's capacity). */
+int    ssegw_line_pool_growth(ssegw *g, uint32_t max_pages);
 
 /* The raw proxy stream handler (api/routes.go:129-232, taken when Accept is exactly text/event-stream, :118): reader and
  * writer in one loop, no channel in between. ssegw_proxy_stream opens the upstream body as a mode P stream (fed through

@@ -86,6 +86,9 @@ typedef struct {
                                     submits the rest (in[consumed:]) for that connection in a later batch, before any newer bytes.
                                   - tool calls / usages / decoded text: sse_collect grows the slot's arenas and decodes the batch again.
                                   sse_result.overflow reports the SSE_OVF_* bits of what was deferred or grown. Not with SSE_FLAG_KERNEL_FUSED.
+                                  - line-pool pages, on a context with a pool growth limit (sse_line_pool_set_growth) above its capacity:
+                                    a line that needs a page when none is free stops its segment at the byte that needed it (deferred
+                                    as above, the connection keeps the pages it holds) and sse_collect grows the pool (SSE_OVF_POOL).
                                   With batches in flight (n_slots > 1): a deferred rest must reach the connection before its newer bytes,
                                   so produce-side deferral is only safe while each connection is in at most one uncollected batch. Growing
                                   the decode arenas has no such limit: the batch is decoded again behind whatever was submitted since. */
@@ -164,7 +167,7 @@ typedef struct { int64_t prompt_tokens, completion_tokens, total_tokens; } sse_u
 #define SSE_SEG_LINE_TOO_LONG 0x04u /* a line exceeded carry_slot_bytes and could not continue in the line pool (longer than
                                        max_line_bytes, or no free page): stream failed, connection dead until reset */
 #define SSE_SEG_DEAD         0x08u  /* connection is in the failed state */
-#define SSE_SEG_DEFERRED     0x10u  /* SSE_FLAG_DEFER: the result arenas were full: only the first `consumed` bytes were taken */
+#define SSE_SEG_DEFERRED     0x10u  /* SSE_FLAG_DEFER: the result arenas (or a growable line pool) were full: only the first `consumed` bytes were taken */
 
 /* A run: contiguous frames/recs produced by up to 64 consecutive lines of one segment. */
 typedef struct {
@@ -196,8 +199,8 @@ typedef struct {
     const sse_seg_result *segs;
     uint32_t n_decoded, n_derived;  /* statistics: lines decoded by the automaton; n_derived is reserved (0) */
     uint32_t overflow;              /* SSE_OVF_* bits: status == SSE_ERR_OVERFLOW: which sse_config capacity to raise; with
-                                       SSE_FLAG_DEFER (status SSE_OK): what this batch deferred (OUT, RUNS) or grew and decoded again
-                                       (TCS, USAGES, TEXT); 0 when everything fit */
+                                       SSE_FLAG_DEFER (status SSE_OK): what this batch deferred (OUT, RUNS, POOL) or grew and decoded
+                                       again (TCS, USAGES, TEXT); 0 when everything fit */
     uint32_t in_base;               /* arena offsets >= in_base refer to in[off - in_base] */
     const uint8_t *in;              /* the batch's input arena (sse_batch.in_arena), lent until sse_release like out */
 } sse_result;
@@ -211,6 +214,8 @@ const uint8_t *sse_at(const sse_result *r, uint32_t off);
 #define SSE_OVF_USAGES 0x04u  /* max_usages */
 #define SSE_OVF_TEXT   0x08u  /* text_arena_bytes */
 #define SSE_OVF_RUNS   0x10u  /* max_runs */
+#define SSE_OVF_POOL   0x20u  /* line-pool pages (SSE_FLAG_DEFER with pool growth): lines deferred for want of a free page; sse_collect
+                                 grew the pool after the batch, up to the limit of sse_line_pool_set_growth */
 
 typedef struct {
     uint8_t *in_arena;     /* pinned; caller writes each segment's bytes at a 16-byte aligned in_off */
@@ -237,7 +242,9 @@ void sse_worst_case_config(sse_config *cfg, uint32_t max_conns, uint32_t bytes_p
 /* Line pool: pages in HBM shared by all connections of a context. A line that outgrows its connection's carry slot
  * continues in pool pages instead of failing the stream; its pages return to the pool when the line completes, when the
  * connection dies or finishes, and on sse_reset_conn / sse_reset_all. A connection fails (SSE_SEG_LINE_TOO_LONG |
- * SSE_SEG_DEAD) only when its line would exceed max_line_bytes or no page is free. A completed pooled line is always
+ * SSE_SEG_DEAD) only when its line would exceed max_line_bytes or no page is free (with SSE_FLAG_DEFER and a growth limit
+ * above the pool's capacity, a line that finds no free page waits for the pool to grow instead: sse_line_pool_set_growth).
+ * A completed pooled line is always
  * materialised in the out arena (never a zero-copy span). A payload of 32 KiB or more is decoded by a whole warp (a context
  * whose longest line, max_line_bytes here or carry_slot_bytes without a pool, is at least that long runs one more kernel per
  * batch, which sse_launch_count counts). Not available with SSE_FLAG_KERNEL_FUSED. */
@@ -257,6 +264,24 @@ int  sse_init_ex(int device, const sse_config *cfg, const sse_line_pool *pool, s
 void sse_line_pool_config(sse_config *cfg, const sse_line_pool *pool);
 /* Pages held by connections now and the most ever held at once; ordered after already submitted batches and resets. */
 int  sse_line_pool_stats(sse_ctx *ctx, uint32_t *pages_in_use, uint32_t *pages_high_water);
+/* Pool growth (SSE_FLAG_DEFER contexts with a line pool): max_pages is the most pages the pool may grow to, 0 = never grow (the
+ * default). While the capacity is below the limit, a line that needs a page when none is free does not fail its connection: its
+ * segment is deferred at the byte that needed the page (SSE_SEG_DEFERRED, consumed counts the bytes before it; the connection
+ * keeps the pages it holds) and the batch reports SSE_OVF_POOL. sse_collect of such a batch then grows the pool to twice its
+ * capacity or by the pages the batch's lines lacked, whichever is more, and never above the limit. The growth is ordered after
+ * every batch already submitted; later batches use the grown pool; page ids, and so held lines, are unchanged by it; the old
+ * pages are freed once no queued work can read them. At the limit a line that finds no page fails as without growth. If the
+ * device cannot allocate a larger pool, the limit becomes the current capacity. The per-batch result capacities stay those of
+ * the initial pool (sse_line_pool_config): a batch that completes more pooled bytes than they hold defers the rest.
+ * Only sse_collect grows the pool. On the device-resident path (sse_upload / sse_launch / sse_download) a line that lacks a page
+ * is deferred and its batch reports SSE_OVF_POOL as well, but the pool does not grow, so the line makes no progress there until
+ * a batch through sse_submit / sse_collect grows it; a growth is queued on the context's own stream, so a caller that launches
+ * on its own stream after an sse_collect synchronises first, as for any mix of the two paths.
+ * SSE_ERR_ARG: no context, no pool, no SSE_FLAG_DEFER, or max_pages nonzero and below the current capacity or SSE_NONE. Ordered
+ * like sse_reset_conn: after already submitted batches. */
+int  sse_line_pool_set_growth(sse_ctx *ctx, uint32_t max_pages);
+/* The pool's pages now (after every growth of the batches collected so far) and its growth limit (0: no growth). */
+int  sse_line_pool_capacity(sse_ctx *ctx, uint32_t *pages, uint32_t *max_pages);
 
 /* pipeline: acquire -> fill -> submit -> collect -> release (one slot = one batch in flight) */
 int sse_acquire(sse_ctx *ctx, int *slot, sse_batch *batch);

@@ -18,7 +18,7 @@ F_FINISH_SHIFT, F_FINISH_MASK = 12, 0x7000
 TC_HAS_ID, TC_HAS_TYPE, TC_HAS_FUNC = 0x1, 0x2, 0x4
 TC_ID_TEXT, TC_TYPE_TEXT, TC_NAME_TEXT, TC_ARGS_TEXT = 0x10, 0x20, 0x40, 0x80
 SEG_TERMINATED, SEG_FINISHED, SEG_LINE_TOO_LONG, SEG_DEAD, SEG_DEFERRED = 0x1, 0x2, 0x4, 0x8, 0x10
-OVF_OUT, OVF_TCS, OVF_USAGES, OVF_TEXT, OVF_RUNS = 0x1, 0x2, 0x4, 0x8, 0x10
+OVF_OUT, OVF_TCS, OVF_USAGES, OVF_TEXT, OVF_RUNS, OVF_POOL = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20
 
 
 class Config(C.Structure):
@@ -113,7 +113,8 @@ def counters_dict(k: Counters) -> dict:
 assert C.sizeof(Seg) == 16 and C.sizeof(Rec) == 32 and C.sizeof(Tc) == 48 and C.sizeof(SegResult) == 32
 
 EXPORTS = [
-    "sse_init", "sse_init_ex", "sse_line_pool_config", "sse_line_pool_stats", "sse_destroy", "sse_strerror", "sse_last_cuda_error", "sse_abi_version", "sse_default_config", "sse_worst_case_config",
+    "sse_init", "sse_init_ex", "sse_line_pool_config", "sse_line_pool_stats", "sse_line_pool_set_growth", "sse_line_pool_capacity",
+    "sse_destroy", "sse_strerror", "sse_last_cuda_error", "sse_abi_version", "sse_default_config", "sse_worst_case_config",
     "sse_acquire", "sse_submit", "sse_poll", "sse_collect", "sse_release", "sse_reset_conn", "sse_reset_all",
     "sse_upload", "sse_launch", "sse_download", "sse_launch_count", "sse_at", "sse_counters_read",
     "sse_agent_new", "sse_agent_free", "sse_agent_reset", "sse_agent_feed", "sse_agent_content",
@@ -145,6 +146,8 @@ def load(build_if_missing: bool = True):
     L.sse_line_pool_config.argtypes = [C.POINTER(Config), C.POINTER(LinePool)]
     L.sse_line_pool_config.restype = None
     L.sse_line_pool_stats.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
+    L.sse_line_pool_set_growth.argtypes = [vp, u32]
+    L.sse_line_pool_capacity.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
     L.sse_destroy.argtypes = [vp]
     L.sse_destroy.restype = None
     L.sse_strerror.argtypes = [i32]

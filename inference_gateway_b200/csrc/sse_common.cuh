@@ -783,6 +783,74 @@ __device__ __noinline__ uint32_t pool_grow_locked(const KParams &P, uint32_t con
     return start;
 }
 
+// SSE_FLAG_DEFER: the pages for a held-back line growing to new_len bytes (old_len of them already in pages: 0 while the line is
+// in the carry slot), taken by lane 0 under the lock as pool_append takes them, and returned to every lane: the page the next
+// bytes go to, SSE_NONE when the line fails (the connection's pages are then returned). While the pool may still grow
+// (PoolHdr.grow) too few free pages are not a failure: the line takes the pages there are and `held` becomes what they, or the
+// carry slot when that holds more (in_slot), have room for. The counting launch counts the pages taken and returned here.
+__device__ __forceinline__ uint32_t pool_reserve_defer(const KParams &P, uint32_t conn, uint32_t lane, uint32_t PB, bool leave_slot,
+                                                       uint32_t old_len, uint32_t new_len, uint32_t &held, uint32_t &in_slot) {
+    uint32_t pg = SSE_NONE;
+    if (lane == 0) {
+        const bool fits = new_len <= P.max_line;
+        const uint32_t have = (old_len + PB - 1) / PB;
+        uint32_t want = (new_len + PB - 1) / PB;
+        if (fits && have == want) {
+            pg = ((volatile PoolChain *)P.pool_chain)[conn].last;   // the bytes fit the last page (read without the lock)
+        } else if (fits || !leave_slot) {
+            pool_lock(P.pool_hdr);
+            if (fits) {
+                volatile PoolHdr *h = P.pool_hdr;
+                const uint32_t n_free = h->n_free;
+                if (want - have > n_free && h->grow) {
+                    atomicAdd(&P.ctr->pool_short, want - have - n_free);
+                    atomicOr(&P.ctr->overflow, SSE_OVF_POOL);      // reported, but the batch stays good (status untouched)
+                    want = have + n_free;
+                    held = want * PB;                             // < new_len: the line stops at a page boundary
+                    if (leave_slot && held <= P.carry_slot) { held = P.carry_slot; in_slot = 1; }   // the slot holds more
+                }
+                if (in_slot) pg = 0;
+                else if (want > have) pg = pool_grow_locked(P, conn, have, want, (old_len % PB) != 0);
+                else pg = ((volatile PoolChain *)P.pool_chain)[conn].last;   // no page free: what the last page has room for
+                if (P.cnt && pg != SSE_NONE && !in_slot && want > have) atomicAdd(P.cnt + CN_P_POOL_PAGES_TAKEN, (unsigned long long)(want - have));
+            }
+            if (pg == SSE_NONE) {
+                if (P.cnt) atomicAdd(P.cnt + CN_P_POOL_PAGES_RETURNED, (unsigned long long)((volatile PoolChain *)P.pool_chain)[conn].n_pages);
+                pool_release_locked(P, conn);
+            }
+            pool_unlock(P.pool_hdr);
+        }
+    }
+    pg = __shfl_sync(FULL, pg, 0); held = __shfl_sync(FULL, held, 0); in_slot = __shfl_sync(FULL, in_slot, 0);
+    __syncwarp();
+    return pg;
+}
+
+// Writes n_src bytes of the warp's window at src to the line's pages from page pg (where the line's next bytes go), after moving the
+// clen bytes of the carry slot to the first pages when the line leaves the slot.
+__device__ __forceinline__ void pool_write(const KParams &P, uint32_t lane, uint32_t PB, uint32_t pg, uint32_t old_len, bool leave_slot,
+                                           const uint8_t *slot, int clen, const uint8_t *src, uint32_t n_src) {
+    uint32_t off = old_len % PB;
+    if (leave_slot) {        // slot -> pages: both 16-byte aligned, whole vectors (the slot is a multiple of 16 bytes long)
+        for (uint32_t d = 0; d < (uint32_t)clen;) {
+            if (off == PB) { pg = pool_next_page(P, pg); off = 0; }
+            const uint32_t n = min(PB - off, (uint32_t)clen - d);
+            const uint4 *s = reinterpret_cast<const uint4 *>(slot + d);
+            uint4 *o = reinterpret_cast<uint4 *>(P.pool + (size_t)pg * PB);
+            for (uint32_t i = lane; i < (n + 15u) >> 4; i += 32) o[i] = s[i];
+            d += n; off += n;
+        }
+        __syncwarp();        // the vector tail past clen is overwritten below
+    }
+    for (uint32_t d = 0; d < n_src;) {
+        if (off == PB) { pg = pool_next_page(P, pg); off = 0; }
+        const uint32_t n = min(PB - off, n_src - d);
+        copy_s2g_vec(P.pool + (size_t)pg * PB + off, src + d, (int)n);
+        d += n; off += n;
+    }
+    __syncwarp();
+}
+
 // Cold path of a line that outgrows the carry slot. The held-back line (clen bytes: in the slot while clen <= carry_slot,
 // else all of them in pool pages) grows by `take` bytes of the warp's window at src. Takes the pages the longer line needs,
 // moves the slot bytes to the first page when the line leaves the slot, appends. Fails, and returns the connection's pages,
@@ -810,26 +878,30 @@ __device__ __noinline__ bool pool_append(const KParams &P, uint32_t conn, const 
     pg = __shfl_sync(FULL, pg, 0);
     __syncwarp();
     if (pg == SSE_NONE) return false;
-    uint32_t off = old_len % PB;
-    if (leave_slot) {        // slot -> pages: both 16-byte aligned, whole vectors (the slot is a multiple of 16 bytes long)
-        for (uint32_t d = 0; d < (uint32_t)clen;) {
-            if (off == PB) { pg = pool_next_page(P, pg); off = 0; }
-            const uint32_t n = min(PB - off, (uint32_t)clen - d);
-            const uint4 *s = reinterpret_cast<const uint4 *>(slot + d);
-            uint4 *o = reinterpret_cast<uint4 *>(P.pool + (size_t)pg * PB);
-            for (uint32_t i = lane; i < (n + 15u) >> 4; i += 32) o[i] = s[i];
-            d += n; off += n;
-        }
-        __syncwarp();        // the vector tail past clen is overwritten below
-    }
-    for (uint32_t d = 0; d < (uint32_t)take;) {
-        if (off == PB) { pg = pool_next_page(P, pg); off = 0; }
-        const uint32_t n = min(PB - off, (uint32_t)take - d);
-        copy_s2g_vec(P.pool + (size_t)pg * PB + off, src + d, (int)n);
-        d += n; off += n;
-    }
-    __syncwarp();
+    pool_write(P, lane, PB, pg, old_len, leave_slot, slot, clen, src, (uint32_t)take);
     return true;
+}
+
+// SSE_FLAG_DEFER: pool_append for the deferring produce kernel. While the pool may still grow (PoolHdr.grow) a line that finds
+// too few free pages is not failed: it takes the pages there are and holds what they, or the carry slot when that holds more,
+// have room for; the pages it lacked go to Counters.pool_short with SSE_OVF_POOL, and sse_collect grows the pool. Returns the
+// bytes of src held: take, or fewer (the caller defers the segment at the first byte not held, and the connection keeps its
+// pages), or -1 when the line fails as pool_append fails it: longer than max_line, or too few free pages in a pool that
+// cannot grow.
+__device__ __noinline__ int pool_append_defer(const KParams &P, uint32_t conn, uint8_t *slot, int clen, const uint8_t *src, int take) {
+    if (take == 0) return 0;
+    const uint32_t lane = lane_id(), PB = P.page_bytes;
+    const bool leave_slot = clen <= (int)P.carry_slot;
+    const uint32_t old_len = leave_slot ? 0u : (uint32_t)clen, new_len = (uint32_t)clen + (uint32_t)take;
+    uint32_t held = new_len, in_slot = 0;     // held: the line's length after the call
+    const uint32_t pg = pool_reserve_defer(P, conn, lane, PB, leave_slot, old_len, new_len, held, in_slot);
+    if (pg == SSE_NONE) return -1;
+    const uint32_t got = held - (uint32_t)clen;
+    if (in_slot) {           // the line stays in the carry slot, filled to its end
+        copy_s2g_bytes(slot + clen, src, (int)got);
+        __syncwarp();
+    } else pool_write(P, lane, PB, pg, old_len, leave_slot, slot, clen, src, got);
+    return (int)got;
 }
 
 // A pooled line is complete (its last byte, the '\n', was appended): gathered from its pages into the out arena with 16-byte
@@ -864,6 +936,12 @@ __device__ __forceinline__ bool hold_back(const KParams &P, uint32_t conn, uint8
     if (clen + take > (int)P.carry_slot) return pool_append(P, conn, slot, clen, src, take);
     copy_s2g_bytes(slot + clen, src, take);
     return true;
+}
+// SSE_FLAG_DEFER: hold_back with pool_append_defer's result: the bytes held (take or fewer), -1 when the line fails.
+__device__ __forceinline__ int hold_back_defer(const KParams &P, uint32_t conn, uint8_t *slot, int clen, const uint8_t *src, int take) {
+    if (clen + take > (int)P.carry_slot) return pool_append_defer(P, conn, slot, clen, src, take);
+    copy_s2g_bytes(slot + clen, src, take);
+    return take;
 }
 
 // SSE_FLAG_DEFER: the held line of clen bytes gives back its last byte, the '\n' just appended, so that the connection's state

@@ -11,7 +11,7 @@
 // line pool (sse_init_ex, optional; one per context):
 //   pool        u8[pool_pages*page_bytes]  pages holding lines longer than the carry slot, page k = bytes [k*page_bytes, ...)
 //                                          of the line in chain order
-//   pool_hdr    PoolHdr                    lock + free-stack height + high-water mark
+//   pool_hdr    PoolHdr                    lock + free-stack height + high-water mark + whether the pool may still grow
 //   pool_stack  u32[pool_pages]            free pages: pool_stack[0 .. n_free)
 //   pool_next   u32[pool_pages]            next page of the same chain
 //   pool_chain  PoolChain[max_conns]       per connection: first / last page, pages held (0: none)
@@ -28,7 +28,8 @@ struct PoolHdr {
     uint32_t lock;         // taken by one lane around every allocation / release (pages move rarely: one per page_bytes of a long line)
     uint32_t n_free;
     uint32_t high_water;   // most pages ever held at once
-    uint32_t pad;
+    uint32_t grow;         // nonzero: the pool may still grow (sse_line_pool_set_growth, below the limit): a line of the SSE_FLAG_DEFER
+                           // produce kernel that finds too few free pages defers instead of failing its connection
 };
 struct PoolChain {
     uint32_t first, last, n_pages, pad;
@@ -57,7 +58,7 @@ struct alignas(8) Counters {
     int32_t  status;
     uint32_t item_ticket;  // split pipeline: next item batch for the decode kernel
     uint32_t n_tiles;      // fused pipeline: tiles written by the plan kernel
-    uint32_t reserved1;
+    uint32_t pool_short;   // SSE_FLAG_DEFER with pool growth: pages lines of this batch asked for and did not find (SSE_OVF_POOL)
     uint32_t overflow;     // SSE_OVF_* bits: which arena was too small (SSE_FLAG_DEFER: also what the produce stage deferred)
     uint32_t n_long;       // split pipeline: work items of at least KParams.long_line payload bytes (items_sorted[0, n_long))
     uint32_t long_ticket;  // split pipeline: next long item for the long-line decode kernel
@@ -155,6 +156,7 @@ int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count);    
 int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device);  // split pipeline, stages 2+3
 int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device);           // SSE_FLAG_DEFER: stage 2 again (grown arenas)
 int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream);              // line pool: reset one connection (SSE_NONE: all)
+int sse_launch_pool_extend(const KParams &p, uint32_t old_pages, bool grow, void *stream); // line pool: pages [old_pages, pool_pages) free
 namespace ssetab { struct DfaTables; }
 int sse_build_tables(ssetab::DfaTables &T);                                            // the decode tables of the schema (host)
 int sse_v2_prepare(int device);                                                        // builds + uploads the automaton tables

@@ -356,6 +356,15 @@ int ssegw_counters(ssegw *g, sse_counters *out) {
     return SSE_OK;
 }
 
+int ssegw_line_pool_growth(ssegw *g, uint32_t max_pages) {
+    if (!g) return SSE_ERR_ARG;
+    for (auto &x : g->ctxs) {
+        const int rc = sse_line_pool_set_growth(x.ctx, max_pages);
+        if (rc != SSE_OK) return rc;
+    }
+    return SSE_OK;
+}
+
 // ---- handleStreamingRequest (api/routes.go:129-232): the raw proxy loop reads and writes in one goroutine
 int ssegw_proxy_stream(ssegw *g) { return ssegw_stream_chat_completions(g, SSE_MODE_P); }
 int ssegw_proxy_step(ssegw *g, int id, uint8_t *buf, size_t cap, size_t *n) {

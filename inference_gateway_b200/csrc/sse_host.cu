@@ -58,6 +58,14 @@ struct Slot {
     uint32_t decode_passes = 0;
     bool cnt_ready = false;                                    // h_cnt holds the counters of the batch last downloaded
     bool ctr_queued = false;                                   // sse_submit queued the D2H of h_ctr (do_download does not)
+    uint32_t pool_short = 0;                                   // SSE_OVF_POOL: pages the collected batch's lines lacked
+    uint32_t pool_gen = 0;                                     // sse_ctx.pool_gen when the batch was launched
+};
+
+// Line-pool arrays replaced by a growth, freed once the event recorded after their last reader has completed.
+struct RetiredPool {
+    uint8_t *pool; uint32_t *stack, *next;
+    cudaEvent_t done;
 };
 
 } // namespace
@@ -77,6 +85,9 @@ struct sse_ctx {
     uint8_t *d_pool = nullptr; PoolHdr *d_pool_hdr = nullptr; uint32_t *d_pool_stack = nullptr, *d_pool_next = nullptr;
     PoolChain *d_pool_chain = nullptr;
     PoolHdr *h_pool_hdr = nullptr;       // pinned: sse_line_pool_stats
+    uint32_t pool_max = 0;               // sse_line_pool_set_growth: most pages the pool may grow to (0: no growth)
+    std::vector<RetiredPool> retired;    // pool arrays a growth replaced, until no queued work can read them
+    uint32_t pool_gen = 0;               // growths so far
     cudaStream_t ctl_stream = nullptr;
     cudaEvent_t last_kernel = nullptr;   // completion of the most recently launched kernel
     bool have_last = false;
@@ -154,6 +165,7 @@ int do_upload(sse_ctx *c, Slot &s, uint32_t n_segs, uint32_t in_bytes, cudaStrea
 int do_launch(sse_ctx *c, Slot &s, uint32_t n_segs, cudaStream_t st) {
     CU(cudaMemsetAsync(s.d_ctr, 0, sizeof(Counters), st));
     s.cnt_ready = false;
+    s.pool_gen = c->pool_gen;
     if (s.d_cnt) CU(cudaMemsetAsync(s.d_cnt, 0, CN_COUNT * sizeof(unsigned long long), st));
     if (n_segs) {
         KParams p = make_params(c, s, n_segs);
@@ -258,6 +270,7 @@ int do_download(sse_ctx *c, Slot &s, sse_result *res, cudaStream_t st) {
     s.ctr_queued = false;
     CU(cudaStreamSynchronize(st));
     Counters k = *s.h_ctr;
+    s.pool_short = k.pool_short;
     memset(res, 0, sizeof *res);
     res->n_segs = s.n_segs;
     s.decode_passes = s.n_segs ? 1u : 0u;
@@ -296,6 +309,63 @@ int do_download(sse_ctx *c, Slot &s, sse_result *res, cudaStream_t st) {
     res->out = s.h_out; res->frames = s.h_frames; res->recs = s.h_recs; res->tcs = s.h_tcs; res->usages = s.h_usages;
     res->text = s.h_text; res->runs = s.h_runs; res->segs = s.h_segres;
     res->in = s.h_in; res->in_base = in_base_of(c->cfg);
+    return SSE_OK;
+}
+
+// Frees the retired pool arrays whose last reader has completed (all: every one, the device being idle).
+void free_retired(sse_ctx *c, bool all) {
+    size_t k = 0;
+    for (RetiredPool &r : c->retired) {
+        if (!all) {
+            const cudaError_t e = cudaEventQuery(r.done);
+            if (e == cudaErrorNotReady && cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();   // still queued: not an error
+            if (e != cudaSuccess) { c->retired[k++] = r; continue; }
+        }
+        cudaFree(r.pool); cudaFree(r.stack); cudaFree(r.next); cudaEventDestroy(r.done);
+    }
+    c->retired.resize(k);
+}
+
+// SSE_FLAG_DEFER with pool growth: a batch's lines lacked `lacked` pages. The pool grows to twice its pages, or by what was
+// lacked when that is more, at most to pool_max. The new arrays start with copies of the old ones, so page ids, chains and held
+// lines stay as they are; the copies and the kernel that frees the new pages are ordered after every submitted batch (which
+// were launched with the old arrays) and every later launch is ordered after them and gets the new arrays. When the device
+// cannot allocate them the pool stays as it is and stops growing: its lines fail at the limit as without growth.
+int grow_pool(sse_ctx *c, uint32_t lacked) {
+    const uint32_t cap = c->pool.pool_pages, PB = c->pool.page_bytes;
+    uint64_t want = (uint64_t)cap * 2u;
+    if (want < (uint64_t)cap + lacked) want = (uint64_t)cap + lacked;
+    if (want > c->pool_max) want = c->pool_max;
+    if (want <= cap) return SSE_OK;
+    free_retired(c, false);
+    RetiredPool old{ c->d_pool, c->d_pool_stack, c->d_pool_next, nullptr };
+    uint8_t *pool = nullptr; uint32_t *stack = nullptr, *next = nullptr;
+    bool ok = cudaMalloc((void **)&pool, (size_t)want * PB) == cudaSuccess && cudaMalloc((void **)&stack, (size_t)want * 4) == cudaSuccess &&
+              cudaMalloc((void **)&next, (size_t)want * 4) == cudaSuccess &&
+              cudaEventCreateWithFlags(&old.done, cudaEventDisableTiming) == cudaSuccess;
+    if (!ok) {
+        if (cudaPeekAtLastError() == cudaErrorMemoryAllocation) cudaGetLastError();   // the failed allocation only
+        cudaFree(pool); cudaFree(stack); cudaFree(next);
+        if (old.done) cudaEventDestroy(old.done);
+        c->pool_max = cap;
+        if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
+        CU(cudaMemsetAsync(&c->d_pool_hdr->grow, 0, sizeof(uint32_t), c->ctl_stream));
+        CU(cudaEventRecord(c->last_kernel, c->ctl_stream));
+        c->have_last = true;
+        return SSE_OK;
+    }
+    cudaStream_t st = c->ctl_stream;
+    if (c->have_last) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
+    CU(cudaMemcpyAsync(pool, c->d_pool, (size_t)cap * PB, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(stack, c->d_pool_stack, (size_t)cap * 4, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(next, c->d_pool_next, (size_t)cap * 4, cudaMemcpyDeviceToDevice, st));
+    CU(cudaEventRecord(old.done, st));
+    c->retired.push_back(old);
+    c->d_pool = pool; c->d_pool_stack = stack; c->d_pool_next = next; c->pool.pool_pages = (uint32_t)want;
+    c->pool_gen++;
+    if (!cu_ok((cudaError_t)sse_launch_pool_extend(pool_params(c), cap, want < c->pool_max, st), "pool extend kernel")) return SSE_ERR_CUDA;
+    CU(cudaEventRecord(c->last_kernel, st));
+    c->have_last = true;
     return SSE_OK;
 }
 
@@ -466,6 +536,7 @@ void sse_destroy(sse_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
+    free_retired(c, true);
     for (auto &s : c->slots) free_slot(s);
     cudaFree(c->d_conns); cudaFree(c->d_carry); cudaFree(c->d_tcache);
     cudaFree(c->d_pool); cudaFree(c->d_pool_hdr); cudaFree(c->d_pool_stack); cudaFree(c->d_pool_next); cudaFree(c->d_pool_chain);
@@ -530,6 +601,9 @@ int sse_collect(sse_ctx *c, int slot, sse_result *res) {
     CU(cudaSetDevice(c->device));
     int rc = do_download(c, s, res, s.stream);
     s.state = SLOT_COLLECTED;
+    // a batch launched before the last growth measured its lack against the smaller pool: its lines try the grown one first
+    if (rc == SSE_OK && (res->overflow & SSE_OVF_POOL) && s.pool_gen == c->pool_gen) rc = grow_pool(c, s.pool_short);
+    else if (!c->retired.empty()) free_retired(c, false);
     return rc;
 }
 
@@ -576,6 +650,25 @@ int sse_line_pool_stats(sse_ctx *c, uint32_t *pages_in_use, uint32_t *pages_high
     CU(cudaStreamSynchronize(c->ctl_stream));
     *pages_in_use = c->pool.pool_pages - c->h_pool_hdr->n_free;
     *pages_high_water = c->h_pool_hdr->high_water;
+    return SSE_OK;
+}
+
+int sse_line_pool_set_growth(sse_ctx *c, uint32_t max_pages) {
+    if (!c || !c->pool.pool_pages || !(c->cfg.flags & SSE_FLAG_DEFER) || max_pages == SSE_NONE ||
+        (max_pages && max_pages < c->pool.pool_pages)) return SSE_ERR_ARG;
+    CU(cudaSetDevice(c->device));
+    c->pool_max = max_pages;
+    if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
+    CU(cudaMemsetAsync(&c->d_pool_hdr->grow, max_pages > c->pool.pool_pages ? 1 : 0, sizeof(uint32_t), c->ctl_stream));
+    CU(cudaEventRecord(c->last_kernel, c->ctl_stream));   // later kernels see the new setting
+    c->have_last = true;
+    return SSE_OK;
+}
+
+int sse_line_pool_capacity(sse_ctx *c, uint32_t *pages, uint32_t *max_pages) {
+    if (!c || !pages || !max_pages) return SSE_ERR_ARG;
+    *pages = c->pool.pool_pages;
+    *max_pages = c->pool_max;
     return SSE_OK;
 }
 

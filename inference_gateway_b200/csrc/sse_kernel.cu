@@ -151,12 +151,23 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
                 }
                 int take = (q < 0) ? (fill - base) : (q - base + 1);
                 uint32_t pages = 0;
-                if constexpr (CNT) pages = pool_held(P, conn);
-                const bool held = hold_back(P, conn, slot, clen, buf + base, take);
-                if constexpr (CNT) tally_pages(T, pages, pool_held(P, conn));
-                if (!held) { dead = true; break; }
-                clen += take;
-                __syncwarp();
+                if constexpr (DEFER) {      // (the counting instantiation counts pages inside pool_append_defer)
+                    const int got = hold_back_defer(P, conn, slot, clen, buf + base, take);
+                    if (got < 0) { dead = true; break; }
+                    clen += got;
+                    __syncwarp();
+                    if (got < take) {        // no page for the rest: the segment stops at the first byte the line could not hold
+                        consumed = (q < 0 ? fill : q + 1) - (take - got) + in_delta;   // base + got (base is not kept)
+                        overflow = true; break;
+                    }
+                } else {
+                    if constexpr (CNT) pages = pool_held(P, conn);
+                    const bool held = hold_back(P, conn, slot, clen, buf + base, take);
+                    if constexpr (CNT) tally_pages(T, pages, pool_held(P, conn));
+                    if (!held) { dead = true; break; }
+                    clen += take;
+                    __syncwarp();
+                }
                 if (q < 0) {
                     pend = 0;
                     if (consumed >= in_len) break;

@@ -638,6 +638,15 @@ __global__ void sse_pool_reset_kernel(const __grid_constant__ KParams P, uint32_
     if (tid == 0) { P.pool_hdr->lock = 0; P.pool_hdr->n_free = P.pool_pages; }
 }
 
+// Line pool growth: the pool's arrays were reallocated with pool_pages pages and the first old_pages copied over (page ids and
+// chains are unchanged); the new pages go on top of the free stack. One block: every thread reads n_free before any writes it.
+__global__ void sse_pool_extend_kernel(const __grid_constant__ KParams P, uint32_t old_pages, uint32_t grow) {
+    const uint32_t n = P.pool_hdr->n_free;
+    for (uint32_t i = threadIdx.x; i < P.pool_pages - old_pages; i += blockDim.x) P.pool_stack[n + i] = old_pages + i;
+    __syncthreads();
+    if (threadIdx.x == 0) { P.pool_hdr->n_free = n + (P.pool_pages - old_pages); P.pool_hdr->grow = grow; }
+}
+
 DfaTables *g_tables_dev[16] = { nullptr };
 
 } // namespace
@@ -722,5 +731,10 @@ int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream) {
     const uint32_t n = p.pool_pages > p.max_conns ? p.pool_pages : p.max_conns;
     const uint32_t grid = conn != SSE_NONE ? 1u : (n + 255u) / 256u < 1024u ? (n + 255u) / 256u : 1024u;
     sse_pool_reset_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, conn);
+    return (int)cudaGetLastError();
+}
+
+int sse_launch_pool_extend(const KParams &p, uint32_t old_pages, bool grow, void *stream) {
+    sse_pool_extend_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(p, old_pages, grow ? 1u : 0u);
     return (int)cudaGetLastError();
 }

@@ -107,14 +107,17 @@ def make_line_pool(pool_pages: int, page_bytes: int = 0, max_line_bytes: int = A
 class SseEngine:
     def __init__(self, device: int = 0, max_conns: int = 1024, bytes_per_batch: int = 1 << 20, line_pool: dict | None = None,
                  **overrides):
-        """line_pool: keyword arguments of make_line_pool() (pool_pages, page_bytes, max_line_bytes), or None for no pool:
-        a line longer than carry_slot_bytes then fails its connection."""
+        """line_pool: keyword arguments of make_line_pool() (pool_pages, page_bytes, max_line_bytes), and optionally max_pages
+        (sse_line_pool_set_growth: with flags=FLAG_DEFER the pool grows on demand up to that many pages instead of failing
+        a line that finds no free page), or None for no pool: a line longer than carry_slot_bytes then fails its connection."""
         self.L = A.load()
         cfg = A.Config()
         self.L.sse_default_config(C.byref(cfg), max_conns, bytes_per_batch)
         for k, v in overrides.items():
             setattr(cfg, k, v)
         self._ctx = C.c_void_p()
+        line_pool = dict(line_pool) if line_pool is not None else None
+        max_pages = line_pool.pop("max_pages", 0) if line_pool is not None else 0
         self.pool = make_line_pool(**line_pool) if line_pool is not None else None
         pp = C.byref(self.pool) if self.pool is not None else None
         A.check(self.L.sse_init_ex(device, C.byref(cfg), pp, C.byref(self._ctx)), "sse_init_ex")
@@ -122,6 +125,18 @@ class SseEngine:
             self.L.sse_line_pool_config(C.byref(cfg), pp)   # the capacities the context allocated
         self.cfg = cfg
         self.device = device
+        if max_pages:
+            self.line_pool_growth(max_pages)
+
+    def line_pool_growth(self, max_pages: int):
+        """sse_line_pool_set_growth: the pool may grow up to max_pages pages (0: never), ordered after the batches submitted."""
+        A.check(self.L.sse_line_pool_set_growth(self._ctx, max_pages), "sse_line_pool_set_growth")
+
+    def line_pool_capacity(self):
+        """(pages, growth limit) of the line pool: its pages after the growths of the batches collected so far; limit 0: none."""
+        pages, limit = C.c_uint32(), C.c_uint32()
+        A.check(self.L.sse_line_pool_capacity(self._ctx, C.byref(pages), C.byref(limit)), "sse_line_pool_capacity")
+        return pages.value, limit.value
 
     def pool_stats(self):
         """(pages in use, high-water mark) of the line pool, after every batch submitted so far."""

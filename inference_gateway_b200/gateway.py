@@ -49,7 +49,8 @@ class Gateway:
     def __init__(self, device: int = 0, max_conns: int = 256, bytes_per_batch: int = 1 << 20, line_pool: dict | None = None,
                  config: A.Config | None = None, devices: list[int] | None = None, depth: int = 1):
         """line_pool: keyword arguments of engine.make_line_pool() (pool_pages, page_bytes, max_line_bytes): lines longer than the
-        64 KiB carry slot continue in a shared device page pool instead of failing their stream.
+        64 KiB carry slot continue in a shared device page pool instead of failing their stream. max_pages in it
+        (ssegw_line_pool_growth; a config with FLAG_DEFER) lets every context's pool grow on demand up to that many pages.
         config: an sse_config to run on (ssegw_new_cfg; max_conns and bytes_per_batch are then ignored), e.g. default capacities
         with FLAG_DEFER; None: the worst-case config.
         devices, depth: one context per entry of devices (a device may repeat), each with up to depth (1 .. config.n_slots)
@@ -90,7 +91,10 @@ class Gateway:
         L.ssegw_agent_tool_calls.argtypes = [vp, i32, C.POINTER(A.ToolCall), C.c_size_t]
         L.ssegw_agent_tool_calls.restype = C.c_size_t
         L.ssegw_counters.argtypes = [vp, C.POINTER(A.Counters)]
+        L.ssegw_line_pool_growth.argtypes = [vp, C.c_uint32]
         st = i32()
+        line_pool = dict(line_pool) if line_pool is not None else None
+        max_pages = line_pool.pop("max_pages", 0) if line_pool is not None else 0
         self._pool = make_line_pool(**line_pool) if line_pool is not None else None
         if devices is not None or depth != 1:
             if config is None:
@@ -107,6 +111,12 @@ class Gateway:
             self.g = L.ssegw_new_ex(device, max_conns, bytes_per_batch, C.byref(self._pool), C.byref(st))
         if not self.g:
             raise A.SseError(st.value, "ssegw_new")
+        if max_pages:
+            rc = L.ssegw_line_pool_growth(self.g, max_pages)
+            if rc != A.SSE_OK:
+                L.ssegw_free(self.g)
+                self.g = None
+                raise A.SseError(rc, "ssegw_line_pool_growth")
         self._buf = C.create_string_buffer(1 << 20)
         self._taps = {}          # stream id -> the Telemetry it feeds, kept alive until the stream is released
 

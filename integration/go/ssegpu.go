@@ -55,6 +55,9 @@ func envUint32(name string) uint32 {
 // GPU_LINE_POOL_PAGES > 0 gives the context a line pool of that many pages (GPU_LINE_POOL_PAGE_BYTES each, default 64 KiB),
 // shared by all connections: a line longer than the carry slot continues there instead of failing its stream, up to
 // GPU_LINE_POOL_MAX_LINE bytes per connection (default and ceiling SSE_MAX_LINE_BYTES, 16 MiB - 1).
+// GPU_LINE_POOL_MAX_PAGES > GPU_LINE_POOL_PAGES lets the pool grow on demand up to that many pages
+// (sse_line_pool_set_growth): a line that finds no free page waits as a deferred rest while the pool grows, instead of
+// failing its stream. It requires GPU_DEFER=1.
 //
 // GPU_COUNTERS=1 sets SSE_FLAG_COUNTERS: the counting kernels run and Counters(slot) reports what they did for each batch
 // (INTEGRATION.md section 2 maps the fields to metric names).
@@ -88,6 +91,16 @@ func NewContext(device int, maxConns, bytesPerBatch, nSlots uint32) (*Context, e
 		if err := statusErr("sse_init_ex", C.sse_init_ex(C.int(device), &cfg, &pool, &ctx)); err != nil {
 			return nil, err
 		}
+		if maxPages := envUint32("GPU_LINE_POOL_MAX_PAGES"); maxPages > 0 {
+			if cfg.flags&C.SSE_FLAG_DEFER == 0 {
+				C.sse_destroy(ctx)
+				return nil, errors.New("GPU_LINE_POOL_MAX_PAGES requires GPU_DEFER=1")
+			}
+			if err := statusErr("sse_line_pool_set_growth", C.sse_line_pool_set_growth(ctx, C.uint32_t(maxPages))); err != nil {
+				C.sse_destroy(ctx)
+				return nil, err
+			}
+		}
 		return &Context{c: ctx}, nil
 	}
 	if err := statusErr("sse_init", C.sse_init(C.int(device), &cfg, &ctx)); err != nil {
@@ -110,6 +123,14 @@ func (x *Context) LinePoolStats() (inUse, highWater uint32, err error) {
 	var u, h C.uint32_t
 	err = statusErr("sse_line_pool_stats", C.sse_line_pool_stats(x.c, &u, &h))
 	return uint32(u), uint32(h), err
+}
+
+// LinePoolCapacity returns the line pool's pages now (after the growths of the batches collected so far) and its growth
+// limit (0: no growth).
+func (x *Context) LinePoolCapacity() (pages, maxPages uint32, err error) {
+	var p, m C.uint32_t
+	err = statusErr("sse_line_pool_capacity", C.sse_line_pool_capacity(x.c, &p, &m))
+	return uint32(p), uint32(m), err
 }
 
 func (x *Context) Close() { C.sse_destroy(x.c) }
