@@ -13,6 +13,7 @@
  *   ssegw_proxy_stream / _step    handleStreamingRequest, the raw /proxy/:provider/... stream loop (api/routes.go:129-232)
  *   ssegw_counters                  what the device did for the collected batches (SSE_FLAG_COUNTERS), for export as metrics
  *   ssegw_line_pool_growth          lets the line pools grow on demand (SSE_FLAG_DEFER) instead of failing streams when full
+ *   ssegw_trim                      gives back what that growth, and the growth of the decode arenas, took
  *   ssegw_mcp_writer_step           one turn of handleMCPStreamingRequest's writer (api/middlewares/mcp.go:253-299): the
  *                                   terminal-frame rule (:261-268) and the upstream-error sniff that may set 503 (:272-280)
  */
@@ -103,6 +104,11 @@ int    ssegw_counters(ssegw *g, sse_counters *out);
  * whose line finds no free page; the stream's rest waits in its queue, like any deferred rest, until the pool has grown.
  * Returns the first error (SSE_ERR_ARG: no gateway, no pool, no SSE_FLAG_DEFER, or max_pages below a pool's capacity). */
 int    ssegw_line_pool_growth(ssegw *g, uint32_t max_pages);
+/* sse_trim(ctx, min_pool_pages) on every context of the gateway: gives back the line-pool pages and decode arenas that growth
+ * took (SSE_FLAG_DEFER), e.g. on the operator's timer after a burst. Streams holding lines go on unchanged; batches in flight are
+ * waited for on the device, collected by later pumps as usual, and their slots' arenas shrink when they are released. Returns
+ * the first error (SSE_ERR_ARG: no gateway, a config without SSE_FLAG_DEFER, or min_pool_pages == SSE_NONE). */
+int    ssegw_trim(ssegw *g, uint32_t min_pool_pages);
 
 /* The raw proxy stream handler (api/routes.go:129-232, taken when Accept is exactly text/event-stream, :118): reader and
  * writer in one loop, no channel in between. ssegw_proxy_stream opens the upstream body as a mode P stream (fed through

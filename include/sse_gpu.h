@@ -84,7 +84,8 @@ typedef struct {
                                     fit; its connection state describes exactly the bytes before that point, the segment is flagged
                                     SSE_SEG_DEFERRED and sse_seg_result.consumed tells how many of its bytes the batch took. The caller
                                     submits the rest (in[consumed:]) for that connection in a later batch, before any newer bytes.
-                                  - tool calls / usages / decoded text: sse_collect grows the slot's arenas and decodes the batch again.
+                                  - tool calls / usages / decoded text: sse_collect grows the slot's arenas and decodes the batch again
+                                    (they stay grown until sse_trim).
                                   sse_result.overflow reports the SSE_OVF_* bits of what was deferred or grown. Not with SSE_FLAG_KERNEL_FUSED.
                                   - line-pool pages, on a context with a pool growth limit (sse_line_pool_set_growth) above its capacity:
                                     a line that needs a page when none is free stops its segment at the byte that needed it (deferred
@@ -262,7 +263,8 @@ int  sse_init_ex(int device, const sse_config *cfg, const sse_line_pool *pool, s
  * config already has (a worst-case config stays overflow-free, a default one stays sized for realistic traffic). A NULL or
  * zero-page pool leaves cfg unchanged. */
 void sse_line_pool_config(sse_config *cfg, const sse_line_pool *pool);
-/* Pages held by connections now and the most ever held at once; ordered after already submitted batches and resets. */
+/* Pages held by connections now and the most ever held at once; ordered after already submitted batches and resets. The
+ * high-water mark is never lowered, so after sse_trim it may exceed the pool's capacity. */
 int  sse_line_pool_stats(sse_ctx *ctx, uint32_t *pages_in_use, uint32_t *pages_high_water);
 /* Pool growth (SSE_FLAG_DEFER contexts with a line pool): max_pages is the most pages the pool may grow to, 0 = never grow (the
  * default). While the capacity is below the limit, a line that needs a page when none is free does not fail its connection: its
@@ -280,8 +282,26 @@ int  sse_line_pool_stats(sse_ctx *ctx, uint32_t *pages_in_use, uint32_t *pages_h
  * SSE_ERR_ARG: no context, no pool, no SSE_FLAG_DEFER, or max_pages nonzero and below the current capacity or SSE_NONE. Ordered
  * like sse_reset_conn: after already submitted batches. */
 int  sse_line_pool_set_growth(sse_ctx *ctx, uint32_t max_pages);
-/* The pool's pages now (after every growth of the batches collected so far) and its growth limit (0: no growth). */
+/* The pool's pages now (after every growth of the batches collected so far, and every sse_trim) and its growth limit (0: no growth). */
 int  sse_line_pool_capacity(sse_ctx *ctx, uint32_t *pages, uint32_t *max_pages);
+/* Give back what on-demand growth (SSE_FLAG_DEFER) took. Returns once the old memory is freed.
+ *   Line pool (only with a growth limit: a pool without one never grew): the pool shrinks to max(min_pool_pages, pages held
+ *     now, 1) pages when that is below its capacity, else it stays as it is. The held pages move to the first pages of the new
+ *     pool on the device, in chain order; lines held across the trim go on byte for byte as if nothing happened, and
+ *     sse_line_pool_stats' pages in use is unchanged. The pool grows again on demand, up to its limit.
+ *   Decode arenas: each slot's tool-call, usage and text arenas, device and pinned, go back to the config's capacities: at once
+ *     for a free slot, at its sse_release for a slot that holds a batch (its results may still be lent to the caller).
+ * Ordered like sse_reset_conn: after every batch already submitted, whose completion on the device it waits for; it does not
+ * collect them, and their results, which do not refer to pool pages, are collected afterwards as usual. A batch submitted
+ * before the trim that reports SSE_OVF_POOL does not grow the trimmed pool (its lines try it first, as after a growth). On the
+ * device-resident path (sse_upload / sse_launch / sse_download) the caller synchronises its own streams before the trim, as for
+ * any mix of the two paths.
+ * SSE_ERR_ARG: no context, no SSE_FLAG_DEFER, or min_pool_pages == SSE_NONE. SSE_ERR_NOMEM: the device could not allocate the
+ * smaller pool (it stays as it was). */
+int  sse_trim(sse_ctx *ctx, uint32_t min_pool_pages);
+/* Device and pinned bytes the context holds now: every allocation, slots, pool and grown arenas included (and a growth's old
+ * pool arrays until they are freed, at the next sse_collect or sse_trim). SSE_ERR_ARG, writing nothing, for a NULL argument. */
+int  sse_memory_held(sse_ctx *ctx, uint64_t *device_bytes, uint64_t *pinned_bytes);
 
 /* pipeline: acquire -> fill -> submit -> collect -> release (one slot = one batch in flight) */
 int sse_acquire(sse_ctx *ctx, int *slot, sse_batch *batch);

@@ -114,6 +114,7 @@ assert C.sizeof(Seg) == 16 and C.sizeof(Rec) == 32 and C.sizeof(Tc) == 48 and C.
 
 EXPORTS = [
     "sse_init", "sse_init_ex", "sse_line_pool_config", "sse_line_pool_stats", "sse_line_pool_set_growth", "sse_line_pool_capacity",
+    "sse_trim", "sse_memory_held",
     "sse_destroy", "sse_strerror", "sse_last_cuda_error", "sse_abi_version", "sse_default_config", "sse_worst_case_config",
     "sse_acquire", "sse_submit", "sse_poll", "sse_collect", "sse_release", "sse_reset_conn", "sse_reset_all",
     "sse_upload", "sse_launch", "sse_download", "sse_launch_count", "sse_at", "sse_counters_read",
@@ -148,6 +149,8 @@ def load(build_if_missing: bool = True):
     L.sse_line_pool_stats.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
     L.sse_line_pool_set_growth.argtypes = [vp, u32]
     L.sse_line_pool_capacity.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
+    L.sse_trim.argtypes = [vp, u32]
+    L.sse_memory_held.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.sse_destroy.argtypes = [vp]
     L.sse_destroy.restype = None
     L.sse_strerror.argtypes = [i32]

@@ -157,6 +157,9 @@ int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int
 int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device);           // SSE_FLAG_DEFER: stage 2 again (grown arenas)
 int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream);              // line pool: reset one connection (SSE_NONE: all)
 int sse_launch_pool_extend(const KParams &p, uint32_t old_pages, bool grow, void *stream); // line pool: pages [old_pages, pool_pages) free
+// line pool trim: the held pages of p's idle pool repacked into the first `held` pages of new arrays of `pages` pages
+int sse_launch_pool_repack(const KParams &p, uint8_t *pool, uint32_t *stack, uint32_t *next, uint32_t held, uint32_t pages, bool grow,
+                           int sm_count, void *stream);
 namespace ssetab { struct DfaTables; }
 int sse_build_tables(ssetab::DfaTables &T);                                            // the decode tables of the schema (host)
 int sse_v2_prepare(int device);                                                        // builds + uploads the automaton tables

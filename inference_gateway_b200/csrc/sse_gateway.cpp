@@ -365,6 +365,16 @@ int ssegw_line_pool_growth(ssegw *g, uint32_t max_pages) {
     return SSE_OK;
 }
 
+int ssegw_trim(ssegw *g, uint32_t min_pool_pages) {
+    if (!g) return SSE_ERR_ARG;
+    int first = SSE_OK;
+    for (auto &x : g->ctxs) {
+        const int rc = sse_trim(x.ctx, min_pool_pages);
+        if (rc != SSE_OK && first == SSE_OK) first = rc;
+    }
+    return first;
+}
+
 // ---- handleStreamingRequest (api/routes.go:129-232): the raw proxy loop reads and writes in one goroutine
 int ssegw_proxy_stream(ssegw *g) { return ssegw_stream_chat_completions(g, SSE_MODE_P); }
 int ssegw_proxy_step(ssegw *g, int id, uint8_t *buf, size_t cap, size_t *n) {

@@ -60,12 +60,14 @@ struct Slot {
     bool ctr_queued = false;                                   // sse_submit queued the D2H of h_ctr (do_download does not)
     uint32_t pool_short = 0;                                   // SSE_OVF_POOL: pages the collected batch's lines lacked
     uint32_t pool_gen = 0;                                     // sse_ctx.pool_gen when the batch was launched
+    bool trim = false;                                         // sse_trim: shrink the decode arenas at sse_release
 };
 
 // Line-pool arrays replaced by a growth, freed once the event recorded after their last reader has completed.
 struct RetiredPool {
     uint8_t *pool; uint32_t *stack, *next;
     cudaEvent_t done;
+    uint32_t pages;
 };
 
 } // namespace
@@ -87,7 +89,8 @@ struct sse_ctx {
     PoolHdr *h_pool_hdr = nullptr;       // pinned: sse_line_pool_stats
     uint32_t pool_max = 0;               // sse_line_pool_set_growth: most pages the pool may grow to (0: no growth)
     std::vector<RetiredPool> retired;    // pool arrays a growth replaced, until no queued work can read them
-    uint32_t pool_gen = 0;               // growths so far
+    uint32_t pool_gen = 0;               // growths and trims so far
+    uint64_t device_bytes = 0, pinned_bytes = 0;   // sse_memory_held: what the allocations below hold now
     cudaStream_t ctl_stream = nullptr;
     cudaEvent_t last_kernel = nullptr;   // completion of the most recently launched kernel
     bool have_last = false;
@@ -97,8 +100,20 @@ struct sse_ctx {
 
 namespace {
 
-template <class T> bool dalloc(T *&p, size_t n) { return cu_ok(cudaMalloc((void **)&p, n ? n * sizeof(T) : sizeof(T)), "cudaMalloc"); }
-template <class T> bool halloc(T *&p, size_t n) { return cu_ok(cudaHostAlloc((void **)&p, n ? n * sizeof(T) : sizeof(T), cudaHostAllocDefault), "cudaHostAlloc"); }
+// Every allocation of a context goes through these (or adds its bytes to device_bytes / pinned_bytes where it is made), and every
+// free before sse_destroy takes its bytes off, so that sse_memory_held is what the context holds.
+template <class T> size_t alloc_bytes(size_t n) { return n ? n * sizeof(T) : sizeof(T); }
+template <class T> bool dalloc(sse_ctx *c, T *&p, size_t n) {
+    if (!cu_ok(cudaMalloc((void **)&p, alloc_bytes<T>(n)), "cudaMalloc")) return false;
+    c->device_bytes += alloc_bytes<T>(n);
+    return true;
+}
+template <class T> bool halloc(sse_ctx *c, T *&p, size_t n) {
+    if (!cu_ok(cudaHostAlloc((void **)&p, alloc_bytes<T>(n), cudaHostAllocDefault), "cudaHostAlloc")) return false;
+    c->pinned_bytes += alloc_bytes<T>(n);
+    return true;
+}
+uint64_t pool_bytes(const sse_ctx *c, uint32_t pages) { return (uint64_t)pages * (c->pool.page_bytes + 8u); }   // pages, stack, next
 
 void free_slot(Slot &s) {
     if (s.stream) cudaStreamDestroy(s.stream);
@@ -205,14 +220,28 @@ sse_config worst_decode_caps(const sse_ctx *c) {
     return w;
 }
 
-// One decode-stage arena of a slot grows from *cap to want elements of T, device and pinned (the slot's stream is idle).
-template <class T> int grow_arena(T *&d, T *&h, uint32_t &cap, uint32_t want) {
+// One decode-stage arena of a slot goes from cap to want elements of T, device and pinned (the slot's stream is idle): grows it
+// (redecode) or gives back what a growth took (sse_trim).
+template <class T> int resize_arena(sse_ctx *c, T *&d, T *&h, uint32_t &cap, uint32_t want) {
     T *nd = nullptr, *nh = nullptr;
-    if (cudaMalloc((void **)&nd, (size_t)want * sizeof(T)) != cudaSuccess) { cudaGetLastError(); return SSE_ERR_NOMEM; }
-    if (cudaHostAlloc((void **)&nh, (size_t)want * sizeof(T), cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); cudaFree(nd); return SSE_ERR_NOMEM; }
+    if (cudaMalloc((void **)&nd, alloc_bytes<T>(want)) != cudaSuccess) { cudaGetLastError(); return SSE_ERR_NOMEM; }
+    if (cudaHostAlloc((void **)&nh, alloc_bytes<T>(want), cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); cudaFree(nd); return SSE_ERR_NOMEM; }
     cudaFree(d); cudaFreeHost(h);
+    c->device_bytes += alloc_bytes<T>(want) - alloc_bytes<T>(cap);
+    c->pinned_bytes += alloc_bytes<T>(want) - alloc_bytes<T>(cap);
     d = nd; h = nh; cap = want;
     return SSE_OK;
+}
+
+// sse_trim: the slot's decode arenas back to the configured capacities (the slot holds no batch, or its stream is idle and its
+// results are no longer lent).
+int trim_arenas(sse_ctx *c, Slot &s) {
+    int rc = SSE_OK;
+    if (s.cap_tcs != c->cfg.max_tcs) rc = resize_arena(c, s.d_tcs, s.h_tcs, s.cap_tcs, c->cfg.max_tcs);
+    if (rc == SSE_OK && s.cap_usages != c->cfg.max_usages) rc = resize_arena(c, s.d_usages, s.h_usages, s.cap_usages, c->cfg.max_usages);
+    if (rc == SSE_OK && s.cap_text != c->cfg.text_arena_bytes) rc = resize_arena(c, s.d_text, s.h_text, s.cap_text, c->cfg.text_arena_bytes);
+    s.trim = rc != SSE_OK;   // an allocation failed: the next sse_release tries again
+    return rc;
 }
 
 // SSE_FLAG_DEFER: the decode stage ran out of tool-call, usage or text arena (k: its counters, which count on past a capacity, so
@@ -232,7 +261,7 @@ int redecode(sse_ctx *c, Slot &s, Counters &k, cudaStream_t st, uint32_t &grown)
     };
     auto grow = [&](auto *&d, auto *&h, uint32_t &cap, uint32_t need, uint32_t worst) {
         const uint32_t n = want(cap, need, worst);
-        return n > cap ? grow_arena(d, h, cap, n) : (int)SSE_ERR_NOMEM;
+        return n > cap ? resize_arena(c, d, h, cap, n) : (int)SSE_ERR_NOMEM;
     };
     while (k.status == SSE_ERR_OVERFLOW) {
         const uint32_t ovf = k.overflow & (SSE_OVF_TCS | SSE_OVF_USAGES | SSE_OVF_TEXT);
@@ -322,6 +351,7 @@ void free_retired(sse_ctx *c, bool all) {
             if (e != cudaSuccess) { c->retired[k++] = r; continue; }
         }
         cudaFree(r.pool); cudaFree(r.stack); cudaFree(r.next); cudaEventDestroy(r.done);
+        c->device_bytes -= pool_bytes(c, r.pages);
     }
     c->retired.resize(k);
 }
@@ -338,7 +368,7 @@ int grow_pool(sse_ctx *c, uint32_t lacked) {
     if (want > c->pool_max) want = c->pool_max;
     if (want <= cap) return SSE_OK;
     free_retired(c, false);
-    RetiredPool old{ c->d_pool, c->d_pool_stack, c->d_pool_next, nullptr };
+    RetiredPool old{ c->d_pool, c->d_pool_stack, c->d_pool_next, nullptr, cap };
     uint8_t *pool = nullptr; uint32_t *stack = nullptr, *next = nullptr;
     bool ok = cudaMalloc((void **)&pool, (size_t)want * PB) == cudaSuccess && cudaMalloc((void **)&stack, (size_t)want * 4) == cudaSuccess &&
               cudaMalloc((void **)&next, (size_t)want * 4) == cudaSuccess &&
@@ -361,11 +391,46 @@ int grow_pool(sse_ctx *c, uint32_t lacked) {
     CU(cudaMemcpyAsync(next, c->d_pool_next, (size_t)cap * 4, cudaMemcpyDeviceToDevice, st));
     CU(cudaEventRecord(old.done, st));
     c->retired.push_back(old);
+    c->device_bytes += pool_bytes(c, (uint32_t)want);
     c->d_pool = pool; c->d_pool_stack = stack; c->d_pool_next = next; c->pool.pool_pages = (uint32_t)want;
     c->pool_gen++;
     if (!cu_ok((cudaError_t)sse_launch_pool_extend(pool_params(c), cap, want < c->pool_max, st), "pool extend kernel")) return SSE_ERR_CUDA;
     CU(cudaEventRecord(c->last_kernel, st));
     c->have_last = true;
+    return SSE_OK;
+}
+
+// sse_trim of a pool with a growth limit; the context's stream has just waited for every submitted batch, so the pool is idle
+// and n_free is final. The pool shrinks to max(min_pages, pages held, 1) pages when that is below its capacity: the held pages
+// are repacked into the first pages of new, smaller arrays (sse_launch_pool_repack), the rest go on the free stack. Every
+// later launch is ordered after the repack and gets the new arrays; the old ones are freed before this returns (cudaFree waits
+// for the queued repack, their last reader).
+int trim_pool(sse_ctx *c, uint32_t min_pages) {
+    cudaStream_t st = c->ctl_stream;
+    CU(cudaMemcpyAsync(c->h_pool_hdr, c->d_pool_hdr, sizeof(PoolHdr), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    free_retired(c, false);   // every growth's copy is done
+    const uint32_t cap = c->pool.pool_pages, held = cap - c->h_pool_hdr->n_free, PB = c->pool.page_bytes;
+    uint32_t want = min_pages > held ? min_pages : held;
+    if (want < 1) want = 1;
+    if (want >= cap) return SSE_OK;
+    uint8_t *pool = nullptr; uint32_t *stack = nullptr, *next = nullptr;
+    if (cudaMalloc((void **)&pool, (size_t)want * PB) != cudaSuccess || cudaMalloc((void **)&stack, (size_t)want * 4) != cudaSuccess ||
+        cudaMalloc((void **)&next, (size_t)want * 4) != cudaSuccess) {
+        if (cudaPeekAtLastError() == cudaErrorMemoryAllocation) cudaGetLastError();   // the failed allocation only
+        cudaFree(pool); cudaFree(stack); cudaFree(next);
+        return SSE_ERR_NOMEM;
+    }
+    KParams p = pool_params(c);   // the old arrays
+    const int e = sse_launch_pool_repack(p, pool, stack, next, held, want, want < c->pool_max, c->sm_count, st);
+    if (!cu_ok((cudaError_t)e, "pool repack kernels")) { cudaFree(pool); cudaFree(stack); cudaFree(next); return SSE_ERR_CUDA; }
+    CU(cudaEventRecord(c->last_kernel, st));
+    c->have_last = true;
+    cudaFree(c->d_pool); cudaFree(c->d_pool_stack); cudaFree(c->d_pool_next);
+    c->device_bytes += pool_bytes(c, want);
+    c->device_bytes -= pool_bytes(c, cap);
+    c->d_pool = pool; c->d_pool_stack = stack; c->d_pool_next = next; c->pool.pool_pages = want;
+    c->pool_gen++;            // a batch launched before the trim reports its lack against the old pool: it does not grow this one
     return SSE_OK;
 }
 
@@ -491,15 +556,15 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
     bool ok = true;
     ok = ok && cu_ok(cudaStreamCreateWithFlags(&c->ctl_stream, cudaStreamNonBlocking), "cudaStreamCreate");
     ok = ok && cu_ok(cudaEventCreateWithFlags(&c->last_kernel, cudaEventDisableTiming), "cudaEventCreate");
-    ok = ok && dalloc(c->d_conns, cfg->max_conns);
-    ok = ok && dalloc(c->d_carry, (size_t)cfg->max_conns * cfg->carry_slot_bytes);
+    ok = ok && dalloc(c, c->d_conns, cfg->max_conns);
+    ok = ok && dalloc(c, c->d_carry, (size_t)cfg->max_conns * cfg->carry_slot_bytes);
     ok = ok && cu_ok(cudaMemset(c->d_conns, 0, (size_t)cfg->max_conns * sizeof(ConnState)), "cudaMemset");
-    ok = ok && dalloc(c->d_tcache, sse_fused_tcache_words());
+    ok = ok && dalloc(c, c->d_tcache, sse_fused_tcache_words());
     ok = ok && cu_ok(cudaMemset(c->d_tcache, 0, (size_t)sse_fused_tcache_words() * sizeof(uint32_t)), "cudaMemset");
     if (ok && pool.pool_pages) {
-        ok = ok && dalloc(c->d_pool, (size_t)pool.pool_pages * pool.page_bytes) && dalloc(c->d_pool_hdr, 1);
-        ok = ok && dalloc(c->d_pool_stack, pool.pool_pages) && dalloc(c->d_pool_next, pool.pool_pages);
-        ok = ok && dalloc(c->d_pool_chain, cfg->max_conns) && halloc(c->h_pool_hdr, 1);
+        ok = ok && dalloc(c, c->d_pool, (size_t)pool.pool_pages * pool.page_bytes) && dalloc(c, c->d_pool_hdr, 1);
+        ok = ok && dalloc(c, c->d_pool_stack, pool.pool_pages) && dalloc(c, c->d_pool_next, pool.pool_pages);
+        ok = ok && dalloc(c, c->d_pool_chain, cfg->max_conns) && halloc(c, c->h_pool_hdr, 1);
         ok = ok && cu_ok(cudaMemset(c->d_pool_hdr, 0, sizeof(PoolHdr)), "cudaMemset");
         ok = ok && cu_ok((cudaError_t)sse_launch_pool_reset(pool_params(c), SSE_NONE, c->ctl_stream), "pool reset kernel");
         ok = ok && cu_ok(cudaStreamSynchronize(c->ctl_stream), "cudaStreamSynchronize");
@@ -509,23 +574,23 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
         if (!ok) break;
         ok = ok && cu_ok(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking), "cudaStreamCreate");
         ok = ok && cu_ok(cudaEventCreateWithFlags(&s.kernel_done, cudaEventDisableTiming), "cudaEventCreate");
-        ok = ok && halloc(s.h_in, (size_t)cfg->in_arena_bytes + 16) && halloc(s.h_segs, cfg->max_segs);
-        ok = ok && halloc(s.h_out, cfg->out_arena_bytes) && halloc(s.h_frames, cfg->max_frames) && halloc(s.h_recs, cfg->max_recs);
-        ok = ok && halloc(s.h_tcs, cfg->max_tcs) && halloc(s.h_usages, cfg->max_usages) && halloc(s.h_text, cfg->text_arena_bytes);
-        ok = ok && halloc(s.h_runs, cfg->max_runs) && halloc(s.h_segres, cfg->max_segs) && halloc(s.h_ctr, 1);
-        ok = ok && dalloc(s.d_segs, cfg->max_segs);
-        ok = ok && dalloc(s.d_out, (size_t)in_base_of(*cfg) + cfg->in_arena_bytes + 16);
+        ok = ok && halloc(c, s.h_in, (size_t)cfg->in_arena_bytes + 16) && halloc(c, s.h_segs, cfg->max_segs);
+        ok = ok && halloc(c, s.h_out, cfg->out_arena_bytes) && halloc(c, s.h_frames, cfg->max_frames) && halloc(c, s.h_recs, cfg->max_recs);
+        ok = ok && halloc(c, s.h_tcs, cfg->max_tcs) && halloc(c, s.h_usages, cfg->max_usages) && halloc(c, s.h_text, cfg->text_arena_bytes);
+        ok = ok && halloc(c, s.h_runs, cfg->max_runs) && halloc(c, s.h_segres, cfg->max_segs) && halloc(c, s.h_ctr, 1);
+        ok = ok && dalloc(c, s.d_segs, cfg->max_segs);
+        ok = ok && dalloc(c, s.d_out, (size_t)in_base_of(*cfg) + cfg->in_arena_bytes + 16);
         if (ok) s.d_in = s.d_out + in_base_of(*cfg);
         // recs[max_recs]: the sink record of the empty work items a deferred allocation leaves (SSE_FLAG_DEFER), never returned
-        ok = ok && dalloc(s.d_frames, cfg->max_frames) && dalloc(s.d_recs, (size_t)cfg->max_recs + 1);
+        ok = ok && dalloc(c, s.d_frames, cfg->max_frames) && dalloc(c, s.d_recs, (size_t)cfg->max_recs + 1);
         s.cap_tcs = cfg->max_tcs; s.cap_usages = cfg->max_usages; s.cap_text = cfg->text_arena_bytes;
-        ok = ok && dalloc(s.d_tcs, cfg->max_tcs) && dalloc(s.d_usages, cfg->max_usages) && dalloc(s.d_text, cfg->text_arena_bytes);
-        ok = ok && dalloc(s.d_runs, cfg->max_runs) && dalloc(s.d_segres, cfg->max_segs) && dalloc(s.d_ctr, 1);
-        ok = ok && dalloc(s.d_items, cfg->max_recs) && dalloc(s.d_segterm, cfg->max_segs);
-        ok = ok && dalloc(s.d_items2, cfg->max_recs);
-        ok = ok && dalloc(s.d_tiles, (size_t)cfg->max_segs + 64);
+        ok = ok && dalloc(c, s.d_tcs, cfg->max_tcs) && dalloc(c, s.d_usages, cfg->max_usages) && dalloc(c, s.d_text, cfg->text_arena_bytes);
+        ok = ok && dalloc(c, s.d_runs, cfg->max_runs) && dalloc(c, s.d_segres, cfg->max_segs) && dalloc(c, s.d_ctr, 1);
+        ok = ok && dalloc(c, s.d_items, cfg->max_recs) && dalloc(c, s.d_segterm, cfg->max_segs);
+        ok = ok && dalloc(c, s.d_items2, cfg->max_recs);
+        ok = ok && dalloc(c, s.d_tiles, (size_t)cfg->max_segs + 64);
         if (ok && (cfg->flags & SSE_FLAG_COUNTERS))
-            ok = dalloc(s.d_cnt, CN_COUNT) && halloc(s.h_cnt, CN_COUNT) && cu_ok(cudaMemset(s.d_cnt, 0, CN_COUNT * sizeof(unsigned long long)), "cudaMemset");
+            ok = dalloc(c, s.d_cnt, CN_COUNT) && halloc(c, s.h_cnt, CN_COUNT) && cu_ok(cudaMemset(s.d_cnt, 0, CN_COUNT * sizeof(unsigned long long)), "cudaMemset");
     }
     if (!ok) { sse_destroy(c); return SSE_ERR_CUDA; }
     *out = c;
@@ -614,6 +679,32 @@ int sse_release(sse_ctx *c, int slot) {
     s.state = SLOT_FREE;
     s.cnt_ready = false;
     s.ctr_queued = false;
+    if (s.trim) { CU(cudaSetDevice(c->device)); return trim_arenas(c, s); }
+    return SSE_OK;
+}
+
+int sse_trim(sse_ctx *c, uint32_t min_pool_pages) {
+    if (!c || !(c->cfg.flags & SSE_FLAG_DEFER) || min_pool_pages == SSE_NONE) return SSE_ERR_ARG;
+    CU(cudaSetDevice(c->device));
+    if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
+    CU(cudaStreamSynchronize(c->ctl_stream));
+    int rc = SSE_OK;
+    if (c->pool.pool_pages && c->pool_max) rc = trim_pool(c, min_pool_pages);
+    // a slot that holds a batch may still lend its results (or a device-resident download) to the caller: sse_release trims it
+    for (Slot &s : c->slots) {
+        s.trim = true;
+        if (s.state == SLOT_FREE) {
+            const int r = trim_arenas(c, s);
+            if (rc == SSE_OK) rc = r;
+        }
+    }
+    return rc;
+}
+
+int sse_memory_held(sse_ctx *c, uint64_t *device_bytes, uint64_t *pinned_bytes) {
+    if (!c || !device_bytes || !pinned_bytes) return SSE_ERR_ARG;
+    *device_bytes = c->device_bytes;
+    *pinned_bytes = c->pinned_bytes;
     return SSE_OK;
 }
 

@@ -647,6 +647,60 @@ __global__ void sse_pool_extend_kernel(const __grid_constant__ KParams P, uint32
     if (threadIdx.x == 0) { P.pool_hdr->n_free = n + (P.pool_pages - old_pages); P.pool_hdr->grow = grow; }
 }
 
+// Line pool trim, step 1 (one block; P holds the old arrays, the pool is idle and its `held` pages are all in chains): numbers
+// the held pages densely in chain order. An exclusive scan of PoolChain.n_pages gives every connection its first new page, base;
+// its chain is rewritten in place (first = base, last = base + n - 1, next'[i] = i + 1) and the old id of its k-th page goes to
+// src[base + k]. src is the top `held` entries of the new free stack, above n_free, where nothing reads them once the copy is
+// done; its bottom `pages - held` entries become the free pages [held, pages). Carry lengths, and so every connection's offset in
+// its last page, are untouched.
+__global__ void __launch_bounds__(1024) sse_pool_repack_chains_kernel(const __grid_constant__ KParams P, uint32_t *new_stack,
+                                                                      uint32_t *new_next, uint32_t held, uint32_t pages, uint32_t grow) {
+    __shared__ uint32_t warp_sum[32];
+    const uint32_t t = threadIdx.x, lane = t & 31u, w = t >> 5;
+    const uint32_t per = (P.max_conns + blockDim.x - 1) / blockDim.x;
+    const uint32_t c0 = min(t * per, P.max_conns), c1 = min(c0 + per, P.max_conns);
+    uint32_t n = 0;
+    for (uint32_t c = c0; c < c1; c++) n += P.pool_chain[c].n_pages;
+    uint32_t x = n;   // inclusive scan over the block: within the warp, then over the warp totals
+    for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(FULL, x, d); if (lane >= d) x += y; }
+    if (lane == 31) warp_sum[w] = x;
+    __syncthreads();
+    if (w == 0) {
+        uint32_t s = lane < (blockDim.x >> 5) ? warp_sum[lane] : 0u;
+        for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(FULL, s, d); if (lane >= d) s += y; }
+        warp_sum[lane] = s;
+    }
+    __syncthreads();
+    uint32_t base = x - n + (w ? warp_sum[w - 1] : 0u);
+    uint32_t *src = new_stack + (pages - held);
+    for (uint32_t c = c0; c < c1; c++) {
+        PoolChain ch = P.pool_chain[c];
+        if (!ch.n_pages) continue;
+        uint32_t pg = ch.first;
+        for (uint32_t k = 0; k < ch.n_pages; k++) {
+            src[base + k] = pg;
+            new_next[base + k] = k + 1 < ch.n_pages ? base + k + 1 : SSE_NONE;
+            if (k + 1 < ch.n_pages) pg = P.pool_next[pg];
+        }
+        ch.first = base; ch.last = base + ch.n_pages - 1;
+        P.pool_chain[c] = ch;
+        base += ch.n_pages;
+    }
+    for (uint32_t i = t; i < pages - held; i += blockDim.x) new_stack[i] = held + i;
+    if (t == 0) { P.pool_hdr->lock = 0; P.pool_hdr->n_free = pages - held; P.pool_hdr->grow = grow; }
+}
+
+// Line pool trim, step 2: new page i = old page src[i], for the held pages only, 16 bytes per load and store (page_bytes is a
+// multiple of 16). A block copies whole pages, so no thread divides by the page size.
+__global__ void __launch_bounds__(256) sse_pool_repack_copy_kernel(const uint4 *__restrict__ old_pool, uint4 *__restrict__ new_pool,
+                                                                   const uint32_t *__restrict__ src, uint32_t held, uint32_t vecs_per_page) {
+    for (uint32_t p = blockIdx.x; p < held; p += gridDim.x) {
+        const uint4 *s = old_pool + (size_t)src[p] * vecs_per_page;
+        uint4 *d = new_pool + (size_t)p * vecs_per_page;
+        for (uint32_t v = threadIdx.x; v < vecs_per_page; v += blockDim.x) d[v] = s[v];
+    }
+}
+
 DfaTables *g_tables_dev[16] = { nullptr };
 
 } // namespace
@@ -736,5 +790,16 @@ int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream) {
 
 int sse_launch_pool_extend(const KParams &p, uint32_t old_pages, bool grow, void *stream) {
     sse_pool_extend_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(p, old_pages, grow ? 1u : 0u);
+    return (int)cudaGetLastError();
+}
+
+int sse_launch_pool_repack(const KParams &p, uint8_t *pool, uint32_t *stack, uint32_t *next, uint32_t held, uint32_t pages, bool grow,
+                           int sm_count, void *stream) {
+    sse_pool_repack_chains_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(p, stack, next, held, pages, grow ? 1u : 0u);
+    if (held) {
+        const uint32_t grid = held < 8u * (uint32_t)sm_count ? held : 8u * (uint32_t)sm_count;   // 8 blocks of 256 fill an SM
+        sse_pool_repack_copy_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint4 *)p.pool, (uint4 *)pool, stack + (pages - held),
+                                                                            held, p.page_bytes / 16u);
+    }
     return (int)cudaGetLastError();
 }

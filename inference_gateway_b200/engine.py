@@ -144,6 +144,20 @@ class SseEngine:
         A.check(self.L.sse_line_pool_stats(self._ctx, C.byref(used), C.byref(hw)), "sse_line_pool_stats")
         return used.value, hw.value
 
+    def trim(self, min_pool_pages: int | None = None):
+        """sse_trim: gives back what on-demand growth took (FLAG_DEFER). A pool with a growth limit shrinks to
+        max(min_pool_pages, pages held, 1) pages (default: the pages the engine was created with) when that is below its capacity;
+        every slot's decode arenas go back to the config's capacities, a slot that holds a batch at its release."""
+        if min_pool_pages is None:
+            min_pool_pages = self.pool.pool_pages if self.pool is not None else 0
+        A.check(self.L.sse_trim(self._ctx, min_pool_pages), "sse_trim")
+
+    def memory_held(self):
+        """sse_memory_held: (device bytes, pinned host bytes) the context holds now."""
+        dev, pin = C.c_uint64(), C.c_uint64()
+        A.check(self.L.sse_memory_held(self._ctx, C.byref(dev), C.byref(pin)), "sse_memory_held")
+        return dev.value, pin.value
+
     def close(self):
         if self._ctx:
             self.L.sse_destroy(self._ctx)

@@ -92,6 +92,7 @@ class Gateway:
         L.ssegw_agent_tool_calls.restype = C.c_size_t
         L.ssegw_counters.argtypes = [vp, C.POINTER(A.Counters)]
         L.ssegw_line_pool_growth.argtypes = [vp, C.c_uint32]
+        L.ssegw_trim.argtypes = [vp, C.c_uint32]
         st = i32()
         line_pool = dict(line_pool) if line_pool is not None else None
         max_pages = line_pool.pop("max_pages", 0) if line_pool is not None else 0
@@ -217,6 +218,13 @@ class Gateway:
         k.struct_size = C.sizeof(A.Counters)
         A.check(self.L.ssegw_counters(self.g, C.byref(k)), "ssegw_counters")
         return A.counters_dict(k)
+
+    def trim(self, min_pool_pages: int | None = None):
+        """ssegw_trim: sse_trim on every context (the config must have FLAG_DEFER); min_pool_pages defaults to the pages of the
+        line pool the gateway was created with."""
+        if min_pool_pages is None:
+            min_pool_pages = self._pool.pool_pages if self._pool is not None else 0
+        A.check(self.L.ssegw_trim(self.g, min_pool_pages), "ssegw_trim")
 
     def release(self, sid: int):
         self.L.ssegw_release_stream(self.g, sid)

@@ -45,6 +45,11 @@ type Batcher interface {
 	Close(conn uint32)
 	// Open streams, for placement.
 	Streams() int
+	// Trim runs Context.Trim between two ticks of the batcher's goroutine. When to call it (e.g. a timer after bursts of
+	// long lines) is the operator's policy; the batcher never trims on its own.
+	Trim(minPages uint32) error
+	// MemoryHeld is Context.MemoryHeld, e.g. for export as gauges.
+	MemoryHeld() (device, pinned uint64, err error)
 }
 
 // inFlight is one submitted batch and the connections (with their generation: a connection closed and opened again

@@ -133,6 +133,20 @@ func (x *Context) LinePoolCapacity() (pages, maxPages uint32, err error) {
 	return uint32(p), uint32(m), err
 }
 
+// Trim gives back what on-demand growth (GPU_DEFER=1) took: a line pool with a growth limit shrinks to max(minPages, pages
+// held, 1) pages, and every slot's decode arenas go back to the config's capacities (a slot that holds a batch at its
+// Release). Connections holding lines go on unchanged. It waits for the batches already submitted to finish on the device.
+func (x *Context) Trim(minPages uint32) error {
+	return statusErr("sse_trim", C.sse_trim(x.c, C.uint32_t(minPages)))
+}
+
+// MemoryHeld returns the device and pinned host bytes the context holds now, grown pool and arenas included.
+func (x *Context) MemoryHeld() (device, pinned uint64, err error) {
+	var d, p C.uint64_t
+	err = statusErr("sse_memory_held", C.sse_memory_held(x.c, &d, &p))
+	return uint64(d), uint64(p), err
+}
+
 func (x *Context) Close() { C.sse_destroy(x.c) }
 
 // Batch is one acquired slot: Arena and Segs alias pinned memory owned by the library.
