@@ -151,10 +151,10 @@ struct WarpTally {
 };
 #endif
 
-// launch wrappers (sse_kernel.cu)
-int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count);           // split pipeline, stage 1
-int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device);  // split pipeline, stages 2+3
-int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device);           // SSE_FLAG_DEFER: stage 2 again (grown arenas)
+// launch wrappers (sse_kernel.cu). The batch wrappers add the kernels they launch to `launches` (sse_launch_count).
+int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count, uint64_t &launches);              // split pipeline, stage 1
+int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches); // split pipeline, stages 2+3
+int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches);  // SSE_FLAG_DEFER: stage 2 again (grown arenas)
 int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream);              // line pool: reset one connection (SSE_NONE: all)
 int sse_launch_pool_extend(const KParams &p, uint32_t old_pages, bool grow, void *stream); // line pool: pages [old_pages, pool_pages) free
 // line pool trim: the held pages of p's idle pool repacked into the first `held` pages of new arrays of `pages` pages
@@ -166,6 +166,6 @@ int sse_v2_prepare(int device);                                                 
 int sse_long_prepare(int device);                                                      // long-line decode kernel: occupancy (sse_long.cu)
 void sse_launch_long_decode(const KParams &p, const ssetab::DfaTables *tables, void *stream, int sm_count, int device);   // stage 2a
 int sse_fused_prepare(int device);                                                     // fused pipeline: tables + kernel attributes
-int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device);        // plan kernel + fused tile kernel
+int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches);   // plan kernel + fused tile kernel
 uint32_t sse_fused_max_line(void);
 uint32_t sse_fused_tcache_words(void);                                                 // size of KParams.tcache                                                     // longest carry_slot_bytes the fused kernel supports

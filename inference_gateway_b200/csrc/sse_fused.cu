@@ -106,23 +106,8 @@ struct FSmem {
     alignas(8) unsigned long long mbar;
     uint32_t scan_a[F_WARPS], scan_b[F_WARPS];
     uint32_t bc[16];
-    long long prof_t;
 };
 static_assert(F_CTAS_PER_SM == 2 && sizeof(FSmem) <= 113 * 1024, "two CTAs per SM");
-
-#ifdef SSE_PROF
-__device__ unsigned long long g_prof[160];
-#define PROF(i) do { if (threadIdx.x == 0) { const long long t_ = clock64(); atomicAdd(&g_prof[i], (unsigned long long)(t_ - S.prof_t)); S.prof_t = t_; } } while (0)
-#else
-#define PROF(i) do { } while (0)
-#endif
-#ifdef SSE_PROF
-#define PCOUNT(i, n) atomicAdd(&g_prof[i], (unsigned long long)(n))
-#define PSTAMP(k) do { __syncwarp(); if ((threadIdx.x & 31u) == 0) { const long long t_ = clock64(); atomicAdd(&g_prof[64 + (k) * 16 + (threadIdx.x >> 5)], (unsigned long long)(t_ - ts_)); ts_ = t_; } } while (0)
-#else
-#define PSTAMP(k) do { } while (0)
-#define PCOUNT(i, n) do { } while (0)
-#endif
 
 // ---------------------------------------------------------------- bulk copy + mbarrier (PTX)
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -1057,7 +1042,6 @@ __device__ __noinline__ void t_build(const KParams &P, FSmem &S, uint32_t rslot,
     __threadfence_block();
     S.ts_used = off + words;
     S.thead[n_struct] = off;                               // published: readers see a complete template
-    PCOUNT(51, 1); PCOUNT(52, words);
 }
 
 // A line retires: final syntax check, record, termination bookkeeping (agent.go:205-242).
@@ -1297,7 +1281,6 @@ __device__ __noinline__ bool warp_replay(const KParams &P, FSmem &S, uint32_t j,
         if (__all_sync(FULL, ok)) { T = U; break; }
     }
     if (!T) return false;
-    if (lane == 0) PCOUNT(49, 1);
     // ---- 4. the captures
     const uint32_t cseg = T[6] & 0xFFu, fseg = (T[6] >> 8) & 0xFFu, n_ops = T[3] >> 16, tc_count = T[1] >> 24, tflags = (T[1] >> 16) & 0xFFu;
     if (lane == 0) {
@@ -1338,7 +1321,7 @@ __device__ __noinline__ void stage2_automaton(const KParams &P, FSmem &S, bool h
             while ((~m) & ((1u << NREC) - 1u)) {
                 const uint32_t b = (uint32_t)__ffs((~m) & ((1u << NREC) - 1u)) - 1u;
                 const uint32_t old = atomicCAS(&S.rec_busy, m, m | (1u << b));
-                if (old == m) { PCOUNT(53, 1); L.rslot = b; FRec &R = S.rec[b]; R.n = 0; R.nonsimple = 0; R.n_str = 0; R.n_arr = 0; break; }
+                if (old == m) { L.rslot = b; FRec &R = S.rec[b]; R.n = 0; R.nonsimple = 0; R.n_str = 0; R.n_arr = 0; break; }
                 m = old;
             }
         }
@@ -1361,7 +1344,7 @@ __device__ void stage2(const KParams &P, FSmem &S, uint32_t n_jobs, uint32_t rb)
     for (uint32_t j = wid; j < n_jobs; j += F_WARPS) {
         bool hit = false;
         if ((P.flags & SSE_FLAG_TEMPLATES)) hit = warp_replay(P, S, j, rb);
-        if (!hit && lane == 0) { PCOUNT(50, 1); FRes z; z.cpos = z.clen = z.toff = 0; z.misc = 0; S.res[j] = z; }
+        if (!hit && lane == 0) { FRes z; z.cpos = z.clen = z.toff = 0; z.misc = 0; S.res[j] = z; }
     }
     __syncwarp();
     // the lines no template took: lane i has this warp's i-th line
@@ -1394,10 +1377,8 @@ __device__ __forceinline__ void stage2_records(const KParams &P, FSmem &S, uint3
 __device__ __noinline__ void process_window(const KParams &P, FSmem &S, uint32_t first_seg, uint32_t nseg, uint32_t fill) {
     const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
     const bool zero_copy = !(P.flags & SSE_FLAG_COPY_OUT);
-    PROF(0);
     stage1a(S, fill);
     __syncthreads();
-    PROF(1);
 
     uint32_t r_start = 0;
     #pragma unroll 1
@@ -1477,7 +1458,6 @@ __device__ __noinline__ void process_window(const KParams &P, FSmem &S, uint32_t
             ln.start = (uint16_t)start; ln.a = (uint16_t)a; ln.b = (uint16_t)b; ln.seg = (uint8_t)lo;
         }
         __syncthreads();
-        PROF(2);
         // ---------------- allocate records, decode jobs and materialised bytes (one atomicAdd each per round)
         if (k < n_lines && k >= S.seg[my_seg].dead) { kind = K_DROP; lflags &= LF_RMODE; mat = 0; flen = 0; }
         uint32_t vrj = ((lflags & LF_PARSE) ? 1u : 0u) | ((lflags & LF_JOB) ? 0x10000u : 0u), vb = mat;
@@ -1513,11 +1493,8 @@ __device__ __noinline__ void process_window(const KParams &P, FSmem &S, uint32_t
         }
         __syncthreads();
         // ---------------- decode
-        PROF(3);
         stage2(P, S, tot_j, rb);
-        PROF(8);
         __syncthreads();
-        PROF(4);
         stage2_records(P, S, tot_j, rb);
         __syncthreads();
         #pragma unroll 1
@@ -1576,7 +1553,6 @@ __device__ __noinline__ void process_window(const KParams &P, FSmem &S, uint32_t
             }
         }
         __syncthreads();
-        PROF(5);
         // ---------------- this round's run of every segment; connection state
         if (tid < nseg) {
             FSeg &sg = S.seg[tid];
@@ -1744,9 +1720,6 @@ sse_fused_kernel(const __grid_constant__ KParams P, const FTables *__restrict__ 
     __syncthreads();
     uint32_t phase = 0;
     const uint32_t n_tiles = min(P.ctr->n_tiles, P.cap_tiles);
-#ifdef SSE_PROF
-    if (tid == 0) S.prof_t = clock64();
-#endif
 
     if (tid == 0) S.bc[0] = atomicAdd(&P.ctr->ticket, 1u);
     __syncthreads();
@@ -1808,10 +1781,8 @@ sse_fused_kernel(const __grid_constant__ KParams P, const FTables *__restrict__ 
             __syncthreads();
             if (total) process_window(P, S, first, nseg, total);
             __syncthreads();
-            PROF(6);
             for (uint32_t i = w; i < nseg; i += F_WARPS) finish_segment(P, S, first, i);
             __syncthreads();
-            PROF(7);
             continue;
         }
 
@@ -1936,26 +1907,17 @@ int sse_fused_prepare(int device) {
     return 0;
 }
 
-extern "C" int sse_prof_read(unsigned long long *out16) {
-#ifdef SSE_PROF
-    unsigned long long z[160] = { 0 };
-    if (cudaMemcpyFromSymbol(out16, g_prof, sizeof z) != cudaSuccess) return -1;
-    cudaMemcpyToSymbol(g_prof, z, sizeof z);
-    return 0;
-#else
-    (void)out16; return -1;
-#endif
-}
-
 uint32_t sse_fused_max_line(void) { return TILE - 32u; }
 uint32_t sse_fused_tcache_words(void) { return 8192u; }   // (both engines' layouts fit)
 
-int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device) {
+int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches) {
     const uint32_t groups = (p.n_segs + PLAN_GROUP - 1) / PLAN_GROUP;
     sse_plan_kernel<<<(groups + 3) / 4, 128, 0, (cudaStream_t)stream>>>(p);
+    launches++;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return (int)e;
     // persistent: the resident CTAs pull tiles by ticket
     sse_fused_kernel<<<sm_count * F_CTAS_PER_SM, F_THREADS, sizeof(FSmem), (cudaStream_t)stream>>>(p, g_ftables_dev[device]);
+    launches++;
     return (int)cudaGetLastError();
 }

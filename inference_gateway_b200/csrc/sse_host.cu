@@ -33,31 +33,49 @@ bool cu_ok(cudaError_t e, const char *what) {
 
 enum SlotState { SLOT_FREE = 0, SLOT_ACQUIRED, SLOT_SUBMITTED, SLOT_COLLECTED };
 
+// One allocation of a context: n elements of T, in device memory or in pinned host memory. buf_alloc and buf_free are the only
+// functions that allocate or free one, and the only ones that count its bytes, so that sse_memory_held is what the context holds.
+template <class T> struct Buf {
+    T *p = nullptr;
+    size_t n = 0;
+    bool pinned = false;
+};
+
+// An array on the device and its pinned copy on the host, which the upload or do_download copies between; cap() elements each.
+template <class T> struct Pair {
+    Buf<T> d, h{nullptr, 0, true};
+    uint32_t cap() const { return (uint32_t)h.n; }
+};
+
+// The line pool's arrays, for one page count: page bytes, free stack and next-page links. A growth or a trim replaces all three.
+struct PoolArrays {
+    Buf<uint8_t> pages;
+    Buf<uint32_t> stack, next;
+};
+
+// Only the head of Counters travels to the host: the rest is the sort's per-bucket scratch, which the device alone reads.
+constexpr size_t CTR_HEAD = offsetof(Counters, class_count);
+
 struct Slot {
     int state = SLOT_FREE;
     cudaStream_t stream = nullptr;
     cudaEvent_t kernel_done = nullptr;
-    // host (pinned)
-    uint8_t *h_in = nullptr; sse_seg *h_segs = nullptr;
-    uint8_t *h_out = nullptr; sse_frame *h_frames = nullptr; sse_rec *h_recs = nullptr; sse_tc *h_tcs = nullptr;
-    sse_usage *h_usages = nullptr; uint8_t *h_text = nullptr; sse_run *h_runs = nullptr; sse_seg_result *h_segres = nullptr;
-    Counters *h_ctr = nullptr;
-    // device
-    uint8_t *d_in = nullptr; sse_seg *d_segs = nullptr;
-    uint8_t *d_out = nullptr; sse_frame *d_frames = nullptr; sse_rec *d_recs = nullptr; sse_tc *d_tcs = nullptr;
-    sse_usage *d_usages = nullptr; uint8_t *d_text = nullptr; sse_run *d_runs = nullptr; sse_seg_result *d_segres = nullptr;
-    Counters *d_ctr = nullptr;
-    uint4 *d_items = nullptr; uint32_t *d_segterm = nullptr;   // split pipeline scratch (device only)
-    uint4 *d_items2 = nullptr;                                 // items ordered for the decode kernel
-    uint2 *d_tiles = nullptr;                                  // fused pipeline: tile list of the plan kernel
+    Buf<uint8_t> h_in{nullptr, 0, true};
+    uint8_t *d_in = nullptr;                                   // inside out.d (slot_buffers)
+    Pair<sse_seg> segs;
+    Pair<uint8_t> out;
+    Pair<sse_frame> frames; Pair<sse_rec> recs; Pair<sse_run> runs; Pair<sse_seg_result> segres; Pair<Counters> ctr;
+    Pair<sse_tc> tcs; Pair<sse_usage> usages; Pair<uint8_t> text;   // decode-stage arenas: SSE_FLAG_DEFER grows them per slot
+    Buf<uint4> items; Buf<uint32_t> segterm;                   // split pipeline scratch (device only)
+    Buf<uint4> items2;                                         // items ordered for the decode kernel
+    Buf<uint2> tiles;                                          // fused pipeline: tile list of the plan kernel
     uint32_t n_segs = 0, in_bytes = 0;
-    uint32_t cap_tcs = 0, cap_usages = 0, cap_text = 0;        // decode-stage capacities (SSE_FLAG_DEFER grows them per slot)
-    // SSE_FLAG_COUNTERS: the batch's counter block (CN_*), device and pinned; kept apart from Counters, which the default path
-    // clears and downloads every batch
-    unsigned long long *d_cnt = nullptr, *h_cnt = nullptr;
+    // SSE_FLAG_COUNTERS: the batch's counter block (CN_*); kept apart from Counters, which the default path clears and downloads
+    // every batch
+    Pair<unsigned long long> cnt;
     uint32_t decode_passes = 0;
-    bool cnt_ready = false;                                    // h_cnt holds the counters of the batch last downloaded
-    bool ctr_queued = false;                                   // sse_submit queued the D2H of h_ctr (do_download does not)
+    bool cnt_ready = false;                                    // cnt.h holds the counters of the batch last downloaded
+    bool ctr_queued = false;                                   // sse_submit queued the D2H of ctr.h (do_download does not)
     uint32_t pool_short = 0;                                   // SSE_OVF_POOL: pages the collected batch's lines lacked
     uint32_t pool_gen = 0;                                     // sse_ctx.pool_gen when the batch was launched
     bool trim = false;                                         // sse_trim: shrink the decode arenas at sse_release
@@ -65,9 +83,8 @@ struct Slot {
 
 // Line-pool arrays replaced by a growth, freed once the event recorded after their last reader has completed.
 struct RetiredPool {
-    uint8_t *pool; uint32_t *stack, *next;
+    PoolArrays arrays;
     cudaEvent_t done;
-    uint32_t pages;
 };
 
 } // namespace
@@ -80,119 +97,146 @@ struct sse_ctx {
     int device = 0;
     int sm_count = 0;
     sse_config cfg{};
-    ConnState *d_conns = nullptr;
-    uint8_t *d_carry = nullptr;
-    uint32_t *d_tcache = nullptr;        // fused kernel: skeleton templates kept between launches
+    Buf<ConnState> conns;
+    Buf<uint8_t> carry;
+    Buf<uint32_t> tcache;                // fused kernel: skeleton templates kept between launches
     sse_line_pool pool{};                // pool_pages == 0: no line pool
-    uint8_t *d_pool = nullptr; PoolHdr *d_pool_hdr = nullptr; uint32_t *d_pool_stack = nullptr, *d_pool_next = nullptr;
-    PoolChain *d_pool_chain = nullptr;
-    PoolHdr *h_pool_hdr = nullptr;       // pinned: sse_line_pool_stats
+    PoolArrays pool_arrays;
+    Buf<PoolHdr> pool_hdr;
+    Buf<PoolChain> pool_chain;
+    Buf<PoolHdr> h_pool_hdr{nullptr, 0, true};   // sse_line_pool_stats
     uint32_t pool_max = 0;               // sse_line_pool_set_growth: most pages the pool may grow to (0: no growth)
     std::vector<RetiredPool> retired;    // pool arrays a growth replaced, until no queued work can read them
     uint32_t pool_gen = 0;               // growths and trims so far
-    uint64_t device_bytes = 0, pinned_bytes = 0;   // sse_memory_held: what the allocations below hold now
+    uint64_t device_bytes = 0, pinned_bytes = 0;   // sse_memory_held: what the buffers above and the slots' hold now
     cudaStream_t ctl_stream = nullptr;
-    cudaEvent_t last_kernel = nullptr;   // completion of the most recently launched kernel
-    bool have_last = false;
+    cudaEvent_t last_kernel = nullptr;   // completion of the most recently launched kernel (or of sse_init_ex)
     std::vector<Slot> slots;
     uint64_t launches = 0;
 };
 
 namespace {
 
-// Every allocation of a context goes through these (or adds its bytes to device_bytes / pinned_bytes where it is made), and every
-// free before sse_destroy takes its bytes off, so that sse_memory_held is what the context holds.
 template <class T> size_t alloc_bytes(size_t n) { return n ? n * sizeof(T) : sizeof(T); }
-template <class T> bool dalloc(sse_ctx *c, T *&p, size_t n) {
-    if (!cu_ok(cudaMalloc((void **)&p, alloc_bytes<T>(n)), "cudaMalloc")) return false;
-    c->device_bytes += alloc_bytes<T>(n);
-    return true;
-}
-template <class T> bool halloc(sse_ctx *c, T *&p, size_t n) {
-    if (!cu_ok(cudaHostAlloc((void **)&p, alloc_bytes<T>(n), cudaHostAllocDefault), "cudaHostAlloc")) return false;
-    c->pinned_bytes += alloc_bytes<T>(n);
-    return true;
-}
-uint64_t pool_bytes(const sse_ctx *c, uint32_t pages) { return (uint64_t)pages * (c->pool.page_bytes + 8u); }   // pages, stack, next
 
-void free_slot(Slot &s) {
+// After a failed allocation only cudaErrorMemoryAllocation is cleared, so that a later launch does not report it; any other
+// error stays for the next check to find.
+template <class T> bool buf_alloc(sse_ctx *c, Buf<T> &b, size_t n) {
+    const cudaError_t e = b.pinned ? cudaHostAlloc((void **)&b.p, alloc_bytes<T>(n), cudaHostAllocDefault)
+                                   : cudaMalloc((void **)&b.p, alloc_bytes<T>(n));
+    if (!cu_ok(e, b.pinned ? "cudaHostAlloc" : "cudaMalloc")) {
+        if (cudaPeekAtLastError() == cudaErrorMemoryAllocation) cudaGetLastError();
+        b.p = nullptr;
+        return false;
+    }
+    b.n = n;
+    (b.pinned ? c->pinned_bytes : c->device_bytes) += alloc_bytes<T>(n);
+    return true;
+}
+
+template <class T> void buf_free(sse_ctx *c, Buf<T> &b) {
+    if (!b.p) return;
+    if (b.pinned) cudaFreeHost(b.p);
+    else cudaFree(b.p);
+    (b.pinned ? c->pinned_bytes : c->device_bytes) -= alloc_bytes<T>(b.n);
+    b.p = nullptr;
+    b.n = 0;
+}
+
+void pool_free(sse_ctx *c, PoolArrays &a) { buf_free(c, a.pages); buf_free(c, a.stack); buf_free(c, a.next); }
+
+// All three arrays for `pages` pages, or none.
+bool pool_alloc(sse_ctx *c, PoolArrays &a, uint32_t pages) {
+    if (buf_alloc(c, a.pages, (size_t)pages * c->pool.page_bytes) && buf_alloc(c, a.stack, pages) && buf_alloc(c, a.next, pages))
+        return true;
+    pool_free(c, a);
+    return false;
+}
+
+// f(buffer, element count) for every buffer of a slot, with the counts cfg gives them (resize changes the decode arenas'
+// later). Where a count is not the capacity it serves:
+//   out.d  holds [out arena | pad | in arena] (in_base_of): d_in points into it;
+//   recs.d has one record more than recs.h: recs[max_recs] is the sink record of the empty work items a deferred allocation
+//          leaves (SSE_FLAG_DEFER), never returned;
+//   h_in   mirrors the device's in arena, 16 bytes of padding past in_arena_bytes included.
+template <class F> void slot_buffers(Slot &s, const sse_config &cfg, F f) {
+    auto both = [&](auto &pair, size_t n) { f(pair.h, n); f(pair.d, n); };
+    f(s.h_in, (size_t)cfg.in_arena_bytes + 16);
+    f(s.out.h, cfg.out_arena_bytes); f(s.out.d, (size_t)in_base_of(cfg) + cfg.in_arena_bytes + 16);
+    f(s.recs.h, cfg.max_recs); f(s.recs.d, (size_t)cfg.max_recs + 1);
+    both(s.segs, cfg.max_segs); both(s.frames, cfg.max_frames); both(s.tcs, cfg.max_tcs); both(s.usages, cfg.max_usages);
+    both(s.text, cfg.text_arena_bytes); both(s.runs, cfg.max_runs); both(s.segres, cfg.max_segs); both(s.ctr, 1);
+    if (cfg.flags & SSE_FLAG_COUNTERS) both(s.cnt, CN_COUNT);
+    f(s.items, cfg.max_recs); f(s.segterm, cfg.max_segs); f(s.items2, cfg.max_recs); f(s.tiles, (size_t)cfg.max_segs + 64);
+}
+
+void free_slot(sse_ctx *c, Slot &s) {
     if (s.stream) cudaStreamDestroy(s.stream);
     if (s.kernel_done) cudaEventDestroy(s.kernel_done);
-    cudaFreeHost(s.h_in); cudaFreeHost(s.h_segs); cudaFreeHost(s.h_out); cudaFreeHost(s.h_frames); cudaFreeHost(s.h_recs);
-    cudaFreeHost(s.h_tcs); cudaFreeHost(s.h_usages); cudaFreeHost(s.h_text); cudaFreeHost(s.h_runs); cudaFreeHost(s.h_segres);
-    cudaFreeHost(s.h_ctr); cudaFreeHost(s.h_cnt); cudaFree(s.d_cnt);
-    cudaFree(s.d_segs); cudaFree(s.d_out);   // d_in lives inside d_out's allocation
-    cudaFree(s.d_frames); cudaFree(s.d_recs); cudaFree(s.d_tcs);
-    cudaFree(s.d_usages); cudaFree(s.d_text); cudaFree(s.d_runs); cudaFree(s.d_segres); cudaFree(s.d_ctr); cudaFree(s.d_items); cudaFree(s.d_segterm); cudaFree(s.d_items2); cudaFree(s.d_tiles);
+    slot_buffers(s, c->cfg, [&](auto &b, size_t) { buf_free(c, b); });
 }
 
-KParams make_params(sse_ctx *c, Slot &s, uint32_t n_segs) {
+// KParams for the line-pool maintenance kernels (no batch slot involved)
+KParams pool_params(sse_ctx *c) {
     KParams p{};
-    p.in = s.d_in; p.segs = s.d_segs; p.n_segs = n_segs; p.max_conns = c->cfg.max_conns;
-    p.conns = c->d_conns; p.carry = c->d_carry; p.carry_slot = c->cfg.carry_slot_bytes;
-    p.out = s.d_out; p.cap_out = c->cfg.out_arena_bytes; p.in_base = in_base_of(c->cfg);
-    p.frames = s.d_frames; p.cap_frames = c->cfg.max_frames;
-    p.recs = s.d_recs; p.cap_recs = c->cfg.max_recs;
-    p.tcs = s.d_tcs; p.cap_tcs = s.cap_tcs;
-    p.usages = s.d_usages; p.cap_usages = s.cap_usages;
-    p.text = s.d_text; p.cap_text = s.cap_text;
-    p.runs = s.d_runs; p.cap_runs = c->cfg.max_runs;
-    p.seg_results = s.d_segres; p.ctr = s.d_ctr;
-    p.items = s.d_items; p.cap_items = c->cfg.max_recs; p.seg_term = s.d_segterm;
-    p.items_sorted = s.d_items2; p.flags = c->cfg.flags;
-    p.tiles = s.d_tiles; p.cap_tiles = c->cfg.max_segs + 64;
-    p.tcache = (c->cfg.flags & SSE_FLAG_TEMPLATES) ? c->d_tcache : nullptr;
-    p.pool = c->d_pool; p.pool_hdr = c->d_pool_hdr; p.pool_stack = c->d_pool_stack; p.pool_next = c->d_pool_next;
-    p.pool_chain = c->d_pool_chain;
-    p.page_bytes = c->pool.page_bytes; p.pool_pages = c->pool.pool_pages;
-    p.max_line = c->pool.pool_pages ? c->pool.max_line_bytes : c->cfg.carry_slot_bytes;
-    p.long_line = (SSE_LONG_LINE && !(c->cfg.flags & SSE_FLAG_KERNEL_FUSED) && p.max_line >= SSE_LONG_LINE) ? SSE_LONG_LINE : 0u;
-    p.cnt = s.d_cnt;
+    p.max_conns = c->cfg.max_conns; p.conns = c->conns.p;
+    p.pool = c->pool_arrays.pages.p; p.pool_stack = c->pool_arrays.stack.p; p.pool_next = c->pool_arrays.next.p;
+    p.pool_hdr = c->pool_hdr.p; p.pool_chain = c->pool_chain.p; p.page_bytes = c->pool.page_bytes; p.pool_pages = c->pool.pool_pages;
     return p;
 }
 
-// KParams for the line-pool maintenance kernel (no batch slot involved)
-KParams pool_params(sse_ctx *c) {
-    KParams p{};
-    p.max_conns = c->cfg.max_conns; p.conns = c->d_conns;
-    p.pool = c->d_pool; p.pool_hdr = c->d_pool_hdr; p.pool_stack = c->d_pool_stack; p.pool_next = c->d_pool_next;
-    p.pool_chain = c->d_pool_chain; p.page_bytes = c->pool.page_bytes; p.pool_pages = c->pool.pool_pages;
+KParams make_params(sse_ctx *c, Slot &s, uint32_t n_segs) {
+    KParams p = pool_params(c);
+    p.in = s.d_in; p.segs = s.segs.d.p; p.n_segs = n_segs;
+    p.carry = c->carry.p; p.carry_slot = c->cfg.carry_slot_bytes;
+    p.out = s.out.d.p; p.cap_out = c->cfg.out_arena_bytes; p.in_base = in_base_of(c->cfg);
+    p.frames = s.frames.d.p; p.cap_frames = c->cfg.max_frames;
+    p.recs = s.recs.d.p; p.cap_recs = c->cfg.max_recs;
+    p.tcs = s.tcs.d.p; p.cap_tcs = s.tcs.cap();
+    p.usages = s.usages.d.p; p.cap_usages = s.usages.cap();
+    p.text = s.text.d.p; p.cap_text = s.text.cap();
+    p.runs = s.runs.d.p; p.cap_runs = c->cfg.max_runs;
+    p.seg_results = s.segres.d.p; p.ctr = s.ctr.d.p;
+    p.items = s.items.p; p.cap_items = c->cfg.max_recs; p.seg_term = s.segterm.p;
+    p.items_sorted = s.items2.p; p.flags = c->cfg.flags;
+    p.tiles = s.tiles.p; p.cap_tiles = c->cfg.max_segs + 64;
+    p.tcache = (c->cfg.flags & SSE_FLAG_TEMPLATES) ? c->tcache.p : nullptr;
+    p.max_line = c->pool.pool_pages ? c->pool.max_line_bytes : c->cfg.carry_slot_bytes;
+    p.long_line = (SSE_LONG_LINE && !(c->cfg.flags & SSE_FLAG_KERNEL_FUSED) && p.max_line >= SSE_LONG_LINE) ? SSE_LONG_LINE : 0u;
+    p.cnt = s.cnt.d.p;
     return p;
 }
 
 int validate_segs(sse_ctx *c, Slot &s, uint32_t n_segs, uint32_t in_bytes) {
     if (n_segs > c->cfg.max_segs || in_bytes > c->cfg.in_arena_bytes) return SSE_ERR_ARG;
     for (uint32_t i = 0; i < n_segs; i++) {
-        const sse_seg &g = s.h_segs[i];
+        const sse_seg &g = s.segs.h.p[i];
         if (g.conn >= c->cfg.max_conns || (g.in_off & 15u) || (uint64_t)g.in_off + g.in_len > in_bytes) return SSE_ERR_ARG;
     }
     return SSE_OK;
 }
 
 int do_upload(sse_ctx *c, Slot &s, uint32_t n_segs, uint32_t in_bytes, cudaStream_t st) {
-    if (n_segs) CU(cudaMemcpyAsync(s.d_segs, s.h_segs, (size_t)n_segs * sizeof(sse_seg), cudaMemcpyHostToDevice, st));
-    if (in_bytes) CU(cudaMemcpyAsync(s.d_in, s.h_in, ((size_t)in_bytes + 15) & ~(size_t)15, cudaMemcpyHostToDevice, st));
+    if (n_segs) CU(cudaMemcpyAsync(s.segs.d.p, s.segs.h.p, (size_t)n_segs * sizeof(sse_seg), cudaMemcpyHostToDevice, st));
+    if (in_bytes) CU(cudaMemcpyAsync(s.d_in, s.h_in.p, ((size_t)in_bytes + 15) & ~(size_t)15, cudaMemcpyHostToDevice, st));
     s.n_segs = n_segs; s.in_bytes = in_bytes;
     (void)c;
     return SSE_OK;
 }
 
 int do_launch(sse_ctx *c, Slot &s, uint32_t n_segs, cudaStream_t st) {
-    CU(cudaMemsetAsync(s.d_ctr, 0, sizeof(Counters), st));
+    CU(cudaMemsetAsync(s.ctr.d.p, 0, sizeof(Counters), st));
     s.cnt_ready = false;
     s.pool_gen = c->pool_gen;
-    if (s.d_cnt) CU(cudaMemsetAsync(s.d_cnt, 0, CN_COUNT * sizeof(unsigned long long), st));
+    if (s.cnt.d.p) CU(cudaMemsetAsync(s.cnt.d.p, 0, CN_COUNT * sizeof(unsigned long long), st));
     if (n_segs) {
         KParams p = make_params(c, s, n_segs);
         int e;
-        if (c->cfg.flags & SSE_FLAG_KERNEL_FUSED) {   // plan + single-pass tile kernel
-            e = sse_launch_fused(p, (void *)st, c->sm_count, c->device);
-            c->launches += 2;
-        }
+        if (c->cfg.flags & SSE_FLAG_KERNEL_FUSED)   // plan + single-pass tile kernel
+            e = sse_launch_fused(p, (void *)st, c->sm_count, c->device, c->launches);
         else {   // default: produce -> sort -> decode (templates / automaton) -> finalize
-            e = sse_launch_produce_kernel(p, (void *)st, c->sm_count);
-            if (e == 0) e = sse_launch_decode_finalize(p, (void *)st, c->sm_count, c->device);
-            c->launches += p.long_line ? 7 : 6;   // produce, bucket hist/scan/scatter, [long-line decode,] decode, finalize
+            e = sse_launch_produce_kernel(p, (void *)st, c->sm_count, c->launches);
+            if (e == 0) e = sse_launch_decode_finalize(p, (void *)st, c->sm_count, c->device, c->launches);
         }
         if (e != 0) { cu_ok((cudaError_t)e, "stream kernel launch"); return SSE_ERR_CUDA; }
     }
@@ -220,26 +264,23 @@ sse_config worst_decode_caps(const sse_ctx *c) {
     return w;
 }
 
-// One decode-stage arena of a slot goes from cap to want elements of T, device and pinned (the slot's stream is idle): grows it
-// (redecode) or gives back what a growth took (sse_trim).
-template <class T> int resize_arena(sse_ctx *c, T *&d, T *&h, uint32_t &cap, uint32_t want) {
-    T *nd = nullptr, *nh = nullptr;
-    if (cudaMalloc((void **)&nd, alloc_bytes<T>(want)) != cudaSuccess) { cudaGetLastError(); return SSE_ERR_NOMEM; }
-    if (cudaHostAlloc((void **)&nh, alloc_bytes<T>(want), cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); cudaFree(nd); return SSE_ERR_NOMEM; }
-    cudaFree(d); cudaFreeHost(h);
-    c->device_bytes += alloc_bytes<T>(want) - alloc_bytes<T>(cap);
-    c->pinned_bytes += alloc_bytes<T>(want) - alloc_bytes<T>(cap);
-    d = nd; h = nh; cap = want;
+// One decode-stage arena of a slot goes to `want` elements, device and pinned (the slot's stream is idle): grows it (redecode) or
+// gives back what a growth took (sse_trim). The new arrays are allocated before the old ones are freed, which stay when that fails.
+template <class T> int resize(sse_ctx *c, Pair<T> &a, uint32_t want) {
+    Pair<T> b;
+    if (!buf_alloc(c, b.d, want) || !buf_alloc(c, b.h, want)) { buf_free(c, b.d); return SSE_ERR_NOMEM; }
+    buf_free(c, a.d); buf_free(c, a.h);
+    a = b;
     return SSE_OK;
 }
 
 // sse_trim: the slot's decode arenas back to the configured capacities (the slot holds no batch, or its stream is idle and its
 // results are no longer lent).
 int trim_arenas(sse_ctx *c, Slot &s) {
-    int rc = SSE_OK;
-    if (s.cap_tcs != c->cfg.max_tcs) rc = resize_arena(c, s.d_tcs, s.h_tcs, s.cap_tcs, c->cfg.max_tcs);
-    if (rc == SSE_OK && s.cap_usages != c->cfg.max_usages) rc = resize_arena(c, s.d_usages, s.h_usages, s.cap_usages, c->cfg.max_usages);
-    if (rc == SSE_OK && s.cap_text != c->cfg.text_arena_bytes) rc = resize_arena(c, s.d_text, s.h_text, s.cap_text, c->cfg.text_arena_bytes);
+    auto back = [&](auto &a, uint32_t n) { return a.cap() == n ? (int)SSE_OK : resize(c, a, n); };
+    int rc = back(s.tcs, c->cfg.max_tcs);
+    if (rc == SSE_OK) rc = back(s.usages, c->cfg.max_usages);
+    if (rc == SSE_OK) rc = back(s.text, c->cfg.text_arena_bytes);
     s.trim = rc != SSE_OK;   // an allocation failed: the next sse_release tries again
     return rc;
 }
@@ -259,46 +300,43 @@ int redecode(sse_ctx *c, Slot &s, Counters &k, cudaStream_t st, uint32_t &grown)
         if (v < need) v = need;
         return (uint32_t)(v > 0xF0000000ull ? 0xF0000000ull : v);
     };
-    auto grow = [&](auto *&d, auto *&h, uint32_t &cap, uint32_t need, uint32_t worst) {
-        const uint32_t n = want(cap, need, worst);
-        return n > cap ? resize_arena(c, d, h, cap, n) : (int)SSE_ERR_NOMEM;
+    auto grow = [&](auto &a, uint32_t need, uint32_t worst) {
+        const uint32_t n = want(a.cap(), need, worst);
+        return n > a.cap() ? resize(c, a, n) : (int)SSE_ERR_NOMEM;
     };
     while (k.status == SSE_ERR_OVERFLOW) {
         const uint32_t ovf = k.overflow & (SSE_OVF_TCS | SSE_OVF_USAGES | SSE_OVF_TEXT);
         if (!ovf) return SSE_ERR_OVERFLOW;   // not reachable: with SSE_FLAG_DEFER only the decode stage fails a batch
         int rc = SSE_OK;
-        if (ovf & SSE_OVF_TCS) rc = grow(s.d_tcs, s.h_tcs, s.cap_tcs, k.n_tcs, w.max_tcs);
-        if (rc == SSE_OK && (ovf & SSE_OVF_USAGES)) rc = grow(s.d_usages, s.h_usages, s.cap_usages, k.n_usages, w.max_usages);
-        if (rc == SSE_OK && (ovf & SSE_OVF_TEXT)) rc = grow(s.d_text, s.h_text, s.cap_text, k.text_bytes, w.text_arena_bytes);
+        if (ovf & SSE_OVF_TCS) rc = grow(s.tcs, k.n_tcs, w.max_tcs);
+        if (rc == SSE_OK && (ovf & SSE_OVF_USAGES)) rc = grow(s.usages, k.n_usages, w.max_usages);
+        if (rc == SSE_OK && (ovf & SSE_OVF_TEXT)) rc = grow(s.text, k.text_bytes, w.text_arena_bytes);
         if (rc != SSE_OK) return rc;
         grown |= ovf;
         // the lane decoder's items start after the long ones (items_sorted[0, n_long)), which the long-line kernel takes again
         k.n_tcs = k.n_usages = k.text_bytes = 0; k.item_ticket = k.n_long; k.long_ticket = 0; k.status = SSE_OK; k.overflow = 0;
-        *s.h_ctr = k;
-        CU(cudaMemcpyAsync(s.d_ctr, s.h_ctr, offsetof(Counters, class_count), cudaMemcpyHostToDevice, st));
-        if (s.d_cnt) {   // the decode counters describe the pass whose records the batch returns
-            CU(cudaMemsetAsync(s.d_cnt + CN_DECODE_FIRST, 0, (CN_COUNT - CN_DECODE_FIRST) * sizeof(unsigned long long), st));
+        *s.ctr.h.p = k;
+        CU(cudaMemcpyAsync(s.ctr.d.p, s.ctr.h.p, CTR_HEAD, cudaMemcpyHostToDevice, st));
+        if (s.cnt.d.p) {   // the decode counters describe the pass whose records the batch returns
+            CU(cudaMemsetAsync(s.cnt.d.p + CN_DECODE_FIRST, 0, (CN_COUNT - CN_DECODE_FIRST) * sizeof(unsigned long long), st));
             s.decode_passes++;
         }
-        if (c->have_last) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
-        const KParams p = make_params(c, s, s.n_segs);
-        const int e = sse_launch_decode(p, (void *)st, c->sm_count, c->device);
+        CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
+        const int e = sse_launch_decode(make_params(c, s, s.n_segs), (void *)st, c->sm_count, c->device, c->launches);
         if (e != 0) { cu_ok((cudaError_t)e, "decode kernel launch"); return SSE_ERR_CUDA; }
-        c->launches += p.long_line ? 2 : 1;
         CU(cudaEventRecord(c->last_kernel, st));
-        c->have_last = true;
-        CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(s.ctr.h.p, s.ctr.d.p, CTR_HEAD, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
-        k = *s.h_ctr;
+        k = *s.ctr.h.p;
     }
     return SSE_OK;
 }
 
 int do_download(sse_ctx *c, Slot &s, sse_result *res, cudaStream_t st) {
-    if (!s.ctr_queued) CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, st));
+    if (!s.ctr_queued) CU(cudaMemcpyAsync(s.ctr.h.p, s.ctr.d.p, CTR_HEAD, cudaMemcpyDeviceToHost, st));
     s.ctr_queued = false;
     CU(cudaStreamSynchronize(st));
-    Counters k = *s.h_ctr;
+    Counters k = *s.ctr.h.p;
     s.pool_short = k.pool_short;
     memset(res, 0, sizeof *res);
     res->n_segs = s.n_segs;
@@ -320,24 +358,21 @@ int do_download(sse_ctx *c, Slot &s, sse_result *res, cudaStream_t st) {
     auto lim = [](uint32_t n, uint32_t cap) { return n < cap ? n : cap; };
     k.n_frames = lim(k.n_frames, c->cfg.max_frames); k.n_recs = lim(k.n_recs, c->cfg.max_recs); k.n_runs = lim(k.n_runs, c->cfg.max_runs);
     k.out_bytes = lim(k.out_bytes, c->cfg.out_arena_bytes); k.n_items = lim(k.n_items, c->cfg.max_recs);
-    k.n_tcs = lim(k.n_tcs, s.cap_tcs); k.n_usages = lim(k.n_usages, s.cap_usages); k.text_bytes = lim(k.text_bytes, s.cap_text);
+    k.n_tcs = lim(k.n_tcs, s.tcs.cap()); k.n_usages = lim(k.n_usages, s.usages.cap()); k.text_bytes = lim(k.text_bytes, s.text.cap());
     res->n_frames = k.n_frames; res->n_recs = k.n_recs; res->n_tcs = k.n_tcs; res->n_usages = k.n_usages;
     res->n_runs = k.n_runs; res->out_bytes = k.out_bytes; res->text_bytes = k.text_bytes;
     res->n_decoded = k.n_items; res->n_derived = 0;
-    if (k.out_bytes) CU(cudaMemcpyAsync(s.h_out, s.d_out, k.out_bytes, cudaMemcpyDeviceToHost, st));
-    if (k.n_frames) CU(cudaMemcpyAsync(s.h_frames, s.d_frames, (size_t)k.n_frames * sizeof(sse_frame), cudaMemcpyDeviceToHost, st));
-    if (k.n_recs) CU(cudaMemcpyAsync(s.h_recs, s.d_recs, (size_t)k.n_recs * sizeof(sse_rec), cudaMemcpyDeviceToHost, st));
-    if (k.n_tcs) CU(cudaMemcpyAsync(s.h_tcs, s.d_tcs, (size_t)k.n_tcs * sizeof(sse_tc), cudaMemcpyDeviceToHost, st));
-    if (k.n_usages) CU(cudaMemcpyAsync(s.h_usages, s.d_usages, (size_t)k.n_usages * sizeof(sse_usage), cudaMemcpyDeviceToHost, st));
-    if (k.text_bytes) CU(cudaMemcpyAsync(s.h_text, s.d_text, k.text_bytes, cudaMemcpyDeviceToHost, st));
-    if (k.n_runs) CU(cudaMemcpyAsync(s.h_runs, s.d_runs, (size_t)k.n_runs * sizeof(sse_run), cudaMemcpyDeviceToHost, st));
-    if (s.n_segs) CU(cudaMemcpyAsync(s.h_segres, s.d_segres, (size_t)s.n_segs * sizeof(sse_seg_result), cudaMemcpyDeviceToHost, st));
-    if (s.d_cnt) CU(cudaMemcpyAsync(s.h_cnt, s.d_cnt, CN_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    auto d2h = [&](auto &a, uint32_t n) {
+        return n ? cudaMemcpyAsync(a.h.p, a.d.p, (size_t)n * sizeof(*a.h.p), cudaMemcpyDeviceToHost, st) : cudaSuccess;
+    };
+    CU(d2h(s.out, k.out_bytes)); CU(d2h(s.frames, k.n_frames)); CU(d2h(s.recs, k.n_recs)); CU(d2h(s.tcs, k.n_tcs));
+    CU(d2h(s.usages, k.n_usages)); CU(d2h(s.text, k.text_bytes)); CU(d2h(s.runs, k.n_runs)); CU(d2h(s.segres, s.n_segs));
+    if (s.cnt.d.p) CU(d2h(s.cnt, CN_COUNT));
     CU(cudaStreamSynchronize(st));
-    s.cnt_ready = s.d_cnt != nullptr;
-    res->out = s.h_out; res->frames = s.h_frames; res->recs = s.h_recs; res->tcs = s.h_tcs; res->usages = s.h_usages;
-    res->text = s.h_text; res->runs = s.h_runs; res->segs = s.h_segres;
-    res->in = s.h_in; res->in_base = in_base_of(c->cfg);
+    s.cnt_ready = s.cnt.d.p != nullptr;
+    res->out = s.out.h.p; res->frames = s.frames.h.p; res->recs = s.recs.h.p; res->tcs = s.tcs.h.p; res->usages = s.usages.h.p;
+    res->text = s.text.h.p; res->runs = s.runs.h.p; res->segs = s.segres.h.p;
+    res->in = s.h_in.p; res->in_base = in_base_of(c->cfg);
     return SSE_OK;
 }
 
@@ -350,8 +385,8 @@ void free_retired(sse_ctx *c, bool all) {
             if (e == cudaErrorNotReady && cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();   // still queued: not an error
             if (e != cudaSuccess) { c->retired[k++] = r; continue; }
         }
-        cudaFree(r.pool); cudaFree(r.stack); cudaFree(r.next); cudaEventDestroy(r.done);
-        c->device_bytes -= pool_bytes(c, r.pages);
+        pool_free(c, r.arrays);
+        cudaEventDestroy(r.done);
     }
     c->retired.resize(k);
 }
@@ -362,41 +397,33 @@ void free_retired(sse_ctx *c, bool all) {
 // were launched with the old arrays) and every later launch is ordered after them and gets the new arrays. When the device
 // cannot allocate them the pool stays as it is and stops growing: its lines fail at the limit as without growth.
 int grow_pool(sse_ctx *c, uint32_t lacked) {
-    const uint32_t cap = c->pool.pool_pages, PB = c->pool.page_bytes;
+    const uint32_t cap = c->pool.pool_pages;
     uint64_t want = (uint64_t)cap * 2u;
     if (want < (uint64_t)cap + lacked) want = (uint64_t)cap + lacked;
     if (want > c->pool_max) want = c->pool_max;
     if (want <= cap) return SSE_OK;
     free_retired(c, false);
-    RetiredPool old{ c->d_pool, c->d_pool_stack, c->d_pool_next, nullptr, cap };
-    uint8_t *pool = nullptr; uint32_t *stack = nullptr, *next = nullptr;
-    bool ok = cudaMalloc((void **)&pool, (size_t)want * PB) == cudaSuccess && cudaMalloc((void **)&stack, (size_t)want * 4) == cudaSuccess &&
-              cudaMalloc((void **)&next, (size_t)want * 4) == cudaSuccess &&
-              cudaEventCreateWithFlags(&old.done, cudaEventDisableTiming) == cudaSuccess;
-    if (!ok) {
-        if (cudaPeekAtLastError() == cudaErrorMemoryAllocation) cudaGetLastError();   // the failed allocation only
-        cudaFree(pool); cudaFree(stack); cudaFree(next);
-        if (old.done) cudaEventDestroy(old.done);
+    cudaStream_t st = c->ctl_stream;
+    RetiredPool old{ c->pool_arrays, nullptr };
+    PoolArrays grown;
+    if (!pool_alloc(c, grown, (uint32_t)want) || cudaEventCreateWithFlags(&old.done, cudaEventDisableTiming) != cudaSuccess) {
+        if (cudaPeekAtLastError() == cudaErrorMemoryAllocation) cudaGetLastError();   // as buf_alloc does, for the event
+        pool_free(c, grown);
         c->pool_max = cap;
-        if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
-        CU(cudaMemsetAsync(&c->d_pool_hdr->grow, 0, sizeof(uint32_t), c->ctl_stream));
-        CU(cudaEventRecord(c->last_kernel, c->ctl_stream));
-        c->have_last = true;
+        CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
+        CU(cudaMemsetAsync(&c->pool_hdr.p->grow, 0, sizeof(uint32_t), st));
+        CU(cudaEventRecord(c->last_kernel, st));
         return SSE_OK;
     }
-    cudaStream_t st = c->ctl_stream;
-    if (c->have_last) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
-    CU(cudaMemcpyAsync(pool, c->d_pool, (size_t)cap * PB, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(stack, c->d_pool_stack, (size_t)cap * 4, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(next, c->d_pool_next, (size_t)cap * 4, cudaMemcpyDeviceToDevice, st));
+    auto copy = [&](auto &to, const auto &from) { return cudaMemcpyAsync(to.p, from.p, from.n * sizeof(*from.p), cudaMemcpyDeviceToDevice, st); };
+    CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
+    CU(copy(grown.pages, old.arrays.pages)); CU(copy(grown.stack, old.arrays.stack)); CU(copy(grown.next, old.arrays.next));
     CU(cudaEventRecord(old.done, st));
     c->retired.push_back(old);
-    c->device_bytes += pool_bytes(c, (uint32_t)want);
-    c->d_pool = pool; c->d_pool_stack = stack; c->d_pool_next = next; c->pool.pool_pages = (uint32_t)want;
+    c->pool_arrays = grown; c->pool.pool_pages = (uint32_t)want;
     c->pool_gen++;
     if (!cu_ok((cudaError_t)sse_launch_pool_extend(pool_params(c), cap, want < c->pool_max, st), "pool extend kernel")) return SSE_ERR_CUDA;
     CU(cudaEventRecord(c->last_kernel, st));
-    c->have_last = true;
     return SSE_OK;
 }
 
@@ -407,29 +434,21 @@ int grow_pool(sse_ctx *c, uint32_t lacked) {
 // for the queued repack, their last reader).
 int trim_pool(sse_ctx *c, uint32_t min_pages) {
     cudaStream_t st = c->ctl_stream;
-    CU(cudaMemcpyAsync(c->h_pool_hdr, c->d_pool_hdr, sizeof(PoolHdr), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(c->h_pool_hdr.p, c->pool_hdr.p, sizeof(PoolHdr), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     free_retired(c, false);   // every growth's copy is done
-    const uint32_t cap = c->pool.pool_pages, held = cap - c->h_pool_hdr->n_free, PB = c->pool.page_bytes;
+    const uint32_t cap = c->pool.pool_pages, held = cap - c->h_pool_hdr.p->n_free;
     uint32_t want = min_pages > held ? min_pages : held;
     if (want < 1) want = 1;
     if (want >= cap) return SSE_OK;
-    uint8_t *pool = nullptr; uint32_t *stack = nullptr, *next = nullptr;
-    if (cudaMalloc((void **)&pool, (size_t)want * PB) != cudaSuccess || cudaMalloc((void **)&stack, (size_t)want * 4) != cudaSuccess ||
-        cudaMalloc((void **)&next, (size_t)want * 4) != cudaSuccess) {
-        if (cudaPeekAtLastError() == cudaErrorMemoryAllocation) cudaGetLastError();   // the failed allocation only
-        cudaFree(pool); cudaFree(stack); cudaFree(next);
-        return SSE_ERR_NOMEM;
-    }
-    KParams p = pool_params(c);   // the old arrays
-    const int e = sse_launch_pool_repack(p, pool, stack, next, held, want, want < c->pool_max, c->sm_count, st);
-    if (!cu_ok((cudaError_t)e, "pool repack kernels")) { cudaFree(pool); cudaFree(stack); cudaFree(next); return SSE_ERR_CUDA; }
+    PoolArrays small;
+    if (!pool_alloc(c, small, want)) return SSE_ERR_NOMEM;
+    const int e = sse_launch_pool_repack(pool_params(c), small.pages.p, small.stack.p, small.next.p, held, want, want < c->pool_max,
+                                         c->sm_count, st);
+    if (!cu_ok((cudaError_t)e, "pool repack kernels")) { pool_free(c, small); return SSE_ERR_CUDA; }
     CU(cudaEventRecord(c->last_kernel, st));
-    c->have_last = true;
-    cudaFree(c->d_pool); cudaFree(c->d_pool_stack); cudaFree(c->d_pool_next);
-    c->device_bytes += pool_bytes(c, want);
-    c->device_bytes -= pool_bytes(c, cap);
-    c->d_pool = pool; c->d_pool_stack = stack; c->d_pool_next = next; c->pool.pool_pages = want;
+    pool_free(c, c->pool_arrays);
+    c->pool_arrays = small; c->pool.pool_pages = want;
     c->pool_gen++;            // a batch launched before the trim reports its lack against the old pool: it does not grow this one
     return SSE_OK;
 }
@@ -556,16 +575,16 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
     bool ok = true;
     ok = ok && cu_ok(cudaStreamCreateWithFlags(&c->ctl_stream, cudaStreamNonBlocking), "cudaStreamCreate");
     ok = ok && cu_ok(cudaEventCreateWithFlags(&c->last_kernel, cudaEventDisableTiming), "cudaEventCreate");
-    ok = ok && dalloc(c, c->d_conns, cfg->max_conns);
-    ok = ok && dalloc(c, c->d_carry, (size_t)cfg->max_conns * cfg->carry_slot_bytes);
-    ok = ok && cu_ok(cudaMemset(c->d_conns, 0, (size_t)cfg->max_conns * sizeof(ConnState)), "cudaMemset");
-    ok = ok && dalloc(c, c->d_tcache, sse_fused_tcache_words());
-    ok = ok && cu_ok(cudaMemset(c->d_tcache, 0, (size_t)sse_fused_tcache_words() * sizeof(uint32_t)), "cudaMemset");
+    // every wait on last_kernel has an event to wait for
+    ok = ok && cu_ok(cudaEventRecord(c->last_kernel, c->ctl_stream), "cudaEventRecord");
+    ok = ok && buf_alloc(c, c->conns, cfg->max_conns) && buf_alloc(c, c->carry, (size_t)cfg->max_conns * cfg->carry_slot_bytes);
+    ok = ok && cu_ok(cudaMemset(c->conns.p, 0, (size_t)cfg->max_conns * sizeof(ConnState)), "cudaMemset");
+    ok = ok && buf_alloc(c, c->tcache, sse_fused_tcache_words());
+    ok = ok && cu_ok(cudaMemset(c->tcache.p, 0, (size_t)sse_fused_tcache_words() * sizeof(uint32_t)), "cudaMemset");
     if (ok && pool.pool_pages) {
-        ok = ok && dalloc(c, c->d_pool, (size_t)pool.pool_pages * pool.page_bytes) && dalloc(c, c->d_pool_hdr, 1);
-        ok = ok && dalloc(c, c->d_pool_stack, pool.pool_pages) && dalloc(c, c->d_pool_next, pool.pool_pages);
-        ok = ok && dalloc(c, c->d_pool_chain, cfg->max_conns) && halloc(c, c->h_pool_hdr, 1);
-        ok = ok && cu_ok(cudaMemset(c->d_pool_hdr, 0, sizeof(PoolHdr)), "cudaMemset");
+        ok = pool_alloc(c, c->pool_arrays, pool.pool_pages) && buf_alloc(c, c->pool_hdr, 1) && buf_alloc(c, c->pool_chain, cfg->max_conns) &&
+             buf_alloc(c, c->h_pool_hdr, 1);
+        ok = ok && cu_ok(cudaMemset(c->pool_hdr.p, 0, sizeof(PoolHdr)), "cudaMemset");
         ok = ok && cu_ok((cudaError_t)sse_launch_pool_reset(pool_params(c), SSE_NONE, c->ctl_stream), "pool reset kernel");
         ok = ok && cu_ok(cudaStreamSynchronize(c->ctl_stream), "cudaStreamSynchronize");
     }
@@ -574,23 +593,9 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
         if (!ok) break;
         ok = ok && cu_ok(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking), "cudaStreamCreate");
         ok = ok && cu_ok(cudaEventCreateWithFlags(&s.kernel_done, cudaEventDisableTiming), "cudaEventCreate");
-        ok = ok && halloc(c, s.h_in, (size_t)cfg->in_arena_bytes + 16) && halloc(c, s.h_segs, cfg->max_segs);
-        ok = ok && halloc(c, s.h_out, cfg->out_arena_bytes) && halloc(c, s.h_frames, cfg->max_frames) && halloc(c, s.h_recs, cfg->max_recs);
-        ok = ok && halloc(c, s.h_tcs, cfg->max_tcs) && halloc(c, s.h_usages, cfg->max_usages) && halloc(c, s.h_text, cfg->text_arena_bytes);
-        ok = ok && halloc(c, s.h_runs, cfg->max_runs) && halloc(c, s.h_segres, cfg->max_segs) && halloc(c, s.h_ctr, 1);
-        ok = ok && dalloc(c, s.d_segs, cfg->max_segs);
-        ok = ok && dalloc(c, s.d_out, (size_t)in_base_of(*cfg) + cfg->in_arena_bytes + 16);
-        if (ok) s.d_in = s.d_out + in_base_of(*cfg);
-        // recs[max_recs]: the sink record of the empty work items a deferred allocation leaves (SSE_FLAG_DEFER), never returned
-        ok = ok && dalloc(c, s.d_frames, cfg->max_frames) && dalloc(c, s.d_recs, (size_t)cfg->max_recs + 1);
-        s.cap_tcs = cfg->max_tcs; s.cap_usages = cfg->max_usages; s.cap_text = cfg->text_arena_bytes;
-        ok = ok && dalloc(c, s.d_tcs, cfg->max_tcs) && dalloc(c, s.d_usages, cfg->max_usages) && dalloc(c, s.d_text, cfg->text_arena_bytes);
-        ok = ok && dalloc(c, s.d_runs, cfg->max_runs) && dalloc(c, s.d_segres, cfg->max_segs) && dalloc(c, s.d_ctr, 1);
-        ok = ok && dalloc(c, s.d_items, cfg->max_recs) && dalloc(c, s.d_segterm, cfg->max_segs);
-        ok = ok && dalloc(c, s.d_items2, cfg->max_recs);
-        ok = ok && dalloc(c, s.d_tiles, (size_t)cfg->max_segs + 64);
-        if (ok && (cfg->flags & SSE_FLAG_COUNTERS))
-            ok = dalloc(c, s.d_cnt, CN_COUNT) && halloc(c, s.h_cnt, CN_COUNT) && cu_ok(cudaMemset(s.d_cnt, 0, CN_COUNT * sizeof(unsigned long long)), "cudaMemset");
+        slot_buffers(s, *cfg, [&](auto &b, size_t n) { ok = ok && buf_alloc(c, b, n); });
+        if (ok) s.d_in = s.out.d.p + in_base_of(*cfg);
+        if (ok && s.cnt.d.p) ok = cu_ok(cudaMemset(s.cnt.d.p, 0, CN_COUNT * sizeof(unsigned long long)), "cudaMemset");
     }
     if (!ok) { sse_destroy(c); return SSE_ERR_CUDA; }
     *out = c;
@@ -602,10 +607,9 @@ void sse_destroy(sse_ctx *c) {
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
     free_retired(c, true);
-    for (auto &s : c->slots) free_slot(s);
-    cudaFree(c->d_conns); cudaFree(c->d_carry); cudaFree(c->d_tcache);
-    cudaFree(c->d_pool); cudaFree(c->d_pool_hdr); cudaFree(c->d_pool_stack); cudaFree(c->d_pool_next); cudaFree(c->d_pool_chain);
-    cudaFreeHost(c->h_pool_hdr);
+    for (auto &s : c->slots) free_slot(c, s);
+    buf_free(c, c->conns); buf_free(c, c->carry); buf_free(c, c->tcache);
+    pool_free(c, c->pool_arrays); buf_free(c, c->pool_hdr); buf_free(c, c->pool_chain); buf_free(c, c->h_pool_hdr);
     if (c->ctl_stream) cudaStreamDestroy(c->ctl_stream);
     if (c->last_kernel) cudaEventDestroy(c->last_kernel);
     delete c;
@@ -618,7 +622,7 @@ int sse_acquire(sse_ctx *c, int *slot, sse_batch *batch) {
             Slot &s = c->slots[i];
             s.state = SLOT_ACQUIRED;
             *slot = (int)i;
-            batch->in_arena = s.h_in; batch->segs = s.h_segs;
+            batch->in_arena = s.h_in.p; batch->segs = s.segs.h.p;
             batch->in_arena_bytes = c->cfg.in_arena_bytes; batch->max_segs = c->cfg.max_segs;
             return SSE_OK;
         }
@@ -635,13 +639,12 @@ int sse_submit(sse_ctx *c, int slot, uint32_t n_segs, uint32_t in_bytes) {
     CU(cudaSetDevice(c->device));
     rc = do_upload(c, s, n_segs, in_bytes, s.stream);
     if (rc != SSE_OK) return rc;
-    if (c->have_last) CU(cudaStreamWaitEvent(s.stream, c->last_kernel, 0));   // per-connection FIFO across batches
+    CU(cudaStreamWaitEvent(s.stream, c->last_kernel, 0));   // per-connection FIFO across batches
     rc = do_launch(c, s, n_segs, s.stream);
     if (rc != SSE_OK) return rc;
     CU(cudaEventRecord(c->last_kernel, s.stream));
-    c->have_last = true;
     // the counters sse_collect reads first travel now, so that a slot sse_poll reports done is one copy away from its result
-    CU(cudaMemcpyAsync(s.h_ctr, s.d_ctr, offsetof(Counters, class_count), cudaMemcpyDeviceToHost, s.stream));
+    CU(cudaMemcpyAsync(s.ctr.h.p, s.ctr.d.p, CTR_HEAD, cudaMemcpyDeviceToHost, s.stream));
     CU(cudaEventRecord(s.kernel_done, s.stream));
     s.ctr_queued = true;
     s.state = SLOT_SUBMITTED;
@@ -686,7 +689,7 @@ int sse_release(sse_ctx *c, int slot) {
 int sse_trim(sse_ctx *c, uint32_t min_pool_pages) {
     if (!c || !(c->cfg.flags & SSE_FLAG_DEFER) || min_pool_pages == SSE_NONE) return SSE_ERR_ARG;
     CU(cudaSetDevice(c->device));
-    if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
+    CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
     CU(cudaStreamSynchronize(c->ctl_stream));
     int rc = SSE_OK;
     if (c->pool.pool_pages && c->pool_max) rc = trim_pool(c, min_pool_pages);
@@ -711,12 +714,11 @@ int sse_memory_held(sse_ctx *c, uint64_t *device_bytes, uint64_t *pinned_bytes) 
 int sse_reset_conn(sse_ctx *c, uint32_t conn) {
     if (!c || conn >= c->cfg.max_conns) return SSE_ERR_ARG;
     CU(cudaSetDevice(c->device));
-    if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
+    CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
     if (c->pool.pool_pages) {   // the connection's pages go back to the pool with its state
         if (!cu_ok((cudaError_t)sse_launch_pool_reset(pool_params(c), conn, c->ctl_stream), "pool reset kernel")) return SSE_ERR_CUDA;
-    } else CU(cudaMemsetAsync(c->d_conns + conn, 0, sizeof(ConnState), c->ctl_stream));
+    } else CU(cudaMemsetAsync(c->conns.p + conn, 0, sizeof(ConnState), c->ctl_stream));
     CU(cudaEventRecord(c->last_kernel, c->ctl_stream));   // later kernels are ordered after the reset
-    c->have_last = true;
     return SSE_OK;
 }
 
@@ -724,10 +726,10 @@ int sse_reset_all(sse_ctx *c, void *cuda_stream) {
     if (!c) return SSE_ERR_ARG;
     CU(cudaSetDevice(c->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->ctl_stream;
-    if (!cuda_stream && c->have_last) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
-    CU(cudaMemsetAsync(c->d_conns, 0, (size_t)c->cfg.max_conns * sizeof(ConnState), st));
+    if (!cuda_stream) CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
+    CU(cudaMemsetAsync(c->conns.p, 0, (size_t)c->cfg.max_conns * sizeof(ConnState), st));
     if (c->pool.pool_pages && !cu_ok((cudaError_t)sse_launch_pool_reset(pool_params(c), SSE_NONE, st), "pool reset kernel")) return SSE_ERR_CUDA;
-    if (!cuda_stream) { CU(cudaEventRecord(c->last_kernel, st)); c->have_last = true; }
+    if (!cuda_stream) CU(cudaEventRecord(c->last_kernel, st));
     return SSE_OK;
 }
 
@@ -736,11 +738,11 @@ int sse_line_pool_stats(sse_ctx *c, uint32_t *pages_in_use, uint32_t *pages_high
     *pages_in_use = *pages_high_water = 0;
     if (!c->pool.pool_pages) return SSE_OK;
     CU(cudaSetDevice(c->device));
-    if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
-    CU(cudaMemcpyAsync(c->h_pool_hdr, c->d_pool_hdr, sizeof(PoolHdr), cudaMemcpyDeviceToHost, c->ctl_stream));
+    CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
+    CU(cudaMemcpyAsync(c->h_pool_hdr.p, c->pool_hdr.p, sizeof(PoolHdr), cudaMemcpyDeviceToHost, c->ctl_stream));
     CU(cudaStreamSynchronize(c->ctl_stream));
-    *pages_in_use = c->pool.pool_pages - c->h_pool_hdr->n_free;
-    *pages_high_water = c->h_pool_hdr->high_water;
+    *pages_in_use = c->pool.pool_pages - c->h_pool_hdr.p->n_free;
+    *pages_high_water = c->h_pool_hdr.p->high_water;
     return SSE_OK;
 }
 
@@ -749,10 +751,9 @@ int sse_line_pool_set_growth(sse_ctx *c, uint32_t max_pages) {
         (max_pages && max_pages < c->pool.pool_pages)) return SSE_ERR_ARG;
     CU(cudaSetDevice(c->device));
     c->pool_max = max_pages;
-    if (c->have_last) CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
-    CU(cudaMemsetAsync(&c->d_pool_hdr->grow, max_pages > c->pool.pool_pages ? 1 : 0, sizeof(uint32_t), c->ctl_stream));
+    CU(cudaStreamWaitEvent(c->ctl_stream, c->last_kernel, 0));
+    CU(cudaMemsetAsync(&c->pool_hdr.p->grow, max_pages > c->pool.pool_pages ? 1 : 0, sizeof(uint32_t), c->ctl_stream));
     CU(cudaEventRecord(c->last_kernel, c->ctl_stream));   // later kernels see the new setting
-    c->have_last = true;
     return SSE_OK;
 }
 
@@ -789,23 +790,13 @@ int sse_download(sse_ctx *c, int slot, sse_result *res, void *cuda_stream) {
     return do_download(c, s, res, cuda_stream ? (cudaStream_t)cuda_stream : s.stream);
 }
 
-/* debugging aid (tools/dump_templates.py): the fused kernel's template cache, as sse_fused.cu lays it out */
-int sse_debug_tcache(sse_ctx *c, uint32_t *out, uint32_t words) {
-    if (!c || !out || !c->d_tcache) return SSE_ERR_ARG;
-    CU(cudaSetDevice(c->device));
-    CU(cudaDeviceSynchronize());
-    const uint32_t n = words < sse_fused_tcache_words() ? words : sse_fused_tcache_words();
-    CU(cudaMemcpy(out, c->d_tcache, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    return (int)n;
-}
-
 int sse_counters_read(sse_ctx *c, int slot, sse_counters *out) {
     if (!c || !out || out->struct_size != sizeof(sse_counters) || !(c->cfg.flags & SSE_FLAG_COUNTERS) || slot < 0 ||
         slot >= (int)c->slots.size()) return SSE_ERR_ARG;
     const Slot &s = c->slots[slot];
     if ((s.state != SLOT_COLLECTED && s.state != SLOT_ACQUIRED) || !s.cnt_ready) return SSE_ERR_BUSY;
     out->decode_passes = s.decode_passes;
-    memcpy(&out->p_segments, s.h_cnt, CN_COUNT * sizeof(uint64_t));
+    memcpy(&out->p_segments, s.cnt.h.p, CN_COUNT * sizeof(uint64_t));
     return SSE_OK;
 }
 

@@ -470,7 +470,7 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
 } // namespace
 
 template <bool DEFER, bool CNT>
-static int launch_stream_kernel(const KParams &p, void *stream, int sm_count) {
+static int launch_stream_kernel(const KParams &p, void *stream, int sm_count, uint64_t &launches) {
     static bool attr_set = false;
     static int ctas_per_sm = 0;
     const size_t smem = sizeof(CtaSmem);
@@ -487,10 +487,13 @@ static int launch_stream_kernel(const KParams &p, void *stream, int sm_count) {
     int need = (int)((p.n_segs + WARPS_PER_CTA - 1) / WARPS_PER_CTA);
     if (need < grid) grid = need > 0 ? need : 1;
     sse_stream_kernel<DEFER, CNT><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(p);
+    launches++;
     return (int)cudaGetLastError();
 }
 
-int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count) {
-    if (p.cnt) return (p.flags & SSE_FLAG_DEFER) ? launch_stream_kernel<true, true>(p, stream, sm_count) : launch_stream_kernel<false, true>(p, stream, sm_count);
-    return (p.flags & SSE_FLAG_DEFER) ? launch_stream_kernel<true, false>(p, stream, sm_count) : launch_stream_kernel<false, false>(p, stream, sm_count);
+int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count, uint64_t &launches) {
+    if (p.cnt) return (p.flags & SSE_FLAG_DEFER) ? launch_stream_kernel<true, true>(p, stream, sm_count, launches)
+                                                 : launch_stream_kernel<false, true>(p, stream, sm_count, launches);
+    return (p.flags & SSE_FLAG_DEFER) ? launch_stream_kernel<true, false>(p, stream, sm_count, launches)
+                                      : launch_stream_kernel<false, false>(p, stream, sm_count, launches);
 }

@@ -748,9 +748,9 @@ int sse_v2_prepare(int device) {
 
 // the decode kernels the context's flags select: templates (KParams.tcache) and counters (KParams.cnt). The long-line kernel
 // goes first, alone: the lane decoder fills every SM, so the two could not run side by side.
-static void launch_decode_kernel(const KParams &p, cudaStream_t st, int sm_count, int device) {
+static void launch_decode_kernel(const KParams &p, cudaStream_t st, int sm_count, int device, uint64_t &launches) {
     const DfaTables *t = g_tables_dev[device];
-    if (p.long_line) sse_launch_long_decode(p, t, (void *)st, sm_count, device);
+    if (p.long_line) { sse_launch_long_decode(p, t, (void *)st, sm_count, device); launches++; }
     if (p.cnt) {
         if (p.tcache) sse_decode_kernel<true, true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
         else sse_decode_kernel<false, true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
@@ -758,26 +758,29 @@ static void launch_decode_kernel(const KParams &p, cudaStream_t st, int sm_count
         if (p.tcache) sse_decode_kernel<true, false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
         else sse_decode_kernel<false, false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
     }
+    launches++;
 }
 
-int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device) {
+int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches) {
     sse_bucket_hist_kernel<<<sm_count * 2, 512, 0, (cudaStream_t)stream>>>(p);
     sse_bucket_scan_kernel<<<1, SCAN_TPB, 0, (cudaStream_t)stream>>>(p);
     sse_bucket_scatter_kernel<<<sm_count * 2, SCATTER_TPB, 0, (cudaStream_t)stream>>>(p);
-    launch_decode_kernel(p, (cudaStream_t)stream, sm_count, device);
+    launches += 3;
+    launch_decode_kernel(p, (cudaStream_t)stream, sm_count, device, launches);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return (int)e;
     const int tpb = 256;
     if (p.cnt) sse_finalize_kernel<true><<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
     else sse_finalize_kernel<false><<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
+    launches++;
     return (int)cudaGetLastError();
 }
 
 // SSE_FLAG_DEFER, after the tool-call / usage / text arenas of a batch grew: the decode stage again over the items the sort left
 // in items_sorted (the caller has reset the decode counters). Records are rewritten whole, so a second pass gives the records a
 // single pass with large enough arenas gives.
-int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device) {
-    launch_decode_kernel(p, (cudaStream_t)stream, sm_count, device);
+int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches) {
+    launch_decode_kernel(p, (cudaStream_t)stream, sm_count, device, launches);
     return (int)cudaGetLastError();
 }
 

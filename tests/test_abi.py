@@ -1,7 +1,10 @@
-"""CPU: the C-ABI library loads, exports every symbol include/sse_gpu.h declares, has the documented struct
+"""CPU: the C-ABI library loads, exports exactly the symbols include/sse_gpu.h and include/sse_gateway.h declare, has the documented struct
 layouts, and fails loudly without a CUDA device (no CPU fallback). No compute calls here."""
 import ctypes as C
 import os
+import re
+import shutil
+import subprocess
 
 import pytest
 
@@ -21,6 +24,13 @@ def test_exports_every_declared_symbol():
     assert len(gw) >= 12
     for n in gw:
         assert hasattr(L, n), f"{n} is declared in include/sse_gateway.h but not exported"
+    # and nothing else: every sse_* / ssegw_* symbol the library exports is declared by one of the two headers
+    nm = shutil.which("nm")
+    if nm is None:
+        pytest.skip("nm not available")
+    out = subprocess.run([nm, "-D", "--defined-only", A.lib_path()], capture_output=True, text=True, check=True).stdout
+    exported = {f[-1] for f in map(str.split, out.splitlines()) if f and re.match(r"sse(gw)?_", f[-1])}
+    assert exported == set(names) | set(gw)
 
 
 def test_struct_layouts_match_header():
@@ -75,8 +85,6 @@ def test_no_device_is_an_error_not_a_fallback():
 
 
 def test_sass_is_sm90a():
-    import shutil
-    import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
