@@ -68,6 +68,17 @@ def stream_with(line, kind):
     return body + chunk(b"bye", '"stop"') + USAGE + b"data: [DONE]\n\n"
 
 
+def burst(n, rng, size=200_000, kinds=("toolcall", "content", "terminal")):
+    """n streams, each with one long line of about `size` bytes (1,009 more per stream), its kind taken from kinds in turn."""
+    return [stream_with(long_line(kinds[i % len(kinds)], size + 1009 * i, rng), kinds[i % len(kinds)]) for i in range(n)]
+
+
+def holder(rng, size, kind="toolcall"):
+    """A stream with a long line, and where to cut it so that its connection holds `size // 2` bytes of that line in pages."""
+    body = stream_with(long_line(kind, size, rng), kind)
+    return body, len(chunk(b"Hello")) + len(chunk(b"world")) + size // 2
+
+
 def filler_payload(kind: str, n: int) -> bytes:
     """A valid chunk of about n bytes: "strings" carries them in a plain content string. "nostring" is exactly n bytes of a
     number array under a key the decoder does not know (below 16 bytes: a number), so its lane is never inside a string."""

@@ -3,17 +3,13 @@ one batch and in pieces, under SSE_FLAG_DEFER at tiny capacities, with 65,534-65
 the gateway. The verdict is tests/util.py::check_folds: the oracle's agent state and telemetry, telemetry's irregular pieces
 (DESIGN.md §5, deviation 4) finishing with 1, and SSE_ERR_UNDECODED from both feeds in the piece that completes the first line
 past the nesting limit."""
-import ctypes as C
-
-import numpy as np
 import pytest
 
 from inference_gateway_b200 import SseEngine, _abi as A, synth
 from inference_gateway_b200.gateway import Gateway
-from inference_gateway_b200.synth import random_cuts
-from oracle import orc
 from tests import folds
-from tests.util import ENGINES, TINY_DECODE, TINY_PRODUCE, check_agent, check_streams, run_deferred, run_streams
+from tests.gateway_drive import Session, check_sessions, drive, gateway_config
+from tests.util import ENGINES, TINY_DECODE, TINY_PRODUCE, check_streams, run_deferred, run_streams
 
 pytestmark = pytest.mark.gpu
 
@@ -84,71 +80,17 @@ def test_saturated_tool_call_chains(eng, mode):
 
 
 # ------------------------------------------------------------------ the gateway's agent path on the same streams
-N_SLOTS = 4
-
-
-def drive(g, bodies, seed, max_ticks=3000):
-    """Mode R streams written in seeded pieces, one piece per stream and tick, closed after their last piece; pumps until every
-    channel is closed. Returns (frames per stream, stream ids)."""
-    rng = np.random.default_rng(seed)
-    sids = [g.stream_chat_completions(R) for _ in bodies]
-    queue = [random_cuts(rng, b, int(rng.integers(1, 7))) for b in bodies]
-    frames, eof, left, closed = [[] for _ in bodies], [False] * len(bodies), [b""] * len(bodies), [False] * len(bodies)
-    for _ in range(max_ticks):
-        for i, s in enumerate(sids):
-            if not left[i] and queue[i]:
-                left[i] = queue[i].pop(0)
-            if left[i]:
-                left[i] = left[i][g.upstream_write(s, left[i]):]
-        g.pump()
-        for i, s in enumerate(sids):
-            if not closed[i] and not left[i] and not queue[i]:
-                g.upstream_close(s)
-                closed[i] = True
-            try:
-                while (f := g.recv(s)) is not None:
-                    frames[i].append(f)
-            except EOFError:
-                eof[i] = True
-        if all(eof):
-            break
-    else:
-        raise AssertionError("streams still open after max_ticks")
-    assert g.flush() >= 0
-    return frames, sids
-
-
-@pytest.mark.parametrize("depth", [1, N_SLOTS])
+@pytest.mark.parametrize("depth", [1, 4])
 @pytest.mark.parametrize("devices", [[0], [0, 0]], ids=lambda d: f"ctx{len(d)}")
 def test_gateway_agent_on_adversarial_streams(devices, depth):
+    """Untapped mode R streams: a stream is failed in the batch that holds its first line past the nesting limit, so its
+    channel ends after a prefix of the oracle's frames that reaches that line (check_sessions)."""
     c = folds.corpus(seed=2, n_adv=48)
-    b = c["adversarial"] + c["tricky"] + c["merge"]
-    cfg = A.Config()
-    A.load().sse_worst_case_config(C.byref(cfg), len(b), 1 << 20)
-    cfg.n_slots = N_SLOTS
-    g = Gateway(config=cfg, devices=devices, depth=depth)
+    sessions = [Session([b], R, tap=False) for b in c["adversarial"] + c["tricky"] + c["merge"]]
+    g = Gateway(config=gateway_config(len(sessions), worst_case=True), devices=devices, depth=depth)
     try:
-        frames, sids = drive(g, b, seed=depth)
-        n_failed = 0
-        for i, (body, got, s) in enumerate(zip(b, frames, sids)):
-            v = orc.reframe(body)
-            want = [l.out for l in v.lines if l.kind == orc.L_EMITTED]
-            # frames up to and including the first line past the nesting limit (None: no such line)
-            upto, n = None, 0
-            for l in v.lines:
-                n += l.kind == orc.L_EMITTED
-                if l.kind != orc.L_UNREAD and l.depth_limited:
-                    upto = n
-                    break
-            label = f"devices {devices} depth {depth} stream {i}"
-            if upto is None:
-                assert got == want, f"{label}: {len(got)} frames, oracle {len(want)}"
-                check_agent(g.agent_state(s), v, label)
-            else:
-                # the stream is failed in the batch that holds its first line past the nesting limit: its channel ends after a
-                # prefix of the oracle's frames that reaches that line
-                n_failed += 1
-                assert upto <= len(got) <= len(want) and got == want[:len(got)], f"{label}: not a prefix through the line"
-        assert n_failed
+        assert drive(g, sessions, seed=depth, max_ticks=3000) >= 0
     finally:
         g.close()
+    n_limited, _ = check_sessions(sessions, f"devices {devices} depth {depth}")
+    assert n_limited

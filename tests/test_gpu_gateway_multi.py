@@ -1,17 +1,14 @@
 """GPU: the gateway over several contexts with batches in flight (ssegw_new_multi). Streams are cut into seeded pieces and
 written over many ticks; every stream's delivered frames, agent content, tool calls, finish and has_tool_calls are compared
 with the CPU oracle and with a one-context, depth-1 gateway fed the same pieces."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 from inference_gateway_b200 import _abi as A, synth
 from inference_gateway_b200.gateway import Gateway
-from inference_gateway_b200.synth import random_cuts
-from oracle import orc
 from tests.corpus import adversarial_bodies
-from tests.util import TINY_PRODUCE, check_agent
+from tests.gateway_drive import Session, check_sessions, drive, gateway_config
+from tests.util import TINY_PRODUCE
 
 pytestmark = pytest.mark.gpu
 
@@ -20,77 +17,14 @@ RAW = -1                      # the raw proxy loop: ssegw_proxy_stream / ssegw_p
 N_SLOTS = 4
 
 
-def config(conns, batch=1 << 18, flags=0, **caps):
-    cfg = A.Config()
-    A.load().sse_default_config(C.byref(cfg), conns, batch)
-    cfg.n_slots = N_SLOTS
-    cfg.flags = flags
-    for k, v in caps.items():
-        setattr(cfg, k, v)
-    return cfg
+def sessions(bodies, modes):
+    """One untapped session per body; RAW reads through the raw proxy loop."""
+    return [Session([b], P, route="proxy", tap=False) if m == RAW else Session([b], m, tap=False) for b, m in zip(bodies, modes)]
 
 
-class Out:
-    def __init__(self, mode):
-        self.mode, self.frames, self.eof, self.agent = mode, [], False, None
-
-
-def drain(g, sid, o):
-    fn = g.proxy_step if o.mode == RAW else g.recv
-    try:
-        while (e := fn(sid)) is not None:
-            o.frames.append(e)
-    except EOFError:
-        o.eof = True
-
-
-def drive(g, bodies, modes, n_pieces=6, seed=0, max_ticks=5000):
-    """Opens one stream per body (in order), writes each body in seeded pieces, one piece per stream and tick, closes the
-    upstream right after the pump that took its last piece (its batch may still be in flight), and pumps until every channel
-    is closed. Returns ([Out], stream ids)."""
-    rng = np.random.default_rng(seed)
-    sids = [g.proxy_stream() if m == RAW else g.stream_chat_completions(m) for m in modes]
-    outs = [Out(m) for m in modes]
-    queue = [random_cuts(rng, b, int(rng.integers(1, n_pieces + 1))) for b in bodies]
-    left = [b"" for _ in bodies]
-    closed = [False] * len(bodies)
-    for _ in range(max_ticks):
-        for i, sid in enumerate(sids):
-            if not left[i] and queue[i]:
-                left[i] = queue[i].pop(0)
-            if left[i]:
-                left[i] = left[i][g.upstream_write(sid, left[i]):]
-        g.pump()
-        for i, sid in enumerate(sids):
-            if not closed[i] and not left[i] and not queue[i]:
-                g.upstream_close(sid)
-                closed[i] = True
-            drain(g, sid, outs[i])
-        if all(o.eof for o in outs):
-            break
-    else:
-        raise AssertionError("streams still open after max_ticks")
-    assert g.flush() == 0
-    for i, sid in enumerate(sids):
-        if modes[i] == R:
-            outs[i].agent = g.agent_state(sid)
-    return outs, sids
-
-
-def check_oracle(bodies, modes, outs, label):
-    for i, (b, m, o) in enumerate(zip(bodies, modes, outs)):
-        if m == R:
-            v = orc.reframe(b)
-            want = [l.out for l in v.lines if l.kind == orc.L_EMITTED]
-            check_agent(o.agent, v, f"{label} stream {i}")
-        else:
-            want = [l.out for l in orc.passthrough(b, parse=bool(m & A.MODE_PARSE)).lines]
-        assert o.frames == want, f"{label} stream {i} mode {m}: {len(o.frames)} frames, oracle {len(want)}"
-
-
-def check_same(outs, ref, label):
-    for i, (o, r) in enumerate(zip(outs, ref)):
-        assert o.frames == r.frames and o.agent == r.agent, f"{label} stream {i} differs from the one-context depth-1 gateway"
+def check_same(ss, ref, label):
+    for i, (s, r) in enumerate(zip(ss, ref)):
+        assert s.frames == r.frames and s.agent == r.agent, f"{label} stream {i} differs from the one-context depth-1 gateway"
 
 
 @pytest.fixture(scope="module")
@@ -108,28 +42,31 @@ def workload():
 @pytest.fixture(scope="module")
 def reference(workload):
     bodies, modes = workload
-    g = Gateway(device=0, config=config(len(bodies)))
+    ss = sessions(bodies, modes)
+    g = Gateway(device=0, config=gateway_config(len(bodies), 1 << 18))
     try:
-        outs, _ = drive(g, bodies, modes)
+        assert drive(g, ss, seed=0) == 0
     finally:
         g.close()
-    check_oracle(bodies, modes, outs, "one context, depth 1")
-    return outs
+    assert check_sessions(ss, "one context, depth 1")[0] == 0
+    return ss
 
 
 @pytest.mark.parametrize("devices", [[0], [0, 0], [0, 0, 0]], ids=lambda d: f"ctx{len(d)}")
 @pytest.mark.parametrize("depth", [1, 2, N_SLOTS])
 def test_streams_match_the_oracle_and_depth_one(workload, reference, devices, depth):
     bodies, modes = workload
-    g = Gateway(config=config(len(bodies)), devices=devices, depth=depth)
+    ss = sessions(bodies, modes)
+    g = Gateway(config=gateway_config(len(bodies), 1 << 18), devices=devices, depth=depth)
     try:
-        outs, sids = drive(g, bodies, modes)
+        assert drive(g, ss, seed=0) == 0
     finally:
         g.close()
     label = f"devices {devices} depth {depth}"
-    check_oracle(bodies, modes, outs, label)
-    check_same(outs, reference, label)
-    per_ctx = np.bincount(np.asarray(sids) // len(bodies), minlength=len(devices))
+    assert check_sessions(ss, label)[0] == 0
+    check_same(ss, reference, label)
+    # one part per session: each sid is the stream id drive opened before its first tick
+    per_ctx = np.bincount(np.asarray([s.sid for s in ss]) // len(bodies), minlength=len(devices))
     assert per_ctx.max() - per_ctx.min() <= 1
 
 
@@ -139,15 +76,15 @@ def test_counters_add_up_over_contexts(workload, devices, depth):
     the gateway's counters hold every context's batches exactly once."""
     bodies, modes = workload
     keep = [i for i, m in enumerate(modes) if m != R]
-    bodies, modes = [bodies[i] for i in keep], [modes[i] for i in keep]
-    g = Gateway(config=config(len(bodies), flags=A.FLAG_COUNTERS), devices=devices, depth=depth)
+    ss = sessions([bodies[i] for i in keep], [modes[i] for i in keep])
+    g = Gateway(config=gateway_config(len(ss), 1 << 18, flags=A.FLAG_COUNTERS), devices=devices, depth=depth)
     try:
-        outs, _ = drive(g, bodies, modes, seed=3)
+        assert drive(g, ss, seed=3) == 0
         k = g.counters()
     finally:
         g.close()
-    check_oracle(bodies, modes, outs, f"counters devices {devices} depth {depth}")
-    delivered = sum(len(o.frames) for o in outs)
+    assert check_sessions(ss, f"counters devices {devices} depth {depth}")[0] == 0
+    delivered = sum(len(s.frames[0]) for s in ss)
     assert k["p_frames_zero_copy"] + k["p_frames_materialised"] == delivered > 0
 
 
@@ -156,15 +93,16 @@ def test_deferral_keeps_each_stream_in_one_batch_in_flight(workload, devices, de
     """SSE_FLAG_DEFER with produce capacities far below a tick's need: batches defer, and a stream whose rest goes back to its
     queue is never in a second uncollected batch, so every byte arrives once and in order."""
     bodies, modes = workload
-    g = Gateway(config=config(len(bodies), batch=1 << 20, flags=A.FLAG_DEFER | A.FLAG_COUNTERS, **TINY_PRODUCE),
+    ss = sessions(bodies, modes)
+    g = Gateway(config=gateway_config(len(bodies), flags=A.FLAG_DEFER | A.FLAG_COUNTERS, **TINY_PRODUCE),
                 devices=devices, depth=depth)
     try:
-        outs, _ = drive(g, bodies, modes, seed=1)
+        assert drive(g, ss, seed=1) == 0
         k = g.counters()
     finally:
         g.close()
     assert k["p_deferred_rounds"] > 0
-    check_oracle(bodies, modes, outs, f"defer devices {devices} depth {depth}")
+    assert check_sessions(ss, f"defer devices {devices} depth {depth}")[0] == 0
 
 
 def long_body(rng, n_lines, size):
@@ -184,19 +122,20 @@ def test_line_pool_lines_complete_while_batches_are_in_flight(workload, devices,
     rng = np.random.default_rng(7)
     longs = [long_body(rng, 3, 100_000 + 20_000 * i) for i in range(8)]
     b2, m2 = list(bodies[:120]) + longs, list(modes[:120]) + [(R, PP)[i % 2] for i in range(len(longs))]
-    kw = dict(config=config(len(b2)), line_pool=dict(pool_pages=48))
+    kw = dict(config=gateway_config(len(b2), 1 << 18), line_pool=dict(pool_pages=48))
+    ss, ref = sessions(b2, m2), sessions(b2, m2)
     g = Gateway(devices=devices, depth=depth, **kw)
     try:
-        outs, _ = drive(g, b2, m2, n_pieces=12, seed=2)
+        assert drive(g, ss, seed=2, n_pieces=12) == 0
     finally:
         g.close()
-    check_oracle(b2, m2, outs, f"pool devices {devices} depth {depth}")
+    assert check_sessions(ss, f"pool devices {devices} depth {depth}")[0] == 0
     g = Gateway(**kw)
     try:
-        ref, _ = drive(g, b2, m2, n_pieces=12, seed=2)
+        assert drive(g, ref, seed=2, n_pieces=12) == 0
     finally:
         g.close()
-    check_same(outs, ref, f"pool devices {devices} depth {depth}")
+    check_same(ss, ref, f"pool devices {devices} depth {depth}")
 
 
 @pytest.mark.parametrize("mode", [P, R])
@@ -204,7 +143,7 @@ def test_reopened_connection_gets_nothing_of_the_old_stream(mode):
     """A stream released while batches still hold its bytes, and its connection reopened at once: the reset is ordered after
     those batches and what they return for the connection goes to nobody, so the new stream sees exactly its own body."""
     n = 64
-    g = Gateway(config=config(n), devices=[0], depth=N_SLOTS)
+    g = Gateway(config=gateway_config(n, 1 << 18), devices=[0], depth=N_SLOTS)
     try:
         sids = [g.stream_chat_completions(mode) for _ in range(n)]
         assert sids == list(range(n))
@@ -222,24 +161,29 @@ def test_reopened_connection_gets_nothing_of_the_old_stream(mode):
         for s in new:
             assert g.upstream_write(s, body) == len(body)
             g.upstream_close(s)
-        outs = {s: Out(mode) for s in new}
+        ss = {s: Session([body], mode, tap=False) for s in new}
+        eof = set()
         for _ in range(100):
             g.pump()
             for s in new:
-                drain(g, s, outs[s])
-            if all(o.eof for o in outs.values()):
+                try:
+                    while (f := g.recv(s)) is not None:
+                        ss[s].frames[0].append(f)
+                except EOFError:
+                    eof.add(s)
+            if len(eof) == len(new):
                 break
         assert g.flush() == 0
         for s in new:
             if mode == R:
-                outs[s].agent = g.agent_state(s)
-        check_oracle([body] * len(new), [mode] * len(new), [outs[s] for s in new], "reopened")
+                ss[s].agent[0] = g.agent_state(s)
+        assert check_sessions([ss[s] for s in new], "reopened")[0] == 0
     finally:
         g.close()
 
 
 def test_placement_balances_open_streams():
-    g = Gateway(config=config(16), devices=[0, 0, 0], depth=2)
+    g = Gateway(config=gateway_config(16, 1 << 18), devices=[0, 0, 0], depth=2)
     try:
         ctx = lambda s: s // 16
         first = [g.stream_chat_completions(P) for _ in range(3)]

@@ -5,159 +5,20 @@ verdict: every stream's frames are the oracle's; the fold finishes with (0, *orc
 was sent (the MCP agent's final [DONE], fed by the caller, included), or with 1 when body has an irregular piece (DESIGN.md
 §5, deviation 4); a stream whose records include a line past the nesting limit ends after a prefix of the oracle's frames
 that reaches that line, and its fold is not compared. Untapped streams keep their old behaviour next to tapped ones."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 from inference_gateway_b200 import _abi as A, synth
 from inference_gateway_b200.gateway import Gateway, Telemetry
-from inference_gateway_b200.synth import random_cuts
-from oracle import orc
 from tests import folds
-from tests.util import DONE, ENGINES, TINY_DECODE, TINY_PRODUCE, check_agent, irregular_telemetry
+from tests.gateway_drive import (Session, assert_folds_saw_something, check_sessions, check_telemetry, drive, expected,
+                                 gateway_config)
+from tests.util import DONE, ENGINES, TINY_DECODE, TINY_PRODUCE
 
 pytestmark = pytest.mark.gpu
 
 P, R, PP = A.MODE_P, A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
 N_SLOTS = 4
-MiB = 1 << 20
-
-
-def worst_case(conns, flags=0):
-    cfg = A.Config()
-    A.load().sse_worst_case_config(C.byref(cfg), conns, MiB)
-    cfg.n_slots, cfg.flags = N_SLOTS, flags
-    return cfg
-
-
-def default(conns, batch=MiB, flags=0, **caps):
-    cfg = A.Config()
-    A.load().sse_default_config(C.byref(cfg), conns, batch)
-    cfg.n_slots, cfg.flags = N_SLOTS, flags
-    for k, v in caps.items():
-        setattr(cfg, k, v)
-    return cfg
-
-
-class Session:
-    """One client response: the upstream bodies of `parts`, each opened once the one before was delivered to the end and
-    released, in `mode`, read through the channel ("chan") or the raw proxy loop ("proxy"); its own fold unless tap is
-    False."""
-
-    def __init__(self, parts, mode, route="chan", tap=True):
-        self.parts, self.mode, self.route = list(parts), mode, route
-        self.tel = Telemetry() if tap else None
-        self.frames = [[] for _ in self.parts]
-        self.agent = [None] * len(self.parts)
-        self.k, self.sid, self.done = -1, None, False
-        self.queue, self.left, self.upstream_closed = [], b"", False
-
-
-def open_next(g, s, rng, n_pieces):
-    s.k += 1
-    s.sid = g.proxy_stream(telemetry=s.tel) if s.route == "proxy" else g.stream_chat_completions(s.mode, telemetry=s.tel)
-    s.queue = random_cuts(rng, s.parts[s.k], int(rng.integers(1, n_pieces + 1)))
-    s.left, s.upstream_closed = b"", False
-
-
-def drive(g, sessions, seed, n_pieces=6, max_ticks=5000):
-    """Writes every session's streams in seeded pieces, one piece per stream and tick, closes each upstream after the pump that
-    took its last piece, and reads every channel after every pump. A stream whose channel ends is released (mode R: after
-    its agent state was read) and the session's next stream is opened at once, while the other sessions' batches may still
-    be in flight."""
-    rng = np.random.default_rng(seed)
-    for s in sessions:
-        open_next(g, s, rng, n_pieces)
-    for _ in range(max_ticks):
-        live = [s for s in sessions if not s.done]
-        if not live:
-            break
-        for s in live:
-            if not s.left and s.queue:
-                s.left = s.queue.pop(0)
-            if s.left:
-                s.left = s.left[g.upstream_write(s.sid, s.left):]
-        g.pump()
-        for s in live:
-            if not s.upstream_closed and not s.left and not s.queue:
-                g.upstream_close(s.sid)
-                s.upstream_closed = True
-            fn = g.proxy_step if s.route == "proxy" else g.recv
-            try:
-                while (f := fn(s.sid)) is not None:
-                    s.frames[s.k].append(f)
-            except EOFError:
-                if s.mode & A.MODE_R:
-                    s.agent[s.k] = g.agent_state(s.sid)
-                g.release(s.sid)
-                if s.k + 1 < len(s.parts):
-                    open_next(g, s, rng, n_pieces)
-                else:
-                    s.done = True
-    else:
-        raise AssertionError("sessions still open after max_ticks")
-    assert g.flush() >= 0
-
-
-def expected(body, mode):
-    """The oracle's view of one upstream body, its frames, and how many of them reach its first line past the nesting limit
-    (None: no such line)."""
-    if mode & A.MODE_R:
-        v = orc.reframe(body)
-        lines = [(l, l.kind == orc.L_EMITTED) for l in v.lines]
-    else:
-        v = orc.passthrough(body, parse=bool(mode & A.MODE_PARSE))
-        lines = [(l, True) for l in v.lines]
-    want, upto = [], None
-    for l, emitted in lines:
-        if emitted:
-            want.append(l.out)
-        if upto is None and l.kind != orc.L_UNREAD and l.depth_limited:
-            upto = len(want)
-    return v, want, upto
-
-
-def check_telemetry(tel, body, label):
-    rc, usage, calls = tel.finish()
-    if irregular_telemetry(body):
-        assert rc == 1, f"{label}: telemetry finished with {rc} on a body with an irregular piece"
-    else:
-        assert (rc, usage, calls) == (0, *orc.telemetry(body)), f"{label}: telemetry differs from the oracle's"
-    return usage, calls
-
-
-def check_sessions(sessions, label):
-    """The verdict on every session. Returns (sessions ended by a line past the nesting limit, fold results compared)."""
-    n_limited, compared = 0, []
-    for i, s in enumerate(sessions):
-        lab = f"{label} session {i} mode {s.mode} {s.route}{'' if s.tel else ' untapped'}"
-        limited = False
-        for k, (body, got) in enumerate(zip(s.parts, s.frames)):
-            v, want, upto = expected(body, s.mode)
-            # a fold that meets such a line closes the stream: the tap, or the agent fold of a mode R stream
-            if upto is not None and (s.tel is not None or s.mode & A.MODE_R):
-                limited = True
-                assert upto <= len(got) <= len(want) and got == want[:len(got)], \
-                    f"{lab} part {k}: {len(got)} frames are not a prefix of the oracle's {len(want)} through frame {upto}"
-                continue
-            assert got == want, f"{lab} part {k}: {len(got)} frames, oracle {len(want)}"
-            if s.mode & A.MODE_R:
-                check_agent(s.agent[k], v, f"{lab} part {k}")
-        n_limited += limited
-        if s.tel is not None:
-            if not limited:
-                body = b"".join(f for part in s.frames for f in part)
-                if s.mode & A.MODE_R:
-                    s.tel.feed_bytes(DONE)          # the agent's single final [DONE] (agent.go:140-143)
-                    body += DONE
-                compared.append(check_telemetry(s.tel, body, lab))
-            s.tel.close()
-    return n_limited, compared
-
-
-def assert_folds_saw_something(compared):
-    assert any(u != (0, 0, 0) for u, _ in compared) and any(c for _, c in compared)
 
 
 # ------------------------------------------------------------------ workloads
@@ -224,12 +85,11 @@ def plain_bodies():
 @pytest.mark.parametrize("eng", ["split", "fused"])
 def test_tap_on_handler_and_proxy_streams(plain_bodies, eng, devices, depth):
     sessions = plain_sessions(plain_bodies)
-    cfg = worst_case(len(sessions), ENGINES[eng])
-    if eng == "fused":
-        cfg.carry_slot_bytes = 32768        # the tile kernel's lines are at most 49,120 bytes; a smaller slot loosens no bound
-    g = Gateway(config=cfg, devices=devices, depth=depth)
+    # the tile kernel's lines are at most 49,120 bytes; a smaller slot loosens no bound
+    slot = dict(carry_slot_bytes=32768) if eng == "fused" else {}
+    g = Gateway(config=gateway_config(len(sessions), worst_case=True, flags=ENGINES[eng], **slot), devices=devices, depth=depth)
     try:
-        drive(g, sessions, seed=depth + 10 * len(devices))
+        assert drive(g, sessions, seed=depth + 10 * len(devices)) >= 0
     finally:
         g.close()
     n_limited, compared = check_sessions(sessions, f"{eng} devices {devices} depth {depth}")
@@ -244,9 +104,9 @@ def test_mcp_sessions_share_one_fold(devices, depth):
     streams (tapped and untapped). Tool-call indices repeat over the iterations, so telemetry merges across them."""
     c3 = synth_bodies("C3", 40)
     sessions = mcp_sessions(36, seed=depth) + plain_sessions(c3)
-    g = Gateway(config=worst_case(len(sessions)), devices=devices, depth=depth)
+    g = Gateway(config=gateway_config(len(sessions), worst_case=True), devices=devices, depth=depth)
     try:
-        drive(g, sessions, seed=depth)
+        assert drive(g, sessions, seed=depth) >= 0
     finally:
         g.close()
     n_limited, compared = check_sessions(sessions, f"mcp devices {devices} depth {depth}")
@@ -266,10 +126,10 @@ def test_tap_when_batches_defer(eng, devices, depth):
     c = folds.corpus(seed=1, n_adv=24)
     bodies = c["adversarial"] + c["tricky"][::3] + c["merge"] + c["near_misses"][::8] + long_pieces() + synth_bodies("C4", 32)
     sessions = plain_sessions(bodies) + mcp_sessions(12, seed=7)
-    cfg = default(len(sessions), flags=A.FLAG_DEFER | A.FLAG_COUNTERS | ENGINES[eng], **TINY_PRODUCE, **TINY_DECODE)
+    cfg = gateway_config(len(sessions), flags=A.FLAG_DEFER | A.FLAG_COUNTERS | ENGINES[eng], **TINY_PRODUCE, **TINY_DECODE)
     g = Gateway(config=cfg, devices=devices, depth=depth)
     try:
-        drive(g, sessions, seed=3)
+        assert drive(g, sessions, seed=3) >= 0
         k = g.counters()
     finally:
         g.close()
@@ -296,10 +156,10 @@ def test_tap_on_line_pool_lines(devices, depth):
     big = folds.saturated_streams() + longs
     sessions = ([Session([b], PP) for b in big] + [Session([b], R) for b in big]
                 + plain_sessions(synth_bodies("C4", 48)))
-    g = Gateway(config=worst_case(len(sessions)), devices=devices, depth=depth,
+    g = Gateway(config=gateway_config(len(sessions), worst_case=True), devices=devices, depth=depth,
                 line_pool=dict(pool_pages=192, page_bytes=65536, max_line_bytes=512 * 1024))
     try:
-        drive(g, sessions, seed=depth, n_pieces=12)
+        assert drive(g, sessions, seed=depth, n_pieces=12) >= 0
     finally:
         g.close()
     n_limited, compared = check_sessions(sessions, f"pool devices {devices} depth {depth}")
@@ -325,7 +185,7 @@ def test_released_tap_gets_nothing_of_batches_in_flight():
     an old fold holds the telemetry of exactly the frames its stream received, a new fold sees only its own stream, and the
     streams left open, tapped or not, are the oracle's to the end."""
     n = 64
-    g = Gateway(config=default(n), devices=[0], depth=N_SLOTS)
+    g = Gateway(config=gateway_config(n), devices=[0], depth=N_SLOTS)
     try:
         taps = [Telemetry() if i % 4 != 3 else None for i in range(n)]
         sids = [g.stream_chat_completions(PP, telemetry=t) for t in taps]
@@ -394,7 +254,7 @@ def test_released_tap_gets_nothing_of_batches_in_flight():
 # ------------------------------------------------------------------ 6: refusals
 def test_attach_refusals_and_reattach():
     L = A.load()
-    g = Gateway(config=default(4), devices=[0], depth=2)
+    g = Gateway(config=gateway_config(4), devices=[0], depth=2)
     tel, other = Telemetry(), Telemetry()
     try:
         attach = lambda mode, t: L.ssegw_stream_with_telemetry(g.g, mode, t.f if t is not None else None)

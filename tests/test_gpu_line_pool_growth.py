@@ -1,19 +1,16 @@
 """GPU: a line pool that grows on demand (sse_line_pool_set_growth, SSE_FLAG_DEFER). A line that finds no free page defers its
 segment at the byte that needed the page, sse_collect grows the pool, and the stream goes on bit-exact against the CPU oracle;
 at the limit lines fail as without growth. Every batch passes orc_check_result."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 from inference_gateway_b200 import SseEngine, _abi as A
-from inference_gateway_b200.gateway import Gateway, Telemetry
-from inference_gateway_b200.synth import random_cuts
-from oracle import orc
+from inference_gateway_b200.gateway import Gateway
 from tests import folds
-from tests.streams import PAGE, SLOT, chunk, long_line, stream_with
-from tests.util import (ENGINES, TINY_DECODE, ConnOut, check_agent, check_folds, check_result, check_stream, check_streams,
-                        feed_folds, fold_segment, irregular_telemetry, process_all_checked, run_deferred)
+from tests.gateway_drive import Session, check_sessions, drive, gateway_config
+from tests.streams import PAGE, SLOT, burst, chunk, long_line, stream_with
+from tests.util import (DONE, ENGINES, TINY_DECODE, ConnOut, check_folds, check_stream, check_streams, feed_folds, fold_segment,
+                        pool_engine, process_all_checked, run_deferred, run_inflight, run_pieces_deferred)
 
 pytestmark = pytest.mark.gpu
 
@@ -21,35 +18,6 @@ P, R, PP = A.MODE_P, A.MODE_R | A.MODE_PARSE, A.MODE_P | A.MODE_PARSE
 MODES = (P, R, PP)
 MiB = 1 << 20
 SMALL_PAGE = 4096 + 16
-DONE = b"data: [DONE]\n\n"
-
-
-def engine(pages, max_pages, flags=0, page_bytes=PAGE, conns=64, batch=8 * MiB, n_slots=4, **caps):
-    return SseEngine(device=0, max_conns=conns, bytes_per_batch=batch, carry_slot_bytes=SLOT, n_slots=n_slots,
-                     flags=A.FLAG_DEFER | flags, **caps,
-                     line_pool=dict(pool_pages=pages, page_bytes=page_bytes, max_line_bytes=2 * MiB, max_pages=max_pages))
-
-
-def burst(n, rng, size=200_000, kinds=("toolcall", "content", "terminal")):
-    return [stream_with(long_line(kinds[i % len(kinds)], size + 1009 * i, rng), kinds[i % len(kinds)]) for i in range(n)]
-
-
-def run_pieces_deferred(eng, pieces, modes):
-    """pieces[c][b] goes to connection c in batch b; every batch is run to the end (SseEngine.process_all, checked), its
-    deferred rests first in the next batch. Returns (outs, deferrals: (connection, consumed, batch overflow), overflow bits)."""
-    outs = [ConnOut() for _ in pieces]
-    eng.reset_all()
-    deferrals, ovf = [], [0]
-
-    def on_batch(res, conns):
-        ovf[0] |= res.overflow
-        for i, c in enumerate(conns):
-            fold_segment(outs[c], res, i)
-            if int(res.segs[i]["flags"]) & A.SEG_DEFERRED:
-                deferrals.append((c, res.consumed(i), res.overflow))
-    for b in range(max(map(len, pieces))):
-        process_all_checked(eng, [(c, modes[c], pieces[c][b]) for c in range(len(pieces)) if b < len(pieces[c])], on_batch)
-    return outs, deferrals, ovf[0]
 
 
 # ------------------------------------------------------------------ 1: a burst far beyond the initial pool
@@ -57,7 +25,7 @@ def run_pieces_deferred(eng, pieces, modes):
 @pytest.mark.parametrize("mode", MODES, ids=["P", "R", "PP"])
 def test_burst_grows_the_pool(mode, n_batches):
     """40 connections complete 200 KB lines (4 pages each) in the same batches; the pool starts at 8 pages, the limit is 1024."""
-    e = engine(8, 1024, batch=16 * MiB)
+    e = pool_engine(8, 1024, conns=64, batch=16 * MiB)
     try:
         rng = np.random.default_rng(n_batches * 7 + mode)
         bodies = burst(40, rng)
@@ -93,7 +61,7 @@ PLACES = {
 def test_deferral_lands_where_the_page_was_needed(place, mode):
     page, initial, held, length, at = PLACES[place]
     assert at % 8192 == (0 if place in ("slot", "window_end", "newline") else 160)
-    e = engine(initial, 256, page_bytes=page)
+    e = pool_engine(initial, 256, conns=64, batch=8 * MiB, page_bytes=page)
     try:
         rng = np.random.default_rng(len(place))
         other = stream_with(long_line("toolcall", 300_000, rng), "toolcall")
@@ -102,7 +70,8 @@ def test_deferral_lands_where_the_page_was_needed(place, mode):
         assert len(line) == length and (place != "newline" or line[PAGE:] == b"\n")
         body = line + b"\n" + chunk(b"bye", '"stop"') + DONE
         pieces = [[other[:start + held], b"", other[start + held:]], [b"", body]]
-        outs, deferrals, ovf = run_pieces_deferred(e, pieces, [mode, mode])
+        e.reset_all()
+        outs, _, deferrals, _ = run_pieces_deferred(e, pieces, [mode, mode])
         for b, o in ((other, outs[0]), (body, outs[1])):
             check_stream(b, mode, o, f"{place} mode {mode}")
         assert not any(o.flags & (A.SEG_DEAD | A.SEG_LINE_TOO_LONG) for o in outs)
@@ -117,7 +86,7 @@ def test_deferral_lands_where_the_page_was_needed(place, mode):
 def test_limit_stops_growth_and_fails_only_the_unlucky():
     """Twelve 200 KB lines (4 pages each) at once on a pool of 4 pages that may grow to 8: capacity stops at 8, the connections
     that then found no page fail, the others match the oracle."""
-    e = engine(4, 8)
+    e = pool_engine(4, 8, conns=64, batch=8 * MiB)
     try:
         rng = np.random.default_rng(3)
         bodies = burst(12, rng, kinds=("toolcall",))
@@ -145,7 +114,7 @@ def test_limit_stops_growth_and_fails_only_the_unlucky():
 def test_without_growth_the_pool_fails_as_before(limit):
     """The same shape with growth never enabled, or disabled again: no SSE_OVF_POOL, no pool deferral, the capacity stays,
     and each connection completes bit-exact or fails LINE_TOO_LONG | DEAD."""
-    e = engine(8, 0 if limit is None else 64)
+    e = pool_engine(8, 0 if limit is None else 64, conns=64, batch=8 * MiB)
     try:
         if limit is not None:
             e.line_pool_growth(0)
@@ -179,7 +148,7 @@ def test_setter_refusals():
             e.line_pool_growth(64)
     finally:
         e.close()
-    e = engine(8, 0, conns=16, batch=4 * MiB)
+    e = pool_engine(8, 0, conns=16, batch=4 * MiB)
     try:
         for bad in (7, 0xFFFFFFFF):                         # below the capacity, SSE_NONE
             with pytest.raises(A.SseError):
@@ -191,74 +160,11 @@ def test_setter_refusals():
 
 
 # ------------------------------------------------------------------ 4: batches in flight
-def run_inflight(eng, bodies, modes, depth, n_pieces, seed, between=None, abandon=None):
-    """Up to depth uncollected batches. Connection c belongs to group c % depth and a batch takes the ready connections of one
-    group (the next group, in turn, that has any), so that depth batches of disjoint connections are uncollected together. A
-    connection goes into a batch only while it is in no uncollected one, and a deferred rest goes back to the front of its
-    queue when its batch is collected. between(k) runs after submit k; abandon(k) may return (conn, mode, bytes) items for a
-    batch that is submitted after submit k and released without being collected.
-    Returns (outs, per-batch overflow bits, events): events["grew_in_flight"] counts collects that grew the pool while other
-    batches were uncollected (launched with the old pool's arrays), events["stale_pool"] batches that reported SSE_OVF_POOL after
-    the pool had grown since their submit, whose collect did not grow it again."""
-    rng = np.random.default_rng(seed)
-    queue = [random_cuts(rng, b, n_pieces) for b in bodies]
-    outs = [ConnOut() for _ in bodies]
-    busy, inflight, k, g_next, ovf = set(), [], 0, 0, []
-    events = dict(grew_in_flight=0, stale_pool=0, max_in_flight=0)
-    eng.reset_all()
-    while any(queue) or inflight:
-        group = None
-        if len(inflight) < depth:
-            for j in range(depth):
-                g = (g_next + j) % depth
-                if any(queue[c] and c not in busy for c in range(g, len(bodies), depth)):
-                    group = g
-                    break
-        if group is not None:
-            g_next = group + 1
-            items = [(c, modes[c], queue[c].pop(0)) for c in range(group, len(bodies), depth) if queue[c] and c not in busy]
-            slot, arena, segs = eng.acquire()
-            n, nbytes = eng.fill(arena, segs, items)
-            eng.submit(slot, n, nbytes)
-            inflight.append((slot, items, segs[:n].copy(), eng.line_pool_capacity()[0]))
-            events["max_in_flight"] = max(events["max_in_flight"], len(inflight))
-            busy.update(c for c, _, _ in items)
-            if between is not None:
-                between(k)
-            extra = abandon(k) if abandon is not None else None
-            if extra:
-                s2, a2, g2 = eng.acquire()
-                eng.submit(s2, *eng.fill(a2, g2, extra))
-                eng.release(s2)
-            k += 1
-            continue
-        slot, items, segs, pages_at_submit = inflight.pop(0)
-        try:
-            before = eng.line_pool_capacity()[0]
-            res = eng.collect(slot)
-            after = eng.line_pool_capacity()[0]
-            check_result(eng, res, segs)
-            ovf.append(res.overflow)
-            if after > before and inflight:
-                events["grew_in_flight"] += 1
-            if res.overflow & A.OVF_POOL and pages_at_submit != before:
-                assert after == before, "a batch launched before a growth grew the pool again"
-                events["stale_pool"] += 1
-            for i, (c, m, data) in enumerate(items):
-                fold_segment(outs[c], res, i)
-                busy.discard(c)
-                if int(res.segs[i]["flags"]) & A.SEG_DEFERRED:
-                    queue[c].insert(0, data[res.consumed(i):])
-        finally:
-            eng.release(slot)
-    return outs, ovf, events
-
-
 @pytest.mark.parametrize("depth", [2, 4])
 def test_growth_with_batches_in_flight(depth):
     """depth batches of disjoint connections uncollected together: a collect grows the pool while later batches, launched with
     the old arrays, are still queued; those batches' own SSE_OVF_POOL does not grow it again; every stream matches the oracle."""
-    e = engine(8, 2048)
+    e = pool_engine(8, 2048, conns=64, batch=8 * MiB)
     try:
         rng = np.random.default_rng(depth)
         bodies = burst(36, rng)
@@ -277,7 +183,7 @@ def test_resets_stats_and_an_abandoned_batch_between_submits():
     """sse_reset_conn and sse_line_pool_stats after every submit, and batches of other connections (long lines that take and
     lack pages) released without being collected: the pool grows only at collect, the abandoned connections' pages come back
     with their resets, and the collected streams match the oracle."""
-    e = engine(8, 2048, conns=128)
+    e = pool_engine(8, 2048, conns=128, batch=8 * MiB)
     try:
         rng = np.random.default_rng(8)
         bodies = burst(24, rng)
@@ -303,7 +209,7 @@ def test_resets_stats_and_an_abandoned_batch_between_submits():
 def test_pool_and_decode_arenas_grow_in_the_same_batch():
     """Tiny tool-call, usage and text arenas: one batch whose long lines lack pages (SSE_OVF_POOL) also grows the tool-call
     and text arenas and is decoded again; streams and folds match the oracle."""
-    e = engine(8, 1024, **TINY_DECODE)
+    e = pool_engine(8, 1024, conns=64, batch=8 * MiB, **TINY_DECODE)
     try:
         rng = np.random.default_rng(12)
         tc = b"".join(b'data: {"choices":[{"index":0,"delta":{"tool_calls":[{"index":%d,"id":"c%d","function":{"name":"f",'
@@ -338,7 +244,7 @@ def test_pool_and_decode_arenas_grow_in_the_same_batch():
 def test_engines_and_folds_on_grown_pages(name):
     """The split engines, each on a pool of 4 pages that grows: saturated tool-call chains (65,534-65,537 elements) and long
     tool-call arguments complete in grown pages; frames and records match the oracle, and the agent and telemetry folds too."""
-    e = engine(4, 1024, flags=ENGINES[name], text_arena_bytes=32 * MiB)
+    e = pool_engine(4, 1024, flags=A.FLAG_DEFER | ENGINES[name], conns=64, batch=8 * MiB, text_arena_bytes=32 * MiB)
     try:
         rng = np.random.default_rng(21)
         big = folds.saturated_streams() + [stream_with(long_line("toolcall", 400_000 + 5000 * i, rng), "toolcall") for i in range(6)]
@@ -359,72 +265,18 @@ def test_engines_and_folds_on_grown_pages(name):
 
 
 # ------------------------------------------------------------------ 6: the gateway
-def gw_config(conns, batch=1 << 20):
-    cfg = A.Config()
-    A.load().sse_default_config(C.byref(cfg), conns, batch)
-    cfg.n_slots = 4
-    cfg.flags = A.FLAG_DEFER
-    return cfg
-
-
 @pytest.mark.parametrize("tap", [False, True], ids=["plain", "tapped"])
 @pytest.mark.parametrize("devices,depth", [([0], 1), ([0], 4), ([0, 0], 1), ([0, 0], 4)])
 def test_gateway_grows_its_pools(devices, depth, tap):
-    rng = np.random.default_rng(depth * 10 + len(devices))
+    seed = depth * 10 + len(devices)
+    rng = np.random.default_rng(seed)
     bodies = burst(24, rng, size=150_000) + [chunk(b"short %d" % i) + chunk(b"end", '"stop"') + DONE for i in range(8)]
-    modes = [(R, PP)[i % 2] for i in range(len(bodies))]
-    g = Gateway(config=gw_config(len(bodies)), devices=devices, depth=depth,
+    sessions = [Session([b], (R, PP)[i % 2], tap=tap) for i, b in enumerate(bodies)]
+    g = Gateway(config=gateway_config(len(sessions), flags=A.FLAG_DEFER), devices=devices, depth=depth,
                 line_pool=dict(pool_pages=4, max_line_bytes=MiB, max_pages=4096))
-    taps = [Telemetry() if tap else None for _ in bodies]
     try:
-        sids = [g.stream_chat_completions(m, telemetry=t) if t is not None else g.stream_chat_completions(m)
-                for m, t in zip(modes, taps)]
-        queue = [random_cuts(rng, b, 6) for b in bodies]
-        left = [b""] * len(bodies)
-        frames = [[] for _ in bodies]
-        eof = [False] * len(bodies)
-        closed = [False] * len(bodies)
-        for _ in range(20000):
-            for i, sid in enumerate(sids):
-                if not left[i] and queue[i]:
-                    left[i] = queue[i].pop(0)
-                if left[i]:
-                    left[i] = left[i][g.upstream_write(sid, left[i]):]
-            g.pump()
-            for i, sid in enumerate(sids):
-                if not closed[i] and not left[i] and not queue[i]:
-                    g.upstream_close(sid)
-                    closed[i] = True
-                try:
-                    while not eof[i] and (f := g.recv(sid)) is not None:
-                        frames[i].append(f)
-                except EOFError:
-                    eof[i] = True
-            if all(eof):
-                break
-        else:
-            raise AssertionError("streams still open")
-        assert g.flush() >= 0
-        for i, (b, m, sid) in enumerate(zip(bodies, modes, sids)):
-            if m == R:
-                v = orc.reframe(b)
-                want = [l.out for l in v.lines if l.kind == orc.L_EMITTED]
-                check_agent(g.agent_state(sid), v, f"gateway stream {i}")
-            else:
-                want = [l.out for l in orc.passthrough(b, parse=True).lines]
-            assert frames[i] == want, f"gateway {devices} depth {depth} stream {i}: {len(frames[i])} frames, oracle {len(want)}"
-            if taps[i] is not None:
-                body = b"".join(frames[i]) + (DONE if m == R else b"")
-                if m == R:
-                    taps[i].feed_bytes(DONE)
-                rc, usage, calls = taps[i].finish()
-                if irregular_telemetry(body):
-                    assert rc == 1
-                else:
-                    assert (rc, usage, calls) == (0, *orc.telemetry(body)), f"gateway stream {i}: telemetry differs"
-            g.release(sid)
+        assert drive(g, sessions, seed, max_ticks=20000) >= 0
     finally:
         g.close()
-        for t in taps:
-            if t is not None:
-                t.close()
+    n_limited, _ = check_sessions(sessions, f"gateway {devices} depth {depth}")
+    assert n_limited == 0

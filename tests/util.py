@@ -11,6 +11,7 @@ import numpy as np
 
 from inference_gateway_b200 import _abi as A
 from oracle import orc
+from tests.streams import PAGE, SLOT
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = open(os.path.join(ROOT, "include", "sse_gpu.h")).read()
@@ -212,9 +213,34 @@ def run_streams(engine, streams, modes, n_batches=1, seed=0, with_folds=False, k
     return outs
 
 
+def run_pieces_deferred(eng, pieces, modes, conns=None, outs=None, keep_codes=False):
+    """pieces[j][b] goes to connection conns[j] (default: j) in batch b, in mode modes[conns[j]]. Every batch is run to the
+    end with SseEngine.process_all (each submit checked), which submits deferred rests again until every byte was taken.
+    Segments are appended to outs[conns[j]] (new ConnOuts by default), and fed to its folds where it has them (feed_folds, with
+    the batch index as the piece). Returns (outs, batches submitted, deferrals: (connection, consumed, the batch's overflow
+    bits) per deferred segment, the OR of every batch's overflow bits)."""
+    conns = range(len(pieces)) if conns is None else conns
+    outs = [ConnOut() for _ in range(max(conns) + 1)] if outs is None else outs
+    batches, deferrals, ovf = 0, [], 0
+
+    def on_batch(res, cs):
+        nonlocal ovf
+        ovf |= res.overflow
+        for i, c in enumerate(cs):
+            o = outs[c]
+            fold_segment(o, res, i)
+            if int(res.segs[i]["flags"]) & A.SEG_DEFERRED:
+                deferrals.append((c, res.consumed(i), res.overflow))
+            if o.agent is not None:
+                feed_folds(eng.L, o, res, i, b, keep_codes)
+
+    for b in range(max(map(len, pieces))):
+        batches += process_all_checked(eng, [(c, modes[c], p[b]) for c, p in zip(conns, pieces) if b < len(p)], on_batch)
+    return outs, batches, deferrals, ovf
+
+
 def run_deferred(eng, bodies, modes, n_batches=1, seed=0, with_folds=False, n_folds=None, keep_codes=False):
-    """run_streams on an engine with SSE_FLAG_DEFER: every micro-batch of pieces is run to the end with SseEngine.process_all,
-    which submits deferred remainders again until every byte was taken. The agent and telemetry folds are fed for the first
+    """run_streams on an engine with SSE_FLAG_DEFER (run_pieces_deferred). The agent and telemetry folds are fed for the first
     n_folds streams (all by default). Returns (outs, stats)."""
     from inference_gateway_b200.synth import random_cuts
     rng = np.random.default_rng(seed)
@@ -227,23 +253,91 @@ def run_deferred(eng, bodies, modes, n_batches=1, seed=0, with_folds=False, n_fo
     if with_folds:
         for o in outs[:n_folds]:
             o.agent, o.tele = L.sse_agent_new(), L.sse_telemetry_new()
-    stats = dict(batches=0, deferred=0, overflow=0)
-    piece = [0]
+    _, batches, deferrals, ovf = run_pieces_deferred(eng, pieces, modes, outs=outs, keep_codes=keep_codes)
+    return outs, dict(batches=batches, deferred=len(deferrals), overflow=ovf)
 
-    def on_batch(res, conns):
-        stats["overflow"] |= res.overflow
-        for i, c in enumerate(conns):
-            o = outs[c]
-            fold_segment(o, res, i)
-            stats["deferred"] += bool(int(res.segs[i]["flags"]) & A.SEG_DEFERRED)
-            if o.agent is not None:
-                feed_folds(L, o, res, i, piece[0], keep_codes)
 
-    for b in range(max(len(p) for p in pieces)):
-        piece[0] = b
-        items = [(c, modes[c], pieces[c][b]) for c in range(len(bodies)) if b < len(pieces[c])]
-        stats["batches"] += process_all_checked(eng, items, on_batch)
-    return outs, stats
+def run_inflight(eng, bodies, modes, depth, n_pieces, seed, between=None, abandon=None):
+    """Up to depth uncollected batches of disjoint connections: connection c belongs to group c % depth, and a batch takes the
+    ready connections of the next group, in turn, that has any. A connection goes into a batch only while it is in no
+    uncollected one, and a deferred rest goes back to the front of its queue when its batch is collected. between(k) runs
+    after submit k; abandon(k) may return (conn, mode, bytes) items for a batch that is submitted after submit k and released
+    without being collected. The pool's generation counts every change of its capacity (growth or trim).
+    Returns (outs, per-batch overflow bits, events): max_in_flight; grew_in_flight, the collects that grew the pool while other
+    batches were uncollected (launched with the old pool's arrays); stale_pool, the batches that reported SSE_OVF_POOL after
+    the pool changed since their submit, whose collect must not grow it; trims_shrunk, the calls of between that shrank it."""
+    from inference_gateway_b200.synth import random_cuts
+    rng = np.random.default_rng(seed)
+    queue = [random_cuts(rng, b, n_pieces) for b in bodies]
+    outs = [ConnOut() for _ in bodies]
+    busy, inflight, k, g_next, ovf = set(), [], 0, 0, []
+    gen = [0, eng.line_pool_capacity()[0]]
+    events = dict(max_in_flight=0, grew_in_flight=0, stale_pool=0, trims_shrunk=0)
+
+    def track():
+        cap = eng.line_pool_capacity()[0]
+        if cap != gen[1]:
+            gen[0] += 1
+            gen[1] = cap
+    eng.reset_all()
+    while any(queue) or inflight:
+        group = None
+        if len(inflight) < depth:
+            for j in range(depth):
+                g = (g_next + j) % depth
+                if any(queue[c] and c not in busy for c in range(g, len(bodies), depth)):
+                    group = g
+                    break
+        if group is not None:
+            g_next = group + 1
+            items = [(c, modes[c], queue[c].pop(0)) for c in range(group, len(bodies), depth) if queue[c] and c not in busy]
+            slot, arena, segs = eng.acquire()
+            n, nbytes = eng.fill(arena, segs, items)
+            eng.submit(slot, n, nbytes)
+            inflight.append((slot, items, segs[:n].copy(), gen[0]))
+            events["max_in_flight"] = max(events["max_in_flight"], len(inflight))
+            busy.update(c for c, _, _ in items)
+            if between is not None:
+                before = gen[1]
+                between(k)
+                track()
+                events["trims_shrunk"] += gen[1] < before
+            extra = abandon(k) if abandon is not None else None
+            if extra:
+                s2, a2, g2 = eng.acquire()
+                eng.submit(s2, *eng.fill(a2, g2, extra))
+                eng.release(s2)
+            k += 1
+            continue
+        slot, items, segs, gen_at_submit = inflight.pop(0)
+        try:
+            before = eng.line_pool_capacity()[0]
+            res = eng.collect(slot)
+            after = eng.line_pool_capacity()[0]
+            check_result(eng, res, segs)
+            ovf.append(res.overflow)
+            if after > before and inflight:
+                events["grew_in_flight"] += 1
+            if res.overflow & A.OVF_POOL and gen_at_submit != gen[0]:
+                assert after == before, "a batch launched before a growth or trim grew the pool"
+                events["stale_pool"] += 1
+            track()
+            for i, (c, m, data) in enumerate(items):
+                fold_segment(outs[c], res, i)
+                busy.discard(c)
+                if int(res.segs[i]["flags"]) & A.SEG_DEFERRED:
+                    queue[c].insert(0, data[res.consumed(i):])
+        finally:
+            eng.release(slot)
+    return outs, ovf, events
+
+
+def pool_engine(pages, max_pages, *, flags=A.FLAG_DEFER, conns, batch, n_slots=4, page_bytes=PAGE, **caps):
+    """An SseEngine with a carry slot of SLOT bytes and a line pool of `pages` pages of page_bytes, lines up to 2 MiB, that
+    may grow to max_pages (sse_line_pool_set_growth; 0: no growth). caps: other config fields."""
+    from inference_gateway_b200 import SseEngine
+    return SseEngine(device=0, max_conns=conns, bytes_per_batch=batch, carry_slot_bytes=SLOT, n_slots=n_slots, flags=flags,
+                     **caps, line_pool=dict(pool_pages=pages, page_bytes=page_bytes, max_line_bytes=2 << 20, max_pages=max_pages))
 
 
 def run_pieces(eng, pieces, modes):
