@@ -22,7 +22,9 @@
  * Conventions: every function returns 0 (SSE_OK) or a negative sse_status; nothing throws across the
  * ABI; every buffer handed to the caller is allocated by the library (cudaHostAlloc) and stays valid
  * until sse_release()/sse_destroy(); the library never retains caller pointers.  There is NO CPU
- * fallback: without a CUDA device sse_init fails with SSE_ERR_NO_DEVICE.
+ * fallback: without a CUDA device sse_init fails with SSE_ERR_NO_DEVICE.  Contexts share no state: different contexts, on
+ * the same device or on different ones, may be created, driven and destroyed on different threads at the same time; one
+ * context is driven by one thread at a time.
  */
 #ifndef SSE_GPU_H
 #define SSE_GPU_H
@@ -299,8 +301,9 @@ int  sse_line_pool_capacity(sse_ctx *ctx, uint32_t *pages, uint32_t *max_pages);
  * SSE_ERR_ARG: no context, no SSE_FLAG_DEFER, or min_pool_pages == SSE_NONE. SSE_ERR_NOMEM: the device could not allocate the
  * smaller pool (it stays as it was). */
 int  sse_trim(sse_ctx *ctx, uint32_t min_pool_pages);
-/* Device and pinned bytes the context holds now: every allocation, slots, pool and grown arenas included (and a growth's old
- * pool arrays until they are freed, at the next sse_collect or sse_trim). SSE_ERR_ARG, writing nothing, for a NULL argument. */
+/* Device and pinned bytes the context holds now: every allocation, its decode tables, slots, pool and grown arenas included
+ * (and a growth's old pool arrays until they are freed, at the next sse_collect or sse_trim). SSE_ERR_ARG, writing nothing,
+ * for a NULL argument. */
 int  sse_memory_held(sse_ctx *ctx, uint64_t *device_bytes, uint64_t *pinned_bytes);
 
 /* pipeline: acquire -> fill -> submit -> collect -> release (one slot = one batch in flight) */

@@ -151,21 +151,36 @@ struct WarpTally {
 };
 #endif
 
-// launch wrappers (sse_kernel.cu). The batch wrappers add the kernels they launch to `launches` (sse_launch_count).
-int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count, uint64_t &launches);              // split pipeline, stage 1
-int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches); // split pipeline, stages 2+3
-int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches);  // SSE_FLAG_DEFER: stage 2 again (grown arenas)
+// What a context's kernels are launched with. sse_init_ex fills it once, on the context's own device: kernel attributes and
+// occupancy belong to the device they were read on, so no two contexts share them.
+struct LaunchState {
+    int sm_count = 0;
+    int produce_ctas = 0;            // split pipeline: CTAs per SM of the produce kernel the context's flags select
+    int long_ctas = 0;               // split pipeline: CTAs per SM of the long-line decode kernel
+    const void *tables = nullptr;    // the context's decode tables on the device: ssetab::DfaTables, or FTables for the tile kernel
+    uint64_t launches = 0;           // kernels launched so far (sse_launch_count); the batch wrappers add the kernels they launch
+};
+
+// Launch setup on the current device, for a context whose sse_config.flags are `flags`: the shared-memory attribute and the
+// occupancy of each kernel those flags select.
+int sse_produce_prepare(LaunchState &ls, uint32_t flags);                              // sse_kernel.cu
+int sse_decode_prepare(LaunchState &ls, uint32_t flags);                               // sse_kernel2.cu (with sse_long_prepare)
+int sse_long_prepare(LaunchState &ls);                                                 // sse_long.cu
+namespace ssetab { struct DfaTables; }
+int sse_fused_prepare(const ssetab::DfaTables &D, void *image);  // the tile kernel's FTables, derived from D, into `image`; its attribute
+
+// launch wrappers
+int sse_launch_produce_kernel(const KParams &p, void *stream, LaunchState &ls);       // split pipeline, stage 1
+int sse_launch_decode_finalize(const KParams &p, void *stream, LaunchState &ls);      // split pipeline, stages 2+3
+int sse_launch_decode(const KParams &p, void *stream, LaunchState &ls);               // SSE_FLAG_DEFER: stage 2 again (grown arenas)
+void sse_launch_long_decode(const KParams &p, void *stream, LaunchState &ls);         // split pipeline, stage 2a
+int sse_launch_fused(const KParams &p, void *stream, LaunchState &ls);                // plan kernel + fused tile kernel
 int sse_launch_pool_reset(const KParams &p, uint32_t conn, void *stream);              // line pool: reset one connection (SSE_NONE: all)
 int sse_launch_pool_extend(const KParams &p, uint32_t old_pages, bool grow, void *stream); // line pool: pages [old_pages, pool_pages) free
 // line pool trim: the held pages of p's idle pool repacked into the first `held` pages of new arrays of `pages` pages
 int sse_launch_pool_repack(const KParams &p, uint8_t *pool, uint32_t *stack, uint32_t *next, uint32_t held, uint32_t pages, bool grow,
-                           int sm_count, void *stream);
-namespace ssetab { struct DfaTables; }
+                           const LaunchState &ls, void *stream);
 int sse_build_tables(ssetab::DfaTables &T);                                            // the decode tables of the schema (host)
-int sse_v2_prepare(int device);                                                        // builds + uploads the automaton tables
-int sse_long_prepare(int device);                                                      // long-line decode kernel: occupancy (sse_long.cu)
-void sse_launch_long_decode(const KParams &p, const ssetab::DfaTables *tables, void *stream, int sm_count, int device);   // stage 2a
-int sse_fused_prepare(int device);                                                     // fused pipeline: tables + kernel attributes
-int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches);   // plan kernel + fused tile kernel
-uint32_t sse_fused_max_line(void);
-uint32_t sse_fused_tcache_words(void);                                                 // size of KParams.tcache                                                     // longest carry_slot_bytes the fused kernel supports
+uint32_t sse_fused_max_line(void);                                                     // longest carry_slot_bytes the fused kernel supports
+uint32_t sse_fused_tables_bytes(void);                                                 // size of the tile kernel's FTables
+uint32_t sse_fused_tcache_words(void);                                                 // size of KParams.tcache

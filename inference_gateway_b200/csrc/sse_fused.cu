@@ -1856,16 +1856,10 @@ __global__ void __launch_bounds__(128) sse_plan_kernel(const KParams P) {
     emit(cur_first, cnt);
 }
 
-FTables *g_ftables_dev[16] = { nullptr };
-
 } // namespace
 
-int sse_fused_prepare(int device) {
-    if (device < 0 || device >= 16) return (int)cudaErrorInvalidValue;
-    if (g_ftables_dev[device]) return 0;
-    static DfaTables D;
-    if (sse_build_tables(D) != 0) return (int)cudaErrorInvalidValue;
-    static FTables T;
+int sse_fused_prepare(const DfaTables &D, void *image) {
+    FTables &T = *static_cast<FTables *>(image);
     memset(&T, 0, sizeof T);
     memcpy(T.clssym, D.clssym, sizeof T.clssym);
     memcpy(T.tr, D.tr, NST * NCLS);
@@ -1896,28 +1890,21 @@ int sse_fused_prepare(int device) {
         if (ok) { memcpy(T.hash, used, sizeof used); T.hash_mul = mul; break; }
     }
     if (!T.hash_mul) return (int)cudaErrorInvalidValue;
-    FTables *d = nullptr;
-    cudaError_t e = cudaMalloc((void **)&d, sizeof T);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaMemcpy(d, &T, sizeof T, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(sse_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FSmem));
-    if (e != cudaSuccess) return (int)e;
-    g_ftables_dev[device] = d;
-    return 0;
+    return (int)cudaFuncSetAttribute(sse_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FSmem));
 }
 
 uint32_t sse_fused_max_line(void) { return TILE - 32u; }
+uint32_t sse_fused_tables_bytes(void) { return sizeof(FTables); }
 uint32_t sse_fused_tcache_words(void) { return 8192u; }   // (both engines' layouts fit)
 
-int sse_launch_fused(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches) {
+int sse_launch_fused(const KParams &p, void *stream, LaunchState &ls) {
     const uint32_t groups = (p.n_segs + PLAN_GROUP - 1) / PLAN_GROUP;
     sse_plan_kernel<<<(groups + 3) / 4, 128, 0, (cudaStream_t)stream>>>(p);
-    launches++;
+    ls.launches++;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return (int)e;
     // persistent: the resident CTAs pull tiles by ticket
-    sse_fused_kernel<<<sm_count * F_CTAS_PER_SM, F_THREADS, sizeof(FSmem), (cudaStream_t)stream>>>(p, g_ftables_dev[device]);
-    launches++;
+    sse_fused_kernel<<<ls.sm_count * F_CTAS_PER_SM, F_THREADS, sizeof(FSmem), (cudaStream_t)stream>>>(p, static_cast<const FTables *>(ls.tables));
+    ls.launches++;
     return (int)cudaGetLastError();
 }

@@ -15,6 +15,7 @@
 #include <new>
 #include <vector>
 #include "sse_device.cuh"
+#include "sse_tables.h"
 
 static_assert(sizeof(sse_counters) == 8 + CN_COUNT * sizeof(uint64_t) && offsetof(sse_counters, p_segments) == 8 &&
               offsetof(sse_counters, d_items) == 8 + 8 * CN_D_ITEMS && offsetof(sse_counters, c_unquote) == 8 + 8 * CN_C_UNQUOTE,
@@ -95,11 +96,12 @@ static inline uint32_t in_base_of(const sse_config &cfg) { return (cfg.out_arena
 
 struct sse_ctx {
     int device = 0;
-    int sm_count = 0;
+    LaunchState launch;                  // set up by sse_init_ex on `device`
     sse_config cfg{};
+    Buf<uint8_t> tables;                 // the engine's decode tables (launch.tables)
     Buf<ConnState> conns;
     Buf<uint8_t> carry;
-    Buf<uint32_t> tcache;                // fused kernel: skeleton templates kept between launches
+    Buf<uint32_t> tcache;                // SSE_FLAG_TEMPLATES: skeleton templates kept between launches
     sse_line_pool pool{};                // pool_pages == 0: no line pool
     PoolArrays pool_arrays;
     Buf<PoolHdr> pool_hdr;
@@ -112,7 +114,6 @@ struct sse_ctx {
     cudaStream_t ctl_stream = nullptr;
     cudaEvent_t last_kernel = nullptr;   // completion of the most recently launched kernel (or of sse_init_ex)
     std::vector<Slot> slots;
-    uint64_t launches = 0;
 };
 
 namespace {
@@ -167,7 +168,8 @@ template <class F> void slot_buffers(Slot &s, const sse_config &cfg, F f) {
     both(s.segs, cfg.max_segs); both(s.frames, cfg.max_frames); both(s.tcs, cfg.max_tcs); both(s.usages, cfg.max_usages);
     both(s.text, cfg.text_arena_bytes); both(s.runs, cfg.max_runs); both(s.segres, cfg.max_segs); both(s.ctr, 1);
     if (cfg.flags & SSE_FLAG_COUNTERS) both(s.cnt, CN_COUNT);
-    f(s.items, cfg.max_recs); f(s.segterm, cfg.max_segs); f(s.items2, cfg.max_recs); f(s.tiles, (size_t)cfg.max_segs + 64);
+    if (cfg.flags & SSE_FLAG_KERNEL_FUSED) f(s.tiles, (size_t)cfg.max_segs + 64);
+    else { f(s.items, cfg.max_recs); f(s.segterm, cfg.max_segs); f(s.items2, cfg.max_recs); }
 }
 
 void free_slot(sse_ctx *c, Slot &s) {
@@ -200,7 +202,7 @@ KParams make_params(sse_ctx *c, Slot &s, uint32_t n_segs) {
     p.items = s.items.p; p.cap_items = c->cfg.max_recs; p.seg_term = s.segterm.p;
     p.items_sorted = s.items2.p; p.flags = c->cfg.flags;
     p.tiles = s.tiles.p; p.cap_tiles = c->cfg.max_segs + 64;
-    p.tcache = (c->cfg.flags & SSE_FLAG_TEMPLATES) ? c->tcache.p : nullptr;
+    p.tcache = c->tcache.p;
     p.max_line = c->pool.pool_pages ? c->pool.max_line_bytes : c->cfg.carry_slot_bytes;
     p.long_line = (SSE_LONG_LINE && !(c->cfg.flags & SSE_FLAG_KERNEL_FUSED) && p.max_line >= SSE_LONG_LINE) ? SSE_LONG_LINE : 0u;
     p.cnt = s.cnt.d.p;
@@ -233,10 +235,10 @@ int do_launch(sse_ctx *c, Slot &s, uint32_t n_segs, cudaStream_t st) {
         KParams p = make_params(c, s, n_segs);
         int e;
         if (c->cfg.flags & SSE_FLAG_KERNEL_FUSED)   // plan + single-pass tile kernel
-            e = sse_launch_fused(p, (void *)st, c->sm_count, c->device, c->launches);
+            e = sse_launch_fused(p, (void *)st, c->launch);
         else {   // default: produce -> sort -> decode (templates / automaton) -> finalize
-            e = sse_launch_produce_kernel(p, (void *)st, c->sm_count, c->launches);
-            if (e == 0) e = sse_launch_decode_finalize(p, (void *)st, c->sm_count, c->device, c->launches);
+            e = sse_launch_produce_kernel(p, (void *)st, c->launch);
+            if (e == 0) e = sse_launch_decode_finalize(p, (void *)st, c->launch);
         }
         if (e != 0) { cu_ok((cudaError_t)e, "stream kernel launch"); return SSE_ERR_CUDA; }
     }
@@ -322,7 +324,7 @@ int redecode(sse_ctx *c, Slot &s, Counters &k, cudaStream_t st, uint32_t &grown)
             s.decode_passes++;
         }
         CU(cudaStreamWaitEvent(st, c->last_kernel, 0));
-        const int e = sse_launch_decode(make_params(c, s, s.n_segs), (void *)st, c->sm_count, c->device, c->launches);
+        const int e = sse_launch_decode(make_params(c, s, s.n_segs), (void *)st, c->launch);
         if (e != 0) { cu_ok((cudaError_t)e, "decode kernel launch"); return SSE_ERR_CUDA; }
         CU(cudaEventRecord(c->last_kernel, st));
         CU(cudaMemcpyAsync(s.ctr.h.p, s.ctr.d.p, CTR_HEAD, cudaMemcpyDeviceToHost, st));
@@ -444,13 +446,34 @@ int trim_pool(sse_ctx *c, uint32_t min_pages) {
     PoolArrays small;
     if (!pool_alloc(c, small, want)) return SSE_ERR_NOMEM;
     const int e = sse_launch_pool_repack(pool_params(c), small.pages.p, small.stack.p, small.next.p, held, want, want < c->pool_max,
-                                         c->sm_count, st);
+                                         c->launch, st);
     if (!cu_ok((cudaError_t)e, "pool repack kernels")) { pool_free(c, small); return SSE_ERR_CUDA; }
     CU(cudaEventRecord(c->last_kernel, st));
     pool_free(c, c->pool_arrays);
     c->pool_arrays = small; c->pool.pool_pages = want;
     c->pool_gen++;            // a batch launched before the trim reports its lack against the old pool: it does not grow this one
     return SSE_OK;
+}
+
+// sse_init_ex: the launch state of the engine the context's flags select, on the context's device. The decode tables are built
+// on the host once and uploaded into the context's own buffer on ctl_stream; the tile kernel's FTables are derived from them.
+bool prepare_launch(sse_ctx *c, int sm_count) {
+    LaunchState &L = c->launch;
+    L.sm_count = sm_count;
+    ssetab::DfaTables D;
+    int e = sse_build_tables(D) == 0 ? 0 : (int)cudaErrorInvalidValue;
+    std::vector<uint8_t> image;
+    if (c->cfg.flags & SSE_FLAG_KERNEL_FUSED) {
+        image.resize(sse_fused_tables_bytes());
+        if (e == 0) e = sse_fused_prepare(D, image.data());
+    } else {
+        image.assign((const uint8_t *)&D, (const uint8_t *)(&D + 1));
+        if (e == 0) e = sse_produce_prepare(L, c->cfg.flags);
+        if (e == 0) e = sse_decode_prepare(L, c->cfg.flags);
+    }
+    if (!cu_ok((cudaError_t)e, "kernel setup") || !buf_alloc(c, c->tables, image.size())) return false;
+    L.tables = c->tables.p;
+    return cu_ok(cudaMemcpyAsync(c->tables.p, image.data(), image.size(), cudaMemcpyHostToDevice, c->ctl_stream), "cudaMemcpyAsync");
 }
 
 } // namespace
@@ -558,29 +581,23 @@ int sse_init_ex(int device, const sse_config *cfg_in, const sse_line_pool *pool_
         return SSE_ERR_NO_DEVICE;
     }
     CU(cudaSetDevice(device));
+    if ((cfg->flags & SSE_FLAG_KERNEL_FUSED) && cfg->carry_slot_bytes > sse_fused_max_line()) return SSE_ERR_ARG;
     sse_ctx *c = new (std::nothrow) sse_ctx();
     if (!c) return SSE_ERR_NOMEM;
     c->device = device; c->cfg = *cfg; c->pool = pool;
     cudaDeviceProp prop;
-    if (!cu_ok(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties")) { delete c; return SSE_ERR_CUDA; }
-    c->sm_count = prop.multiProcessorCount;
-    if (cfg->flags & SSE_FLAG_KERNEL_FUSED) {
-        if (cfg->carry_slot_bytes > sse_fused_max_line()) { delete c; return SSE_ERR_ARG; }
-        int e2 = sse_fused_prepare(device);
-        if (e2 != 0) { cu_ok((cudaError_t)e2, "sse_fused_prepare"); delete c; return SSE_ERR_CUDA; }
-    } else {
-        int e2 = sse_v2_prepare(device);
-        if (e2 != 0) { cu_ok((cudaError_t)e2, "sse_v2_prepare"); delete c; return SSE_ERR_CUDA; }
-    }
-    bool ok = true;
+    bool ok = cu_ok(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
     ok = ok && cu_ok(cudaStreamCreateWithFlags(&c->ctl_stream, cudaStreamNonBlocking), "cudaStreamCreate");
     ok = ok && cu_ok(cudaEventCreateWithFlags(&c->last_kernel, cudaEventDisableTiming), "cudaEventCreate");
-    // every wait on last_kernel has an event to wait for
+    ok = ok && prepare_launch(c, prop.multiProcessorCount);
+    // every wait on last_kernel has an event to wait for, and every kernel is ordered after the upload of the decode tables
     ok = ok && cu_ok(cudaEventRecord(c->last_kernel, c->ctl_stream), "cudaEventRecord");
     ok = ok && buf_alloc(c, c->conns, cfg->max_conns) && buf_alloc(c, c->carry, (size_t)cfg->max_conns * cfg->carry_slot_bytes);
     ok = ok && cu_ok(cudaMemset(c->conns.p, 0, (size_t)cfg->max_conns * sizeof(ConnState)), "cudaMemset");
-    ok = ok && buf_alloc(c, c->tcache, sse_fused_tcache_words());
-    ok = ok && cu_ok(cudaMemset(c->tcache.p, 0, (size_t)sse_fused_tcache_words() * sizeof(uint32_t)), "cudaMemset");
+    if (ok && (cfg->flags & SSE_FLAG_TEMPLATES)) {
+        ok = buf_alloc(c, c->tcache, sse_fused_tcache_words());
+        ok = ok && cu_ok(cudaMemset(c->tcache.p, 0, (size_t)sse_fused_tcache_words() * sizeof(uint32_t)), "cudaMemset");
+    }
     if (ok && pool.pool_pages) {
         ok = pool_alloc(c, c->pool_arrays, pool.pool_pages) && buf_alloc(c, c->pool_hdr, 1) && buf_alloc(c, c->pool_chain, cfg->max_conns) &&
              buf_alloc(c, c->h_pool_hdr, 1);
@@ -608,7 +625,7 @@ void sse_destroy(sse_ctx *c) {
     cudaDeviceSynchronize();
     free_retired(c, true);
     for (auto &s : c->slots) free_slot(c, s);
-    buf_free(c, c->conns); buf_free(c, c->carry); buf_free(c, c->tcache);
+    buf_free(c, c->tables); buf_free(c, c->conns); buf_free(c, c->carry); buf_free(c, c->tcache);
     pool_free(c, c->pool_arrays); buf_free(c, c->pool_hdr); buf_free(c, c->pool_chain); buf_free(c, c->h_pool_hdr);
     if (c->ctl_stream) cudaStreamDestroy(c->ctl_stream);
     if (c->last_kernel) cudaEventDestroy(c->last_kernel);
@@ -802,7 +819,7 @@ int sse_counters_read(sse_ctx *c, int slot, sse_counters *out) {
 
 int sse_launch_count(sse_ctx *c, uint64_t *kernel_launches) {
     if (!c || !kernel_launches) return SSE_ERR_ARG;
-    *kernel_launches = c->launches;
+    *kernel_launches = c->launch.launches;
     return SSE_OK;
 }
 

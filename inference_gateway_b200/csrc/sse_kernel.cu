@@ -469,31 +469,29 @@ sse_stream_kernel(const __grid_constant__ KParams P) {
 
 } // namespace
 
-template <bool DEFER, bool CNT>
-static int launch_stream_kernel(const KParams &p, void *stream, int sm_count, uint64_t &launches) {
-    static bool attr_set = false;
-    static int ctas_per_sm = 0;
-    const size_t smem = sizeof(CtaSmem);
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(sse_stream_kernel<DEFER, CNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return (int)e;
-        int n = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sse_stream_kernel<DEFER, CNT>, WARPS_PER_CTA * 32, smem);
-        if (e != cudaSuccess) return (int)e;
-        ctas_per_sm = n > 0 ? n : 1;
-        attr_set = true;
-    }
-    int grid = sm_count * ctas_per_sm;   // persistent: one resident wave, warps pull segments by ticket
-    int need = (int)((p.n_segs + WARPS_PER_CTA - 1) / WARPS_PER_CTA);
-    if (need < grid) grid = need > 0 ? need : 1;
-    sse_stream_kernel<DEFER, CNT><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(p);
-    launches++;
-    return (int)cudaGetLastError();
+// the produce kernel SSE_FLAG_DEFER and SSE_FLAG_COUNTERS select
+using ProduceKernel = void (*)(KParams);
+static ProduceKernel produce_kernel(bool defer, bool cnt) {
+    if (cnt) return defer ? sse_stream_kernel<true, true> : sse_stream_kernel<false, true>;
+    return defer ? sse_stream_kernel<true, false> : sse_stream_kernel<false, false>;
 }
 
-int sse_launch_produce_kernel(const KParams &p, void *stream, int sm_count, uint64_t &launches) {
-    if (p.cnt) return (p.flags & SSE_FLAG_DEFER) ? launch_stream_kernel<true, true>(p, stream, sm_count, launches)
-                                                 : launch_stream_kernel<false, true>(p, stream, sm_count, launches);
-    return (p.flags & SSE_FLAG_DEFER) ? launch_stream_kernel<true, false>(p, stream, sm_count, launches)
-                                      : launch_stream_kernel<false, false>(p, stream, sm_count, launches);
+int sse_produce_prepare(LaunchState &ls, uint32_t flags) {
+    const ProduceKernel k = produce_kernel(flags & SSE_FLAG_DEFER, flags & SSE_FLAG_COUNTERS);
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem));
+    if (e != cudaSuccess) return (int)e;
+    int n = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, WARPS_PER_CTA * 32, sizeof(CtaSmem));
+    if (e != cudaSuccess) return (int)e;
+    ls.produce_ctas = n > 0 ? n : 1;
+    return 0;
+}
+
+int sse_launch_produce_kernel(const KParams &p, void *stream, LaunchState &ls) {
+    int grid = ls.sm_count * ls.produce_ctas;   // persistent: one resident wave, warps pull segments by ticket
+    int need = (int)((p.n_segs + WARPS_PER_CTA - 1) / WARPS_PER_CTA);
+    if (need < grid) grid = need > 0 ? need : 1;
+    produce_kernel(p.flags & SSE_FLAG_DEFER, p.cnt)<<<grid, WARPS_PER_CTA * 32, sizeof(CtaSmem), (cudaStream_t)stream>>>(p);
+    ls.launches++;
+    return (int)cudaGetLastError();
 }

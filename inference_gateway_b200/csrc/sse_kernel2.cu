@@ -701,8 +701,6 @@ __global__ void __launch_bounds__(256) sse_pool_repack_copy_kernel(const uint4 *
     }
 }
 
-DfaTables *g_tables_dev[16] = { nullptr };
-
 } // namespace
 
 int sse_build_tables(ssetab::DfaTables &T) {
@@ -717,70 +715,52 @@ int sse_build_tables(ssetab::DfaTables &T) {
             n++;
         }
     // finish_reason values with a code of their own (common_types.go:33-39); any other non-empty value is SSE_FIN_OTHER
-    static const char *const fin_names[] = { "stop", "tool_calls", "length", "content_filter", "function_call" };
-    static const uint8_t fin_vals[] = { SSE_FIN_STOP, SSE_FIN_TOOL_CALLS, SSE_FIN_LENGTH, SSE_FIN_CONTENT_FILTER, SSE_FIN_FUNCTION_CALL };
+    const char *const fin_names[] = { "stop", "tool_calls", "length", "content_filter", "function_call" };
+    const uint8_t fin_vals[] = { SSE_FIN_STOP, SSE_FIN_TOOL_CALLS, SSE_FIN_LENGTH, SSE_FIN_CONTENT_FILTER, SSE_FIN_FUNCTION_CALL };
     return ssetab::build_tables(T, fs, n, fin_names, fin_vals, 5);
 }
 
-int sse_v2_prepare(int device) {
-    if (device < 0 || device >= 16) return (int)cudaErrorInvalidValue;
-    if (g_tables_dev[device]) return 0;
-    static ssetab::DfaTables T;
-    if (sse_build_tables(T) != 0) return (int)cudaErrorInvalidValue;
-    DfaTables *d = nullptr;
-    cudaError_t e = cudaMalloc((void **)&d, sizeof T);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaMemcpy(d, &T, sizeof T, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(sse_decode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(sse_decode_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(sse_decode_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(sse_decode_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
-    if (e != cudaSuccess) return (int)e;
-    const int el = sse_long_prepare(device);
-    if (el != 0) return el;
-    g_tables_dev[device] = d;
-    return 0;
+// the decode kernel SSE_FLAG_TEMPLATES (KParams.tcache) and SSE_FLAG_COUNTERS (KParams.cnt) select
+using DecodeKernel = void (*)(KParams, const DfaTables *);
+static DecodeKernel decode_kernel(bool tcache, bool cnt) {
+    if (cnt) return tcache ? sse_decode_kernel<true, true> : sse_decode_kernel<false, true>;
+    return tcache ? sse_decode_kernel<true, false> : sse_decode_kernel<false, false>;
 }
 
-// the decode kernels the context's flags select: templates (KParams.tcache) and counters (KParams.cnt). The long-line kernel
-// goes first, alone: the lane decoder fills every SM, so the two could not run side by side.
-static void launch_decode_kernel(const KParams &p, cudaStream_t st, int sm_count, int device, uint64_t &launches) {
-    const DfaTables *t = g_tables_dev[device];
-    if (p.long_line) { sse_launch_long_decode(p, t, (void *)st, sm_count, device); launches++; }
-    if (p.cnt) {
-        if (p.tcache) sse_decode_kernel<true, true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
-        else sse_decode_kernel<false, true><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
-    } else {
-        if (p.tcache) sse_decode_kernel<true, false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
-        else sse_decode_kernel<false, false><<<sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, t);
-    }
-    launches++;
+int sse_decode_prepare(LaunchState &ls, uint32_t flags) {
+    const cudaError_t e = cudaFuncSetAttribute(decode_kernel(flags & SSE_FLAG_TEMPLATES, flags & SSE_FLAG_COUNTERS),
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CtaSmem3));
+    if (e != cudaSuccess) return (int)e;
+    return sse_long_prepare(ls);
 }
 
-int sse_launch_decode_finalize(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches) {
-    sse_bucket_hist_kernel<<<sm_count * 2, 512, 0, (cudaStream_t)stream>>>(p);
+// The long-line kernel goes first, alone: the lane decoder fills every SM, so the two could not run side by side.
+static void launch_decode_kernel(const KParams &p, cudaStream_t st, LaunchState &ls) {
+    if (p.long_line) sse_launch_long_decode(p, (void *)st, ls);
+    decode_kernel(p.tcache, p.cnt)<<<ls.sm_count, V3_WARPS * 32, sizeof(CtaSmem3), st>>>(p, static_cast<const DfaTables *>(ls.tables));
+    ls.launches++;
+}
+
+int sse_launch_decode_finalize(const KParams &p, void *stream, LaunchState &ls) {
+    sse_bucket_hist_kernel<<<ls.sm_count * 2, 512, 0, (cudaStream_t)stream>>>(p);
     sse_bucket_scan_kernel<<<1, SCAN_TPB, 0, (cudaStream_t)stream>>>(p);
-    sse_bucket_scatter_kernel<<<sm_count * 2, SCATTER_TPB, 0, (cudaStream_t)stream>>>(p);
-    launches += 3;
-    launch_decode_kernel(p, (cudaStream_t)stream, sm_count, device, launches);
+    sse_bucket_scatter_kernel<<<ls.sm_count * 2, SCATTER_TPB, 0, (cudaStream_t)stream>>>(p);
+    ls.launches += 3;
+    launch_decode_kernel(p, (cudaStream_t)stream, ls);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return (int)e;
     const int tpb = 256;
     if (p.cnt) sse_finalize_kernel<true><<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
     else sse_finalize_kernel<false><<<(p.n_segs + tpb - 1) / tpb, tpb, 0, (cudaStream_t)stream>>>(p);
-    launches++;
+    ls.launches++;
     return (int)cudaGetLastError();
 }
 
 // SSE_FLAG_DEFER, after the tool-call / usage / text arenas of a batch grew: the decode stage again over the items the sort left
 // in items_sorted (the caller has reset the decode counters). Records are rewritten whole, so a second pass gives the records a
 // single pass with large enough arenas gives.
-int sse_launch_decode(const KParams &p, void *stream, int sm_count, int device, uint64_t &launches) {
-    launch_decode_kernel(p, (cudaStream_t)stream, sm_count, device, launches);
+int sse_launch_decode(const KParams &p, void *stream, LaunchState &ls) {
+    launch_decode_kernel(p, (cudaStream_t)stream, ls);
     return (int)cudaGetLastError();
 }
 
@@ -797,10 +777,10 @@ int sse_launch_pool_extend(const KParams &p, uint32_t old_pages, bool grow, void
 }
 
 int sse_launch_pool_repack(const KParams &p, uint8_t *pool, uint32_t *stack, uint32_t *next, uint32_t held, uint32_t pages, bool grow,
-                           int sm_count, void *stream) {
+                           const LaunchState &ls, void *stream) {
     sse_pool_repack_chains_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(p, stack, next, held, pages, grow ? 1u : 0u);
     if (held) {
-        const uint32_t grid = held < 8u * (uint32_t)sm_count ? held : 8u * (uint32_t)sm_count;   // 8 blocks of 256 fill an SM
+        const uint32_t grid = held < 8u * (uint32_t)ls.sm_count ? held : 8u * (uint32_t)ls.sm_count;   // 8 blocks of 256 fill an SM
         sse_pool_repack_copy_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint4 *)p.pool, (uint4 *)pool, stack + (pages - held),
                                                                             held, p.page_bytes / 16u);
     }

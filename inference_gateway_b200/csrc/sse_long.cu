@@ -272,22 +272,22 @@ sse_long_decode_kernel(const __grid_constant__ KParams P, const DfaTables *__res
     }
 }
 
-int g_long_ctas[16] = { 0 };     // CTAs per SM of the long-line kernel, per device
-
 } // namespace
 
-int sse_long_prepare(int device) {
-    if (device < 0 || device >= 16) return (int)cudaErrorInvalidValue;
+// The counting instantiation has the lower occupancy of the two; its CTAs per SM size the grid of both, which are then all resident.
+int sse_long_prepare(LaunchState &ls) {
     int ctas = 0;
     const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, sse_long_decode_kernel<true>, LONG_WARPS * 32, 0);
     if (e != cudaSuccess) return (int)e;
-    g_long_ctas[device] = ctas > 0 ? ctas : 1;
+    ls.long_ctas = ctas > 0 ? ctas : 1;
     return 0;
 }
 
 // Launched before the lane decoder, alone on the stream: the lane decoder fills every SM, so the two could not run side by side.
-void sse_launch_long_decode(const KParams &p, const ssetab::DfaTables *tables, void *stream, int sm_count, int device) {
-    const int grid = sm_count * g_long_ctas[device];
+void sse_launch_long_decode(const KParams &p, void *stream, LaunchState &ls) {
+    const int grid = ls.sm_count * ls.long_ctas;
+    const DfaTables *tables = static_cast<const DfaTables *>(ls.tables);
     if (p.cnt) sse_long_decode_kernel<true><<<grid, LONG_WARPS * 32, 0, (cudaStream_t)stream>>>(p, tables);
     else sse_long_decode_kernel<false><<<grid, LONG_WARPS * 32, 0, (cudaStream_t)stream>>>(p, tables);
+    ls.launches++;
 }
